@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- attention-forward TFLOP/s on B200 (the one hot path), per the driver contract.
+"""bench.py -- attention-forward TFLOP/s on H100 (the one hot path).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
-Workload (config.workload): BASELINE.json configs[4], the configuration the metric's "1/2/4/8 B200"
-clause is quoted on -- B=64 H=32 S=4096 D=128 bf16 causal, sharded over (B*H).  It fits one GPU
+Workload (config.workload): BASELINE.json configs[4], the configuration the metric's "1/2/4/8 H100"
+clause is quoted on -- B=64 H=32 S=4096 D=128 bf16 causal, sharded over (B*H).  It fits one 80 GB GPU
 (Q,K,V,O = 8.6 GB), so N=1 runs ALL of it and N>1 splits the batch: total work fixed => "strong" scaling.
-A step = one forward pass over the whole job: every rank runs the sm_100a kernel on its B/N batches and,
+A step = one forward pass over the whole job: every rank runs the sm_90a kernel on its B/N batches and,
 for N>1, the O shards are all-gathered (NCCL) so every rank ends the step holding the full O.
 
 Printed JSON (rank 0, one line):
@@ -17,11 +17,13 @@ Printed JSON (rank 0, one line):
   e2e          the same metric through the C ABI host-buffer call tfa_fwd_host(): pinned HOST q/k/v in,
                HOST out/lse back, copies inside the timed region.
   roofline     tensor-core bound: achieved = F_per_launch / mean kernel time (CUDA events on the launch
-               stream, measured live here), peak = MEASURED_PEAKS.json bf16_tflops (burst).
+               stream, measured live here), peak = MEASURED_PEAKS.json bf16_tflops when present, else the H100 SXM
+               data sheet's dense BF16 rate (989 TFLOP/s at 700 W).
   cpu_baseline the reference's own C++ CPU attention (oracle/_ref, compiled unmodified) timed on this box's
                host cores on a bounded head-sample of the same workload (rank 0, N=1 only).
   configs      BASELINE.json configs[1..3] timed the same way (N=1 only), for the headline table.
 `--impl reference` times only that CPU path (all host threads) on the same config/metric/unit.
+`--dump-outputs DIR` writes, after the timed steps, what the last step computed (rank 0, see dump_outputs()).
 """
 from __future__ import annotations
 
@@ -46,8 +48,9 @@ EXTRA_CONFIGS = {
     "cfg3: B=4 H=32 S=4096 D=128 bf16 causal": (4, 32, 4096, 128, True),
     "cfg4: B=1 H=32 S=16384 D=128 bf16 causal": (1, 32, 16384, 128, True),
 }
-FALLBACK_PEAK_TFLOPS = 1590.0   # /opt/skills/guides/B200_PROFILING.md fallback
-METRIC = "attention TFLOPs/s (bf16, seqlen\u00d7head_dim) at 1/2/4/8 B200 vs roofline"   # BASELINE.json's metric, verbatim
+FALLBACK_PEAK_TFLOPS = 989.0    # H100 SXM data sheet, dense BF16, 700 W: a bound, not a measured rate
+FALLBACK_HBM_GBS = 3350.0       # H100 SXM data sheet, HBM3
+METRIC = "attention TFLOPs/s (bf16, seqlen\u00d7head_dim) at 1/2/4/8 H100 vs roofline"   # BASELINE.json's metric, verbatim
 try:
     METRIC = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "BASELINE.json")))["metric"]
 except Exception:  # noqa: BLE001  (file absent: keep the literal above)
@@ -70,7 +73,7 @@ def load_peaks():
             return float(d["bf16_tflops"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured"
         except Exception:  # noqa: BLE001
             pass
-    return FALLBACK_PEAK_TFLOPS, 1400.0, "fallback"
+    return FALLBACK_PEAK_TFLOPS, FALLBACK_PEAK_TFLOPS, "data sheet"
 
 
 class ClockSampler:
@@ -191,7 +194,7 @@ def run_reference_arm(args):
                    "step": f"bounded sample: {heads} of {W['B'] * W['H']} (batch*head) problems per step"},
         "cpu_baseline": {"value": val, "unit": "TFLOP/s", "cores": cores, "kind": kind,
                          "sample": f"{heads} heads x S{W['S']} x D{W['D']} causal fp32 per step, "
-                                   f"/root/reference/flash_attention_c flash_attn (OpenMP, all host threads)"},
+                                   f"the reference's flash_attention_c flash_attn (OpenMP, all host threads)"},
         "e2e": {"value": val, "unit": "TFLOP/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
     }
@@ -376,6 +379,8 @@ def run_ours(args):
         barrier()
     launches = tfa.launch_count() - n0
     t_total = e0.elapsed_time(e1) * 1e-3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, fused.buf if fused is not None else (o_full if world > 1 else out), lse)
     if world > 1:
         tt = torch.tensor([t_total], device=dev)
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -394,15 +399,15 @@ def run_ours(args):
     compute_only_value = flops_effective(B, H, S, D) / (k_mean * launches_per_step) / 1e12   # all ranks, kernels only
 
     # fused compute+collective kernel: target = slower of (FLOPs / tensor peak) and (bytes that must leave this GPU
-    # over NVLink / measured 770 GB/s per direction), per /opt/skills/guides/B200_PROFILING.md
+    # over NVLink / 450 GB/s per direction, the H100 SXM data sheet's NVLink rate)
     fused_roofline = None
     if fused is not None:
         nv_bytes = (world - 1) * Bl * H * S * D * 2
         t_flops = F_launch / (peak * 1e12)
-        t_link = nv_bytes / 770e9
+        t_link = nv_bytes / 450e9
         target = max(t_flops, t_link)
         fused_roofline = {"kernel": kernel_main + " + peer stores (tfa_fwd_multi)", "nvlink_bytes_out_per_launch": nv_bytes,
-                          "nvlink_peak_GBps": 770.0, "t_tensor_ms": t_flops * 1e3, "t_nvlink_ms": t_link * 1e3,
+                          "nvlink_peak_GBps": 450.0, "t_tensor_ms": t_flops * 1e3, "t_nvlink_ms": t_link * 1e3,
                           "target_ms": target * 1e3, "achieved_ms": k_mean * 1e3, "frac": target / k_mean,
                           "bound": "nvlink" if t_link > t_flops else "tensor"}
 
@@ -511,7 +516,7 @@ def run_ours(args):
             try:
                 hbm_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
             except Exception:  # noqa: BLE001
-                hbm_peak = 6500.0          # profiling recipe fallback
+                hbm_peak = FALLBACK_HBM_GBS
 
             def time_general(qq, kk, vv, causal_, ns):
                 sc = 1.0 / math.sqrt(qq.shape[-1])
@@ -578,10 +583,6 @@ def run_ours(args):
         except Exception as e:  # noqa: BLE001
             cpu_baseline = {"error": repr(e)}
 
-    comparators = None
-    if world == 1 and not args.no_extras and not args.no_comparators:
-        comparators = run_comparators()
-
     # denominator: the measured BURST cuBLAS figure.  The sustained figure only applies to a seconds-long region whose
     # sampled SM clock actually sat well below max (VERDICT r01 / ADVICE r01: a 0.1-0.2 s region at ~1.9 GHz is burst).
     clocks = clk.summary()
@@ -591,7 +592,6 @@ def run_ours(args):
     roof_peak = peak_sus if sustained_applies else peak
     roof_peak_name = ("bf16_tflops_sustained (%.1f s region, median SM clock %.0f MHz < 0.8 max)" % (region_s, clocks["sm_mhz"])
                       if sustained_applies else "bf16_tflops (burst)")
-    traffic, traffic_src = profiled_traffic(Bl * H / launches_per_step)
     line = {
         "metric": METRIC, "value": value, "unit": "TFLOP/s", "n_gpus": world, "steps": args.steps,
         "warmup": max(args.warmup, 3), "ms_per_step": t_step * 1e3, "higher_is_better": True, "scaling": "strong",
@@ -601,7 +601,7 @@ def run_ours(args):
                        " + O gathered by fused NVLink peer stores in the kernel epilogue (no collective)" if fused is not None
                        else f" + NCCL all-gather of O ({n_chunks} chunk(s))")),
                    "exchange": exchange, "exchange_check": exchange_check,
-                   "flops": "2*B*H*S^2*D", "l2": "inputs (3 x %.0f MB per rank) larger than the 126 MB L2" % (q_bytes(Bl, H, S, D) / 1e6)},
+                   "flops": "2*B*H*S^2*D", "l2": "inputs (3 x %.0f MB per rank) larger than the 50 MB L2" % (q_bytes(Bl, H, S, D) / 1e6)},
         "clocks": clocks,
         "e2e": e2e,
         "gpu_launches": int(launches),
@@ -612,14 +612,13 @@ def run_ours(args):
                      "kernel": kernel_main, "kernel_ms_mean": k_mean * 1e3, "kernel_ms_min": k_min * 1e3,
                      "timing": "CUDA events around each launch inside the timed region",
                      "flops_per_launch": F_launch, "launches_per_step_per_rank": launches_per_step,
-                     "traffic": traffic, "traffic_source": traffic_src,
+                     "traffic": None, "traffic_source": "not measured (no hardware counters on this path)",
                      "algorithmic_bytes_per_launch": (4 * S * D * 2 + 4 * S) * (Bl * H) / launches_per_step},
         "fused_roofline": fused_roofline,
         "compute_only": {"value": compute_only_value, "unit": "TFLOP/s", "note": "kernel only, no all-gather"},
         "cpu_baseline": cpu_baseline,
         "parity": parity,
         "configs": configs,
-        "comparators": comparators,
         "next_rows": next_rows,
     }
     emit(line)
@@ -641,69 +640,22 @@ def kernel_name(tfa):
         v = int(tfa.lib().tfa_internal_last_variant())
     except Exception:  # noqa: BLE001
         v = 0
-    return {0: "fa_fwd_sm100_kernel (one CTA per work item)",
-            4: "fa_fwd_sm100_persist_kernel (persistent, TMA-store epilogue)"}.get(v, str(v))
+    return {0: "fa_fwd_sm90_kernel (one CTA per work item)",
+            4: "fa_fwd_sm90_kernel (persistent: one CTA per SM)"}.get(v, str(v))
 
-
-
-def profiled_traffic(heads_per_launch):
-    """roofline.traffic: dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full`
-    capture of the SAME kernel source (profiles/traffic.json records the capture's commit and the digest of the kernel
-    sources it was taken from); null when the kernel sources changed since -- a stale constant is worse than none."""
-    try:
-        rec = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        import hashlib
-        h = hashlib.sha256()
-        for f in rec["sources"]:
-            h.update(open(os.path.join(ROOT, f), "rb").read())
-        if h.hexdigest() != rec["sources_sha256"]:
-            return None, f"profiles/traffic.json is from commit {rec.get('commit')} and the kernel sources changed since: no traffic claim"
-        return rec["dram_bytes_per_head"] * heads_per_launch, (
-            f"{rec['capture']} (commit {rec.get('commit')}): {rec['dram_bytes_per_head'] / 1e6:.3f} MB per (batch*head) "
-            f"for {rec['algorithmic_bytes_per_head'] / 1e6:.3f} MB algorithmic, scaled by heads per launch")
-    except Exception as e:  # noqa: BLE001
-        return None, f"no profiles/traffic.json ({e!r})"
-
-
-def run_comparators(timeout_s=420):
-    """Library / reference-kernel comparators on cfg2-4 in a SUBPROCESS (scripts/comparators.py)."""
-    import subprocess
-    try:
-        env = dict(os.environ, CMP_BUDGET_S="300")
-        p = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "comparators.py")], capture_output=True, text=True,
-                           timeout=timeout_s, env=env)
-        for ln in p.stdout.splitlines():
-            if ln.startswith("CMP "):
-                return json.loads(ln[4:])
-        return {"error": "no result", "rc": p.returncode, "stderr_tail": p.stderr[-400:]}
-    except Exception as e:  # noqa: BLE001
-        return {"error": repr(e)[:300]}
 
 
 def time_naive_python_cfg1():
-    """BASELINE config 1 (B1 H2 S128 D64 fp32, no scale, no mask) through the reference's naive-Python path
-    tiny_flash_attn.flash_attn_v2_multihead (flash_attention_py/tiny_flash_attn.py:137-196) when its unmodified copy
-    travelled with baseline/_ref (kind "reference"); else the oracle's restatement of the same block algorithm
-    (kind "port")."""
+    """BASELINE config 1 (B1 H2 S128 D64 fp32, no scale, no mask) through the oracle's restatement of the reference's
+    naive-Python block algorithm tiny_flash_attn.flash_attn_v2_multihead (flash_attention_py/tiny_flash_attn.py:137-196)."""
     import torch
     B_, H_, S_, D_ = 1, 2, 128, 64
     g = torch.Generator().manual_seed(20)
     q, k, v = (torch.empty(B_, H_, S_, D_).normal_(0, 0.5, generator=g) for _ in range(3))
     F = flops_effective(B_, H_, S_, D_)
-    ref_dir = os.path.join(ROOT, "baseline", "_ref", "drivers", "py")
-    if os.path.exists(os.path.join(ref_dir, "tiny_flash_attn.py")):
-        sys.path.insert(0, ref_dir)
-        try:
-            import tiny_flash_attn as tfa_py
-            torch.set_num_threads(1)
-            fn = lambda: tfa_py.flash_attn_v2_multihead(q, k, v, device="cpu", BLOCK_M=4)
-            kind, what = "reference", "tiny_flash_attn.flash_attn_v2_multihead(device='cpu', BLOCK_M=4), unmodified copy"
-        finally:
-            sys.path.remove(ref_dir)
-    else:
-        from oracle import oracle as orc
-        fn = lambda: orc.flash_v2_blocks(q.numpy(), k.numpy(), v.numpy(), 4)
-        kind, what = "port", "oracle.flash_v2_blocks (C restatement of tiny_flash_attn.py:137-196)"
+    from oracle import oracle as orc
+    fn = lambda: orc.flash_v2_blocks(q.numpy(), k.numpy(), v.numpy(), 4)
+    kind, what = "port", "oracle.flash_v2_blocks (C restatement of tiny_flash_attn.py:137-196)"
     fn()
     ts = []
     for _ in range(3):
@@ -715,6 +667,24 @@ def time_naive_python_cfg1():
     _t.set_num_threads(os.cpu_count() or 1)
     return {"tflops": F / t / 1e12, "seconds": t, "kind": kind, "cores": 1, "what": what,
             "config": "cfg1: B=1 H=2 S=128 D=64 fp32 non-causal, scale 1"}
+
+
+DUMP_HEADS = 8          # (batch, head) pairs of O written by --dump-outputs: 8 x S x D fp32 = 16 MB at the workload
+
+
+def dump_outputs(d, o, lse):
+    """What the timed path hands its caller, from the last timed step: a fixed, seeded sample of DUMP_HEADS (batch, head)
+    pairs of O (out_heads.npy, float32 (DUMP_HEADS, S, D); which pairs: out_heads_index.npy, float64 (DUMP_HEADS, 2))
+    and this rank's whole LSE (lse.npy, float32 (B, H, S) at N=1)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    B_, H_ = o.shape[0], o.shape[1]
+    pick = np.random.default_rng(20).choice(B_ * H_, size=min(DUMP_HEADS, B_ * H_), replace=False)
+    pick.sort()
+    idx = np.stack([pick // H_, pick % H_], axis=1)
+    np.save(os.path.join(d, "out_heads.npy"), np.stack([o[b_, h_].float().cpu().numpy() for b_, h_ in idx]))
+    np.save(os.path.join(d, "out_heads_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(d, "lse.npy"), lse.float().cpu().numpy())
 
 
 def emit(line: dict) -> None:
@@ -740,7 +710,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
-    ap.add_argument("--no-comparators", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy")
     ap.add_argument("--exchange", default="fused", choices=["fused", "nccl"],
                     help="N>1: how O is gathered (fused peer stores in the kernel epilogue, or ncclAllGather)")
     ap.add_argument("--chunks", type=int, default=1, help="N>1: batch chunks per rank (gather/compute overlap)")

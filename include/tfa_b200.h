@@ -1,10 +1,10 @@
-/* tfa_b200.h -- C ABI of the B200-native (sm_100a) flash-attention forward.
+/* tfa_b200.h -- C ABI of the H100-native (sm_90a) flash-attention forward.
  *
  * This is the drop-in boundary for the ONE hot path of 66RING/tiny-flash-attention:
  * the fused  O = softmax(scale * Q K^T [+ causal mask]) V  forward, plus the row
  * log-sum-exp.  Plain pointers and sizes only: no torch types cross this line.
  *
- * Reference interfaces replaced (paths relative to /root/reference):
+ * Reference interfaces replaced (paths relative to the reference project's root):
  *   - flash_attention_cutlass/include/attention_api.h:10-11 and
  *     flash_attention_cutlass/csrc/flash_attention.cu:741-772
  *       std::vector<torch::Tensor> flash_attention_v2_cutlass(q, k, v, is_causal, softmax_scale)
@@ -46,7 +46,7 @@ extern "C" {
 #define TFA_EINVAL_DTYPE  (-4)  /* dtype not TFA_BF16 / TFA_FP16                  */
 #define TFA_EINVAL_STRIDE (-5)  /* strides not expressible as a TMA tensor map    */
 #define TFA_EDRIVER       (-6)  /* cuTensorMapEncodeTiled unavailable / failed    */
-#define TFA_EARCH         (-7)  /* device is not compute capability 10.x          */
+#define TFA_EARCH         (-7)  /* device is not compute capability 9.0           */
 #define TFA_EDEVICE_FAULT (-8)  /* kernel watchdog fired; see tfa_debug_record()  */
 #define TFA_EINVAL_SCALE  (-9)  /* softmax_scale negative, NaN or infinite         */
 #define TFA_EINVAL_HEADS  (-10) /* Hq not a multiple of Hkv                         */
@@ -106,7 +106,7 @@ int tfa_fwd_multi(const tfa_fwd_args* args, void* const* extra_out, int n_extra)
  *   causal : query row i sees keys j <= i + (Sk - Sq).  Rows that see no key (only when Sk < Sq) get
  *            out = 0 and lse = +inf (the CuTe epilogue's rule for an empty row, flash_attention.cu:620-623).
  *   num_splits: 1 = one pass.  n > 1 = the key range is cut into n chunks processed by independent CTAs (fills
- *            the GPU when B*Hq*ceil(Sq/256) is small), partial results go to `workspace`
+ *            the GPU when B*Hq*ceil(Sq/128) is small), partial results go to `workspace`
  *            (tfa_attn_workspace_bytes()) and a second small kernel merges them through their LSEs.
  *            0 = let the library decide (splits only if a workspace large enough was passed).           */
 typedef struct tfa_attn_args {
@@ -163,14 +163,14 @@ const char* tfa_error_string(int code);
 int tfa_selftest_tma(const void* src, int D, int S, int BH, int x0, int y0, int z0,
                      void* dump_16k, void* stream);
 
-/* One UMMA chain: C(128 x N, fp32) = A(128 x K) * B^T, operands staged by TMA.
+/* One wgmma chain: C(128 x N, fp32) = A(128 x K) * B, operands staged by TMA, two m64 halves.
  *   mode 0: SS, B is (N x K) K-major       (the Q K^T contraction)
  *   mode 1: SS, B is (K x N) MN-major      (V consumed in place)
- *   mode 2: TS, A packed to 16-bit in TMEM, B (K x N) MN-major  (the P V contraction)
+ *   mode 2: RS, A in registers (16-bit pairs), B (K x N) MN-major  (the P V contraction)
  * K in {64,128}, N in {64,128}.  `knobs` (may be NULL) overrides descriptor fields:
  *   knobs[0] = LBO bytes (0 = default), knobs[1] = SBO bytes (0 = default),
  *   knobs[2] = k-step byte advance (0 = default), knobs[3] = flags
- *              (bit0: swap packing order of the two 16-bit halves in TMEM A).     */
+ *              (bit0: swap packing order of the two 16-bit halves of register A). */
 int tfa_selftest_umma(const void* a, const void* b, float* c, int N, int K, int mode,
                       int dtype, const int* knobs, void* stream);
 

@@ -1,13 +1,11 @@
-"""Runs ONE bring-up case of the sm_100a primitives in its own process and prints a JSON verdict.
+"""Runs ONE bring-up case of the sm_90a primitives in its own process and prints a JSON verdict.
 
 Used by tests/test_umma_primitives.py (each case in a subprocess: a device trap poisons the CUDA context
-of the process that hit it, so cases must not share one) and directly from gpurun for sweeps:
+of the process that hit it, so cases must not share one) and directly:
     python tests/prim_runner.py tma
     python tests/prim_runner.py umma '{"N":128,"K":128,"mode":2,"dtype":"bf16"}'
-    python tests/prim_runner.py sweep '{"N":128,"K":128,"mode":1}'      # descriptor-knob sweep -> gpurun_out/
 """
 import ctypes
-import itertools
 import json
 import os
 import sys
@@ -72,34 +70,11 @@ def umma_case(N=128, K=128, mode=0, dtype="bf16", knobs=None, seed=0):
             "max_abs_err": maxerr, "nan": nan, "ok": maxerr == 0.0 and nan == 0}
 
 
-def sweep(N=128, K=128, mode=1, dtype="bf16"):
-    """Try descriptor-field alternatives for the B operand; append every verdict to gpurun_out/umma_sweep.jsonl."""
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    path = os.path.join(ROOT, "gpurun_out", "umma_sweep.jsonl")
-    slab = (N if mode == 0 else K) * 128
-    if mode == 0:
-        lbos, sbos, ksteps = [0, 1024, slab], [0, 128, slab], [0, 64, 16]
-    else:
-        lbos = [0, 1024, 128, 2048, 16, 64 * 128]
-        sbos = [0, slab, 128, 2048, 256]
-        ksteps = [0, 256, 32, 4096, 1024]
-    flags = [0, 1] if mode == 2 else [0]
-    winners = []
-    with open(path, "a") as f:
-        for lbo, sbo, ks, fl in itertools.product(lbos, sbos, ksteps, flags):
-            r = umma_case(N, K, mode, dtype, [lbo, sbo, ks, fl])
-            f.write(json.dumps(r) + "\n")
-            f.flush()
-            if r["ok"]:
-                winners.append(r["knobs"])
-    return {"case": "sweep", "N": N, "K": K, "mode": mode, "winners": winners, "ok": bool(winners)}
-
-
 if __name__ == "__main__":
     kind = sys.argv[1]
     kw = json.loads(sys.argv[2]) if len(sys.argv) > 2 else {}
     try:
-        res = {"tma": tma_case, "umma": umma_case, "sweep": sweep}[kind](**kw)
+        res = {"tma": tma_case, "umma": umma_case}[kind](**kw)
     except Exception as e:  # noqa: BLE001
         res = {"case": kind, "ok": False, "error": repr(e), "debug": tfa_ctypes.debug_record()}
     print("PRIM_RESULT " + json.dumps(res))

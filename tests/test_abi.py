@@ -132,7 +132,7 @@ def test_split_bookkeeping_invariants(built):
 
 
 def test_launch_order_mapping_is_a_bijection(built):
-    """decode_work (csrc/fa_fwd_sm100.cuh) -- the SAME function the kernel runs, called on the host: every CTA index maps
+    """decode_work (csrc/fa_fwd_sm90.cuh) -- the SAME function the kernel runs, called on the host: every CTA index maps
     to a distinct, in-range (batch*head, split, pair); inside a chunk of heads the order is heaviest pair first."""
     import tfa_ctypes
     L = tfa_ctypes.lib()
@@ -164,8 +164,9 @@ def test_launch_order_mapping_is_a_bijection(built):
 
 
 def test_kernel_selection_rule_on_the_host(built):
-    """choose_kernel (csrc/tfa_api.cu) through its host-callable twin: the shapes of profiles/r02_kernel_choice.md, 148 SMs.
-    0 = one CTA per work item, 4 = persistent.  (TFA_KERNEL forces one kernel and is read once per process.)"""
+    """choose_kernel (csrc/tfa_api.cu) through its host-callable twin, on an H100's 132 SMs: the shapes of the H100 A/B
+    (profiles/h100_kernel_choice.txt).  0 = one CTA per work item, 4 = persistent.  (TFA_KERNEL forces one kernel and is
+    read once per process.)"""
     if os.environ.get("TFA_KERNEL"):
         pytest.skip("TFA_KERNEL forces a kernel in this process")
     import tfa_ctypes
@@ -174,21 +175,20 @@ def test_kernel_selection_rule_on_the_host(built):
     f.restype = ctypes.c_int
     CLASSIC, PERSIST = 0, 4
 
-    def pick(B, H, S, D, causal, nsplit=1, sms=148, n_extra=0, Sk=None):
+    def pick(B, H, S, D, causal, nsplit=1, sms=132, n_extra=0, Sk=None):
         return f(D, int(causal), S, S if Sk is None else Sk, B, H, nsplit, sms, n_extra)
 
-    assert pick(4, 32, 4096, 128, True) == PERSIST          # cfg3
-    assert pick(64, 32, 4096, 128, True) == PERSIST         # cfg5
+    assert pick(4, 32, 4096, 128, True) == CLASSIC          # cfg3
+    assert pick(64, 32, 4096, 128, True) == CLASSIC         # cfg5
     assert pick(1, 32, 16384, 128, True) == CLASSIC         # cfg4: few, very long causal items
     assert pick(2, 32, 8192, 128, True) == CLASSIC
-    assert pick(64, 32, 8192, 128, True) == PERSIST         # ... but not when there are >= 32 items per SM
-    assert pick(16, 32, 1024, 128, True) == PERSIST
+    assert pick(16, 32, 1024, 128, True) == PERSIST         # short causal items
     assert pick(4, 32, 4096, 128, False) == PERSIST
     assert pick(2, 32, 8192, 128, False) == PERSIST
-    assert pick(1, 32, 16384, 128, False) == CLASSIC        # 128 KV tiles per item, 13.8 items per SM
-    assert pick(1, 32, 16384, 128, False, nsplit=2) == PERSIST   # split-KV halves the tiles per item
+    assert pick(1, 32, 16384, 128, False) == PERSIST        # 128 KV tiles per item, 31 items per SM
+    assert pick(1, 32, 16384, 128, False, nsplit=2) == PERSIST
     assert pick(4, 16, 2048, 64, False) == PERSIST          # cfg2
-    assert pick(1, 32, 16384, 64, False) == CLASSIC
+    assert pick(1, 32, 16384, 64, False) == PERSIST
     assert pick(4, 32, 4096, 64, True) == CLASSIC           # D=64 causal
-    assert pick(32, 32, 512, 64, True) == PERSIST           # ... except S <= 512
-    assert pick(1, 32, 16384, 128, True, n_extra=1) == PERSIST   # the fused exchange always stores through TMA
+    assert pick(32, 32, 512, 64, True) == PERSIST           # ... except short items
+    assert pick(1, 32, 16384, 128, True, n_extra=1) == PERSIST   # the fused exchange keeps the persistent schedule

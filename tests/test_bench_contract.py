@@ -32,11 +32,11 @@ def test_ours_arm_refuses_to_run_without_gpu():
 
 
 def test_metric_is_baseline_json_verbatim_and_recorded_line_has_the_contract_keys():
-    """The metric string is BASELINE.json's, and the line recorded on a B200 (profiles/) carries every contract key."""
+    """The metric string is BASELINE.json's, and the line recorded on an H100 (profiles/) carries every contract key."""
     sys.path.insert(0, ROOT)
     import bench
     assert bench.METRIC == json.load(open(os.path.join(ROOT, "BASELINE.json")))["metric"]
-    d = json.load(open(os.path.join(ROOT, "profiles", "r01_final_bench_n1.json")))
+    d = json.load(open(os.path.join(ROOT, "profiles", "h100_bench_n1.json")))
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
               "vs_baseline", "dtype", "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline"):
         assert k in d, k

@@ -1,4 +1,4 @@
-"""GPU: the sm_100a forward, called through the C ABI, against the CPU oracle / golden fixtures
+"""GPU: the sm_90a forward, called through the C ABI, against the CPU oracle / golden fixtures
 (bit-for-bit math model of the reference kernel, SURVEY.md A.1) on the same seeded inputs.
 
 Tolerances (north_star: rtol=1e-3 / atol=1e-3 for bf16):
@@ -183,8 +183,7 @@ def test_deterministic(tfa):
 
 def test_classic_and_persistent_kernels_agree_bitwise(tfa):
     """The kernel is selected per process (TFA_KERNEL): the one-CTA-per-item kernel and the persistent kernel do the same
-    arithmetic in the same order, so one causal and one ragged case must agree bit for bit (different schedules, TMA-store
-    vs st.global epilogue)."""
+    arithmetic in the same order, so one causal and one ragged case must agree bit for bit (different schedules)."""
     import os
     import subprocess
     import sys

@@ -1,6 +1,7 @@
 """GPU: which kernel the library picks on its own (`choose_kernel`, csrc/tfa_api.cu) for the shapes the rule was measured on
-(profiles/r02_kernel_choice.md).  The rule is host logic, but the only observable is the variant of the last launch, so the
-shapes are launched for real -- in a subprocess, because TFA_KERNEL (which forces one kernel) is read once per process."""
+(an A/B of both schedules on one H100, profiles/h100_kernel_choice.txt).  The rule is host logic, but the only observable is
+the variant of the last launch, so the shapes are launched for real -- in a subprocess, because TFA_KERNEL (which forces one
+kernel) is read once per process."""
 import os
 import subprocess
 import sys
@@ -11,15 +12,15 @@ pytestmark = pytest.mark.gpu
 
 CLASSIC, PERSIST = 0, 4
 CASES = [
-    # B, H, S, D, causal, expected, why
-    (4, 32, 4096, 128, True, PERSIST, "cfg3"),
-    (1, 32, 16384, 128, True, CLASSIC, "cfg4: few, very long causal items"),
-    (16, 32, 1024, 128, True, PERSIST, "short causal items"),
-    (1, 32, 16384, 128, False, CLASSIC, "non-causal, 128 KV tiles per item, 13.8 items per SM"),
-    (2, 32, 8192, 128, False, PERSIST, "non-causal, 64 KV tiles per item"),
-    (4, 16, 2048, 64, False, PERSIST, "cfg2"),
-    (4, 32, 4096, 64, True, CLASSIC, "D=64 causal"),
-    (32, 32, 512, 64, True, PERSIST, "D=64 causal, S <= 512"),
+    # B, H, S, D, causal, expected, why (H100 A/B, median ms one-CTA-per-item / persistent)
+    (4, 32, 4096, 128, True, CLASSIC, "cfg3: 0.913 / 1.002"),
+    (1, 32, 16384, 128, True, CLASSIC, "cfg4, few very long causal items: 3.16 / 3.66"),
+    (16, 32, 1024, 128, True, PERSIST, "short causal items: 0.423 / 0.378"),
+    (1, 32, 16384, 128, False, PERSIST, "non-causal, 128 KV tiles per item, 31 items per SM: 7.22 / 6.75"),
+    (2, 32, 8192, 128, False, PERSIST, "non-causal, 64 KV tiles per item: 3.36 / 3.26"),
+    (4, 16, 2048, 64, False, PERSIST, "cfg2: 0.235 / 0.225"),
+    (4, 32, 4096, 64, True, CLASSIC, "D=64 causal: 0.817 / 0.893"),
+    (32, 32, 512, 64, True, PERSIST, "D=64 causal, S <= 512: 0.227 / 0.189"),
 ]
 
 CODE = r'''

@@ -1,4 +1,4 @@
-"""GPU: the LAZY-RESCALE branch of the online softmax (rescale_if_needed: O read-modify-write in TMEM, l *= alpha,
+"""GPU: the LAZY-RESCALE branch of the online softmax (O rescaled in registers, l *= alpha,
 P carried against a stale max, values up to 2^8) against the CPU oracle.
 
 The seeded N(0, 0.5^2) inputs of the other parity files never move the running row max by more than 2^8 between KV

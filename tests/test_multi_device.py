@@ -1,5 +1,5 @@
 """GPU, >= 2 devices in ONE process (skipped on the 1-GPU box): per-device host state (ADVICE r01).  The dynamic shared
-memory opt-in, the SM count, the persistent kernel's work counters and the host-buffer workspace all belong to a device;
+memory opt-in, the SM count and the host-buffer workspace all belong to a device;
 a process that runs the forward on cuda:0 and then on cuda:1 must get the oracle's result on both."""
 import numpy as np
 import pytest

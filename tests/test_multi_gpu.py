@@ -1,7 +1,7 @@
 """GPU, >= 2 devices (skipped on the 1-GPU box; tests/test_fused_exchange.py covers the same kernel path on one device):
 the fused attention + all-gather (peer stores from the kernel epilogue) must be the CPU ORACLE's attention on every rank
 (reference arithmetic: flash_attention_c/csrc/attn.cpp:101-167 via oracle.attn_exact), and bit-identical to the
-single-GPU kernel.  Run with `gpurun --gpus 2 -- python -m pytest tests/test_multi_gpu.py -m gpu`."""
+single-GPU kernel.  Run on a machine with >= 2 GPUs: `python -m pytest tests/test_multi_gpu.py -m gpu`."""
 import os
 import subprocess
 import sys

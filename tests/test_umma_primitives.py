@@ -1,5 +1,5 @@
-"""GPU: bring-up tests of the Blackwell primitives the forward kernel is made of (TMA SWIZZLE_128B
-loads, SS-form UMMA with K-major and MN-major B, TS-form UMMA with A packed in TMEM).
+"""GPU: bring-up tests of the Hopper primitives the forward kernel is made of (TMA SWIZZLE_128B
+loads, SS-form wgmma with K-major and MN-major B, RS-form wgmma with A in registers).
 Each case runs in its own process (tests/prim_runner.py)."""
 import json
 import os
@@ -44,6 +44,7 @@ def test_umma_ss_mnmajor_b(built, N, K):
 @pytest.mark.parametrize("dtype", ["bf16", "fp16"])
 @pytest.mark.parametrize("N,K", [(128, 128), (64, 128)])
 def test_umma_ts_a_in_tmem(built, N, K, dtype):
-    """O += P V shape: A (=P) packed two 16-bit values per TMEM column, B (=V) MN-major."""
+    """O += P V shape (the name is from the Blackwell build, where A sat in tensor memory): RS-form wgmma, A (=P)
+    packed two 16-bit values per register, B (=V) MN-major."""
     r = run_case("umma", N=N, K=K, mode=2, dtype=dtype)
     assert r["ok"], r

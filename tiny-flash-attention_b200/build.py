@@ -1,6 +1,6 @@
-"""In-tree build of the B200-native flash-attention forward.
+"""In-tree build of the H100-native flash-attention forward.
 
-Plays the role of the reference's /root/reference/flash_attention_cutlass/build.py:42-84 (which
+Plays the role of the reference's flash_attention_cutlass/build.py:42-84 (which
 builds the `attention_cutlass` CUDAExtension for sm_80/sm_90), but produces two artefacts, both
 next to this file so they travel with the repo snapshot:
 
@@ -8,8 +8,8 @@ next to this file so they travel with the repo snapshot:
   attention_cutlass.<abi>.so           the PyTorch extension module with the reference's name/API,
                                        a thin wrapper that links libtfa_b200.so via $ORIGIN rpath
 
-Everything is compiled for sm_100a only:  -gencode arch=compute_100a,code=sm_100a  (the
-`-arch=sm_100a` shorthand also emits plain compute_100 PTX, which cannot hold tcgen05).
+Everything is compiled for sm_90a only:  -gencode arch=compute_90a,code=sm_90a  (the
+`-arch=sm_90a` shorthand also emits plain compute_90 PTX, which cannot hold wgmma or setmaxnreg).
 
 Usage:  python build.py [--force] [--no-torch-ext]
 """
@@ -33,10 +33,10 @@ CXX = os.environ.get("CXX", "g++")
 LIB_NAME = "libtfa_b200.so"
 EXT_NAME = "attention_cutlass" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so")
 
-CU_SOURCES = ["tfa_api.cu", "tfa_selftest.cu", "tfa_microbench.cu"]
-CU_HEADERS = ["ptx_sm100.cuh", "fa_fwd_sm100.cuh", "fa_fwd_sm100_persist.cuh", "fa_splitkv_combine.cuh"]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+CU_SOURCES = ["tfa_api.cu", "tfa_selftest.cu"]
+CU_HEADERS = ["ptx_sm90.cuh", "fa_fwd_sm90.cuh", "fa_splitkv_combine.cuh"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + [
     "-O3", "-std=c++17", "-lineinfo",
     "--use_fast_math",            # the reference builds with it too (build.py:58); exp uses ex2.approx anyway
     "-Xcompiler", "-fPIC",
@@ -90,7 +90,7 @@ def build_lib(force=False, verbose=True, variant=None, extra_flags=()):
             sys.stderr.write(so)
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
     # link under a temporary name and rename: a snapshot of the tree never sees a half-written library
-    _run([NVCC, "-shared", "-Wno-deprecated-gpu-targets", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out + ".tmp"] + objs + ["-lcudart"], log)
+    _run([NVCC, "-shared", "-Wno-deprecated-gpu-targets"] + GENCODE + ["-o", out + ".tmp"] + objs + ["-lcudart"], log)
     os.replace(out + ".tmp", out)
     for o in objs:
         os.remove(o)
@@ -151,7 +151,7 @@ def build_all(force=False, torch_ext=True, verbose=True):
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:      # python build.py --variant emu4 -DTFA_EMU_PAIRS_PER_8=4
+    if "--variant" in sys.argv:      # python build.py --variant dbg -DTFA_DEBUG_WATCHDOG
         i = sys.argv.index("--variant")
         build_lib(force=True, variant=sys.argv[i + 1], extra_flags=[a for a in sys.argv[i + 2:] if a.startswith("-D")])
     else:

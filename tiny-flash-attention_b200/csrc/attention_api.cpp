@@ -35,7 +35,7 @@ namespace {
 
 // NOTE: every message below is ONE preformatted string.  Multi-argument TORCH_CHECK formats through
 // std::ostream inside this module, and this image's g++ emits weak libstdc++ stream symbols into the .so that
-// crash once the CUDA user-mode driver is loaded (seen on the B200 box: SIGSEGV in ostream::_M_insert<long>).
+// crash once the CUDA user-mode driver is loaded (SIGSEGV in ostream::_M_insert<long>).
 std::string fmt_msg(const char* fmt, long long a = 0, long long b = 0, long long c = 0, long long d = 0,
                     long long e = 0) {
   char buf[256];
@@ -198,7 +198,7 @@ std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Te
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_cutlass", &flash_attention_v2_cutlass,
-        "Flash attention v2 forward, B200-native (sm_100a tcgen05/TMEM/TMA)");
+        "Flash attention v2 forward, H100-native (sm_90a wgmma/TMA)");
   // the name BASELINE.json's north_star uses for the same call
   m.def("flash_attn_fwd", &flash_attention_v2_cutlass, "alias of flash_attention_v2_cutlass");
   m.def("flash_attention_v2_bshd", &flash_attention_v2_bshd, "same op on (B,S,H,D) tensors");

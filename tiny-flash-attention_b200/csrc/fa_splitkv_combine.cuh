@@ -14,7 +14,7 @@
 // half-warp (D=64) owns a row, every global access is a full 16-byte (fp32 in) / 8-byte (16-bit out) vector.
 // Roofline: HBM.  Algorithmic bytes per row: combine nsplit_valid*(4D+4) + 2D + 4, fill 2D + 4.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace tfa {
 

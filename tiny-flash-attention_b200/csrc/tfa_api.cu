@@ -4,12 +4,11 @@
 //   flash_attention_v2_cutlass -> set_params_fprop -> run_flash_attn_cutlass ->
 //   FP16_SWITCH -> FWD_HEADDIM_SWITCH -> BOOL_SWITCH -> run_flash_fwd
 // (/root/reference/flash_attention_cutlass/csrc/flash_attention.cu:320-361,687-772,
-//  csrc/static_switch.h:17-66) for the sm_100a kernel in fa_fwd_sm100.cuh.
+//  csrc/static_switch.h:17-66) for the sm_90a kernel in fa_fwd_sm90.cuh.
 // Differences on purpose (SURVEY.md A.2): arguments are validated and rejected loudly, the
 // caller's stream is honoured, nothing synchronises the device, nothing calls exit().
 #include "../../include/tfa_b200.h"
-#include "fa_fwd_sm100.cuh"
-#include "fa_fwd_sm100_persist.cuh"
+#include "fa_fwd_sm90.cuh"
 #include "fa_splitkv_combine.cuh"
 
 #include <cuda_runtime.h>
@@ -28,8 +27,6 @@ using tfa::FwdParams;
 
 std::atomic<unsigned long long> g_launches{0};
 std::atomic<int> g_last_variant{0};         // kernel the last forward launch used (0 classic, 4 persistent)
-unsigned long long* g_trace_buf = nullptr;   // only read by -DTFA_TRACE variant builds
-int g_trace_block = 0;
 
 // ---- driver entry point for cuTensorMapEncodeTiled (no link-time libcuda dependency) ----
 PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
@@ -64,7 +61,8 @@ void init_dbg() {
 // (B?,H?,S,D)-strided 16-bit tensor -> 4-D tiled map with dims (D, S, H, B); the kernel addresses it as
 // (x = head-dim offset, y = sequence row, z = head, w = batch).  Box = 64 x 128 elements, SWIZZLE_128B.
 int make_tmap(CUtensorMap* m, const void* base, int dtype, int D, int S, int B, int H, long long sb,
-              long long sh, long long ss, int box_rows = 128, int box_cols = 64) {
+              long long sh, long long ss) {
+  constexpr int box_rows = 128, box_cols = 64;
   auto encode = get_encode_fn();
   if (!encode) return TFA_EDRIVER;
   const CUtensorMapDataType dt = (dtype == TFA_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
@@ -80,61 +78,18 @@ int make_tmap(CUtensorMap* m, const void* base, int dtype, int D, int S, int B, 
   for (int i = 0; i < 3; ++i)
     if ((strides[i] % 16) || strides[i] >= (1ull << 40)) return TFA_EINVAL_STRIDE;
   CUresult r = encode(m, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : TFA_EDRIVER;
 }
 
-// ---- per-device state.  Function attributes, SM counts, work counters and workspaces belong to ONE device (context):
+// ---- per-device state.  Function attributes, SM counts and workspaces belong to ONE device (context):
 //      a process that drives several GPUs (tensors on cuda:0, then cuda:1) must not reuse the first device's. ----
 constexpr int kMaxDevices = 64;
 int current_device() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return -1;
   return dev;
-}
-
-// ---- work counters of the persistent kernel: a small pool per device, one {next item, CTAs finished} pair per
-//      in-flight launch.  A pair is zero whenever no launch owns it: the pool is zeroed once at creation and the LAST CTA
-//      of a launch to run out of work resets its pair (fa_fwd_sm100_persist.cuh), so no memset sits in front of every
-//      launch.  A slot is re-used kNumSchedCounters launches later; the event recorded behind each launch is waited for
-//      (host side, normally long complete) before the slot is handed out again, so two in-flight launches never share one.
-//      (The round-1 experimental variants still get a stream-ordered memset: they do not reset.) ----
-constexpr int kNumSchedCounters = 64;
-struct SchedPool {
-  int* base = nullptr;                 // kNumSchedCounters x {counter, done}
-  unsigned next = 0;
-  cudaEvent_t done[kNumSchedCounters] = {};
-  bool used[kNumSchedCounters] = {};
-  std::mutex mu;
-};
-SchedPool g_sched[kMaxDevices];
-int* acquire_sched_counter(cudaStream_t stream, cudaError_t* err, int* slot_out, bool self_resetting) {
-  const int dev = current_device();
-  if (dev < 0) { *err = cudaErrorInvalidDevice; return nullptr; }
-  SchedPool& sp = g_sched[dev];
-  std::lock_guard<std::mutex> lk(sp.mu);
-  if (!sp.base) {
-    void* d = nullptr;
-    if ((*err = cudaMalloc(&d, kNumSchedCounters * 2 * sizeof(int))) != cudaSuccess) return nullptr;
-    if ((*err = cudaMemset(d, 0, kNumSchedCounters * 2 * sizeof(int))) != cudaSuccess) { cudaFree(d); return nullptr; }
-    sp.base = static_cast<int*>(d);
-  }
-  const int slot = static_cast<int>(sp.next++ % kNumSchedCounters);
-  if (sp.used[slot]) {
-    if ((*err = cudaEventSynchronize(sp.done[slot])) != cudaSuccess) return nullptr;   // normally long complete
-  } else {
-    if ((*err = cudaEventCreateWithFlags(&sp.done[slot], cudaEventDisableTiming)) != cudaSuccess) return nullptr;
-    sp.used[slot] = true;
-  }
-  *err = self_resetting ? cudaSuccess : cudaMemsetAsync(sp.base + 2 * slot, 0, 2 * sizeof(int), stream);
-  *slot_out = slot;
-  return sp.base + 2 * slot;
-}
-void release_sched_counter(int slot, cudaStream_t stream) {
-  const int dev = current_device();
-  if (dev < 0) return;
-  cudaEventRecord(g_sched[dev].done[slot], stream);
 }
 
 int num_sms() {
@@ -149,12 +104,9 @@ int num_sms() {
   return v;
 }
 
-// Kernel selection.  TFA_KERNEL (read once) forces one kernel: "classic" = one CTA per work item (fa_fwd_sm100.cuh);
-// "persist" = persistent CTAs with cross-item overlap and the TMA-store epilogue (fa_fwd_sm100_persist.cuh);
-// Unset = AUTO, from the B200 measurements of round 2 (profiles/r02_kernel_choice.md): see choose_kernel().
-// The round-1 experimental variants (column-split softmax, the first persistent kernel and its port) and round 2's D=64
-// kernel with two softmax warpgroups per Q tile were measured on B200 -- 5-20 % slower or faulting -- and removed
-// (profiles/r02_variants_ab.txt, profiles/r02_kernel_choice.md).
+// Kernel selection.  TFA_KERNEL (read once) forces one kernel: "classic" = one CTA per work item; "persist" = one CTA
+// per SM walking the work items, whose producer loads the next item's Q and K/V while the current one finishes (same
+// kernel source, fa_fwd_sm90.cuh, PERSIST = true).  Unset = AUTO: see choose_kernel().
 enum { KV_AUTO = -1, KV_CLASSIC = 0, KV_PERSIST = 4 };
 int kernel_variant() {
   static int v = [] {
@@ -166,33 +118,21 @@ int kernel_variant() {
   }();
   return v;
 }
-// AUTO: the persistent kernel wins where its cross-item overlap and TMA-store epilogue outweigh its slightly longer
-// issue path (rolled issuer, dynamic ring slots): many work items per SM, non-causal items, and the fused exchange
-// (peer stores leave from the TMA engine instead of the softmax warps).  Few, long, lopsided (causal) items per SM are
-// where the one-CTA-per-item kernel's hardware scheduling still wins by ~2 %.
-int choose_kernel(int D, bool causal, long long nitems, long long npairs, long long nkv, int sms, int n_extra) {
+// AUTO, from an A/B of the two schedules on one H100 80GB HBM3 at 700 W (profiles/h100_kernel_choice.txt): the persistent
+// schedule wins on every non-causal shape measured (1-7 %) and on short causal items (S <= 1024: 11-17 %); from S = 4096
+// up, causal items are unequal enough that the hardware's dynamic CTA scheduling wins (4-14 %).  The fused exchange keeps
+// the persistent schedule (its multi-GPU timing has not been measured on H100).
+int choose_kernel(bool causal, long long npairs, int n_extra) {
   const int forced = kernel_variant();
   if (forced != KV_AUTO) return forced;
-  if (n_extra > 0) return KV_PERSIST;
-  const bool few_items = nitems < 32LL * sms;
-  if (!causal) {
-    // D=64 too: +5..14 % (cfg2 0.1106 vs 0.1167 ms, B16 H16 S1024 0.1024 vs 0.1167).  Only few items of >= 128 KV tiles
-    // (S >= 16384) favour the classic kernel: D=128 3.00 vs 3.02-3.12 ms, D=64 2.61-2.73 vs 2.73-2.82 (b18 A/B).
-    return (nkv >= 128 && few_items) ? KV_CLASSIC : KV_PERSIST;
-  }
-  // D=64 causal: classic by 4-9 % from S=2048 up (B4 H32 S4096 0.387 vs 0.408 ms), persistent by 7 % on short items
-  // (B32 H32 S512 0.122 vs 0.131)
-  if (D != 128) return npairs <= 2 ? KV_PERSIST : KV_CLASSIC;
-  // causal: few very long items per SM (S >= 8192 with < 32 items per SM) still favour the classic kernel by 2-8 %
-  return (npairs >= 32 && few_items) ? KV_CLASSIC : KV_PERSIST;
+  if (n_extra > 0 || !causal) return KV_PERSIST;
+  return npairs <= 8 ? KV_PERSIST : KV_CLASSIC;
 }
 
-// the problem as choose_kernel sees it: work items, Q-tile pairs per head, KV tiles per item
-int variant_for(int D, bool causal, int Sq, int Sk, int B, int Hq, int nsplit, int sms, int n_extra) {
-  const long long npairs = (static_cast<long long>(Sq) + 255) / 256;
-  const long long nitems = npairs * B * Hq * nsplit;
-  const long long nkv = ((static_cast<long long>(Sk) + 127) / 128 + nsplit - 1) / nsplit;
-  return choose_kernel(D, causal, nitems, npairs, nkv, sms, n_extra);
+// the problem as choose_kernel sees it: Q-tile pairs per head
+int variant_for(bool causal, int Sq, int n_extra) {
+  const long long npairs = (static_cast<long long>(Sq) + 127) / 128;
+  return choose_kernel(causal, npairs, n_extra);
 }
 
 // cudaFuncSetAttribute is per device (context) and costs well under a microsecond: set it on every launch instead of
@@ -203,25 +143,22 @@ cudaError_t opt_in_smem(K kernel, int bytes) {
 }
 
 template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32>
-int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const tfa::OutMaps& to, FwdParams p,
-                long long nitems, int variant, cudaStream_t stream) {
+int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
+                int variant, cudaStream_t stream) {
   cudaError_t cerr = cudaSuccess;
   g_last_variant.store(variant, std::memory_order_relaxed);
+  long long nblocks = nitems;
   if (variant == KV_PERSIST) {
-    int slot = 0;
-    p.sched_counter = acquire_sched_counter(stream, &cerr, &slot, true);
-    if (cerr != cudaSuccess) return static_cast<int>(cerr);
     const int sms = num_sms();
     if (sms <= 0) return TFA_EARCH;
-    int nblocks = static_cast<int>(nitems < sms ? nitems : sms);             // one CTA per SM
-    auto kern = tfa::fa_fwd_sm100_persist_kernel<D, CAUSAL, IS_BF16, OUT_F32>;
-    if ((cerr = opt_in_smem(kern, tfa::PCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
-    kern<<<nblocks, tfa::PCfg<D>::THREADS, tfa::PCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, to, p);
-    release_sched_counter(slot, stream);
-  } else {
-    auto kern = tfa::fa_fwd_sm100_kernel<D, CAUSAL, IS_BF16, OUT_F32>;
+    if (nblocks > sms) nblocks = sms;                                   // one CTA per SM
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true>;
     if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
-    kern<<<static_cast<int>(nitems), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+    kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  } else {
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false>;
+    if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
+    kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   }
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return static_cast<int>(cudaGetLastError());
@@ -229,8 +166,8 @@ int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
 
 template <int D>
 int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
-             const tfa::OutMaps& to, const FwdParams& p, long long nblocks, int variant, cudaStream_t s) {
-#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_>(tq, tk, tv, to, p, nblocks, variant, s)
+             const FwdParams& p, long long nblocks, int variant, cudaStream_t s) {
+#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_>(tq, tk, tv, p, nblocks, variant, s)
   if (causal) {
     if (bf16) { if (f32) TFA_GO(true, true, true); else TFA_GO(true, true, false); }
     else      { if (f32) TFA_GO(true, false, true); else TFA_GO(true, false, false); }
@@ -242,14 +179,15 @@ int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUte
 }
 
 bool arch_ok() {
-  static std::atomic<int> cache[kMaxDevices];    // 0 = unknown, 1 = sm_10x, 2 = something else
+  static std::atomic<int> cache[kMaxDevices];    // 0 = unknown, 1 = sm_90, 2 = something else
   const int dev = current_device();
   if (dev < 0) return false;
   int v = cache[dev].load(std::memory_order_relaxed);
   if (v == 0) {
-    int major = 0;
+    int major = 0, minor = 0;     // sm_90a code (wgmma, setmaxnreg) runs on compute capability 9.0 only
     if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return false;
-    v = (major == 10) ? 1 : 2;
+    if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return false;
+    v = (major == 9 && minor == 0) ? 1 : 2;
     cache[dev].store(v, std::memory_order_relaxed);
   }
   return v == 1;
@@ -289,11 +227,12 @@ int validate(const Problem& a) {
 }
 
 // Split-KV decision.  `want` 0 = auto: split only when the plain grid would leave more than half of the SMs idle,
-// into as many splits as still fit one wave of CTAs (a 149th CTA would double the time), each with >= 4 KV tiles;
+// into as many splits as still fit one wave of CTAs (one CTA more than the SMs would double the time), each with
+// >= 4 KV tiles;
 // n > 1 = as asked, clamped so that no split is empty.
 int resolve_splits(const Problem& a, int want, int sms) {
   const int sq_eff = (a.causal && a.Sk < a.Sq) ? a.Sk : a.Sq;          // rows that see at least one key
-  const long long items = ((static_cast<long long>(sq_eff) + 255) / 256) * a.B * a.Hq;
+  const long long items = ((static_cast<long long>(sq_eff) + 127) / 128) * a.B * a.Hq;
   const int nkv = (a.Sk + 127) / 128;
   int n = want;
   if (n == 0) {
@@ -384,7 +323,7 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   }
   const int causal_off = causal ? a.Sk - a.Sq : 0;     // >= 0 from here on
 
-  const long long npairs = (static_cast<long long>(a.Sq) + 255) / 256;
+  const long long npairs = (static_cast<long long>(a.Sq) + 127) / 128;
   const int nkv_total = (a.Sk + 127) / 128;
   const int split_tiles = (nkv_total + nsplit - 1) / nsplit;
 
@@ -393,16 +332,7 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
   if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
 
-  const int variant = variant_for(a.D, causal, a.Sq, a.Sk, a.B, a.Hq, nsplit, num_sms(), n_extra);
-  // output tensor maps of the persistent kernels' TMA-store epilogue (16-bit output only): [0] = out, [1..] = peers
-  tfa::OutMaps to;
-  std::memset(&to, 0, sizeof(to));
-  if (variant >= KV_PERSIST && !f32 && nsplit == 1) {
-    const int bc = 64;       // store box: 32 rows x 64 columns (SWIZZLE_128B)
-    if ((rc = make_tmap(&to.m[0], a.out, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, 32, bc))) return rc;
-    for (int i = 0; i < n_extra; ++i)
-      if ((rc = make_tmap(&to.m[1 + i], extra_dst[i], a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, 32, bc))) return rc;
-  }
+  const int variant = variant_for(causal, a.Sq, n_extra);
 
   const long long rows = static_cast<long long>(a.B) * a.Hq * a.Sq;
   float* ws_o = static_cast<float*>(a.ws);
@@ -449,16 +379,13 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
   p.n_extra_dst = n_extra;
   p.dbg = g_dbg_dev;
-  p.trace = g_trace_buf;
-  p.trace_block = g_trace_block;
 
   const long long nitems = npairs * a.B * a.Hq * nsplit;
   if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
   p.total_items = static_cast<int>(nitems);
-  p.sched_counter = nullptr;
   const bool kernel_f32 = f32 || nsplit > 1;
-  if (a.D == 64) rc = dispatch<64>(causal, bf16, kernel_f32, tq, tk, tv, to, p, nitems, variant, stream);
-  else           rc = dispatch<128>(causal, bf16, kernel_f32, tq, tk, tv, to, p, nitems, variant, stream);
+  if (a.D == 64) rc = dispatch<64>(causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
+  else           rc = dispatch<128>(causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
   if (rc) return rc;
 
   if (nsplit > 1) {
@@ -651,9 +578,11 @@ void tfa_host_release(void) {
 unsigned long long tfa_launch_count(void) { return g_launches.load(); }
 // development aid (not in the public header): which kernel the last forward launch used (0 classic, 4 persistent)
 int tfa_internal_last_variant(void) { return g_last_variant.load(); }
-// development aid (not in the public header): the kernel-selection rule as a host function (no device needed)
+// development aid (not in the public header): the kernel-selection rule as a host function (no device needed); it
+// takes the whole problem shape, of which the rule reads the mask, the query length and the exchange
 int tfa_internal_choose_kernel(int D, int causal, int Sq, int Sk, int B, int Hq, int nsplit, int sms, int n_extra) {
-  return variant_for(D, causal != 0, Sq, Sk, B, Hq, nsplit < 1 ? 1 : nsplit, sms, n_extra);
+  (void)D; (void)Sk; (void)B; (void)Hq; (void)nsplit; (void)sms;
+  return variant_for(causal != 0, Sq, n_extra);
 }
 // exported for the self tests living in another translation unit
 void tfa_internal_count_launch(void) { g_launches.fetch_add(1, std::memory_order_relaxed); }
@@ -666,12 +595,6 @@ int tfa_internal_decode_work(int block, int npairs, int nsplit, int head_chunk, 
   tfa::decode_work(block, npairs, nsplit, head_chunk, BH, bh, split, pr);
   out3[0] = bh; out3[1] = split; out3[2] = pr;
   return 0;
-}
-
-// development aid (not in the public header): timeline buffer for -DTFA_TRACE variant builds
-void tfa_internal_set_trace(void* dev_buf, int block) {
-  g_trace_buf = static_cast<unsigned long long*>(dev_buf);
-  g_trace_block = block;
 }
 
 int tfa_debug_record(unsigned int out[8]) {
@@ -689,11 +612,11 @@ const char* tfa_error_string(int code) {
     case 0: return "success";
     case TFA_EINVAL_PTR: return "tfa: null or misaligned (16 B) pointer";
     case TFA_EINVAL_DIM: return "tfa: head_dim must be 64 or 128";
-    case TFA_EINVAL_SHAPE: return "tfa: B, H, S must be >= 1 (and B*H*ceil(S/256) < 2^30); fused exchange needs the square MHA problem";
+    case TFA_EINVAL_SHAPE: return "tfa: B, H, S must be >= 1 (and B*H*ceil(S/128) < 2^30); fused exchange needs the square MHA problem";
     case TFA_EINVAL_DTYPE: return "tfa: dtype must be TFA_BF16 (0) or TFA_FP16 (1)";
     case TFA_EINVAL_STRIDE: return "tfa: strides must be multiples of 8 elements with unit head_dim stride";
     case TFA_EDRIVER: return "tfa: cuTensorMapEncodeTiled unavailable or failed";
-    case TFA_EARCH: return "tfa: this library only runs on compute capability 10.x (B200, sm_100a)";
+    case TFA_EARCH: return "tfa: this library only runs on compute capability 9.0 (H100, sm_90a)";
     case TFA_EDEVICE_FAULT: return "tfa: kernel watchdog fired (see tfa_debug_record)";
     case TFA_EINVAL_SCALE: return "tfa: softmax_scale must be finite and >= 0";
     case TFA_EINVAL_HEADS: return "tfa: query heads must be a multiple of K/V heads";

@@ -1,9 +1,9 @@
 // tfa_selftest.cu -- bring-up kernels for the primitives the forward kernel is built from.
 // One tiny CTA each; the host side (tests/test_umma_primitives.py) checks the raw results.
-// They exist because descriptor conventions (swizzle, LBO/SBO, TMEM operand packing) cannot be
+// They exist because descriptor conventions (swizzle, LBO/SBO, register fragment packing) cannot be
 // verified without hardware, and a wrong guess inside the big kernel is much harder to localise.
 #include "../../include/tfa_b200.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 #include <cudaTypedefs.h>
 #include <cstring>
@@ -33,107 +33,85 @@ selftest_tma_kernel(const __grid_constant__ CUtensorMap tm, int x0, int y0, int 
   for (int i = threadIdx.x; i < 1024; i += 128) dump[i] = reinterpret_cast<const uint4*>(smem)[i];
 }
 
-struct UmmaTestParams {
-  int N, K, mode, fmt;
-  uint32_t lbo_a, sbo_a, lbo_b, sbo_b, kstep_a, kstep_b, slab_a, slab_b, flags;
+struct MmaTestParams {
+  int N, K, mode;
+  uint32_t lbo_b, sbo_b, kstep_b, slab_a, slab_b, flags;
   const uint16_t* a_gmem;   // mode 2: A read by threads
   float* c;
   DebugRecord* dbg;
 };
 
-// A: 128 x K.  smem A (modes 0,1): K/64 slabs of [128 rows x 128 B].
+// C(128 x N) = A(128 x K) * B as two m64 halves, one warpgroup.
+// A: 128 x K.  smem A (modes 0,1): K/64 slabs of [128 rows x 128 B]; mode 2: registers, loaded from global.
 // B mode 0: N x K K-major : K/64 slabs of [N rows x 128 B].
 // B mode 1/2: K x N MN-major: N/64 slabs of [K rows x 128 B].
+template <int N, bool IS_BF16>
 __global__ void __launch_bounds__(128, 1)
-selftest_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                     const UmmaTestParams p) {
+selftest_mma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const MmaTestParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;             // up to 32 KB
   uint8_t* sB = smem + 32768;     // up to 32 KB
   uint64_t* bar_ld = reinterpret_cast<uint64_t*>(smem + 65536);
-  uint64_t* bar_mma = bar_ld + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_ld + 2);
-  const int warp = threadIdx.x >> 5;
+  const int wq = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_ld, 1);
-    mbar_init(bar_mma, 1);
     fence_mbar_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-  const int r = threadIdx.x;
-
-  // TMEM map: C accumulator at columns [0, N); packed A (mode 2) at columns [128, 128 + K/2)
-  if (p.mode == 2) {
-    // each thread packs its own row of A into TMEM, two 16-bit values per 32-bit column
-    for (int c0 = 0; c0 < p.K / 2; c0 += 16) {
-      uint32_t pk[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const uint32_t lo = p.a_gmem[r * p.K + 2 * (c0 + i)];
-        const uint32_t hi = p.a_gmem[r * p.K + 2 * (c0 + i) + 1];
-        pk[i] = (p.flags & 1u) ? ((lo << 16) | hi) : ((hi << 16) | lo);
-      }
-      tmem_st_x16(tmem_base + lane_base + 128 + c0, pk);
-    }
-    tmem_wait_st();
-    tc_fence_before();
-  }
-  __syncthreads();
-
   if (threadIdx.x == 0) {
-    tc_fence_after();
-    const int nslab_b = (p.mode == 0) ? p.K / 64 : p.N / 64;
-    const uint32_t bytes = (p.mode != 2 ? 128 * p.K * 2 : 0) + p.N * p.K * 2;
+    const int nslab_b = (p.mode == 0) ? p.K / 64 : N / 64;
+    const uint32_t bytes = (p.mode != 2 ? 128 * p.K * 2 : 0) + N * p.K * 2;
     mbar_arrive_expect_tx(bar_ld, bytes);
     if (p.mode != 2)
       for (int sl = 0; sl < p.K / 64; ++sl) tma_load_3d(sA + sl * p.slab_a, &tmA, bar_ld, sl * 64, 0, 0);
     for (int sl = 0; sl < nslab_b; ++sl) tma_load_3d(sB + sl * p.slab_b, &tmB, bar_ld, sl * 64, 0, 0);
-    mbar_wait(bar_ld, 0, p.dbg, 101, 0);
-    tc_fence_after();
+  }
+  mbar_wait(bar_ld, 0, p.dbg, 101, 0);
 
-    const uint32_t idesc = umma_idesc_f16(p.fmt, 128, p.N, 0, p.mode == 0 ? 0 : 1);
-    const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
+  const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
+  for (int half = 0; half < 2; ++half) {
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    const int row = half * 64 + wq * 16 + g;      // this thread's rows: row, row + 8
+    reg_fence(d);
+    wgmma_fence();
     for (int k = 0; k < p.K / 16; ++k) {
-      // A (K-major): 4 k-steps of 32 B inside a 128-B slab row, then next slab
-      const uint32_t a_off = (k / 4) * p.slab_a + (k % 4) * p.kstep_a;
       uint32_t b_off;
-      if (p.mode == 0) b_off = (k / 4) * p.slab_b + (k % 4) * p.kstep_b;   // K-major B
-      else b_off = k * p.kstep_b;                                           // MN-major B: 16 rows per k-step
-      const uint64_t bd = umma_smem_desc(b_addr + b_off, p.lbo_b, p.sbo_b);
+      if (p.mode == 0) b_off = (k / 4) * p.slab_b + (k % 4) * p.kstep_b;   // K-major B: 32 B per k-step inside a slab
+      else b_off = k * p.kstep_b;                                          // MN-major B: 16 rows per k-step
+      const uint64_t bd = gmma_desc(b_addr + b_off, p.lbo_b, p.sbo_b);
       if (p.mode == 2) {
-        umma_ts(tmem_base, tmem_base + 128 + k * 8, bd, idesc, k > 0);
+        // A fragment: {row, cols 2tq..+1}, {row+8, same}, {row, cols 2tq+8..+9}, {row+8, same}, 16-bit pairs
+        uint32_t a[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int r = row + (q & 1) * 8, col = 16 * k + 2 * tq + (q >> 1) * 8;
+          const uint32_t lo = p.a_gmem[r * p.K + col], hi = p.a_gmem[r * p.K + col + 1];
+          a[q] = (p.flags & 1u) ? ((lo << 16) | hi) : ((hi << 16) | lo);
+        }
+        Wgmma<N, IS_BF16>::rs(d, a, bd, k > 0);
       } else {
-        const uint64_t ad = umma_smem_desc(a_addr + a_off, p.lbo_a, p.sbo_a);
-        umma_ss(tmem_base, ad, bd, idesc, k > 0);
+        // A (K-major): 4 k-steps of 32 B inside a 128-B slab row, then the next slab; rows [64 half, +64)
+        const uint32_t a_off = half * 64 * 128 + (k / 4) * p.slab_a + (k % 4) * 32;
+        const uint64_t ad = gmma_desc(a_addr + a_off, 16, 1024);
+        if (p.mode == 0) Wgmma<N, IS_BF16>::template ss<0>(d, ad, bd, k > 0);
+        else Wgmma<N, IS_BF16>::template ss<1>(d, ad, bd, k > 0);
       }
     }
-    umma_commit(bar_mma);
-  }
-  __syncwarp();
-  mbar_wait(bar_mma, 0, p.dbg, 102, 0);
-  tc_fence_after();
-  for (int c0 = 0; c0 < p.N; c0 += 32) {
-    uint32_t v[32];
-    tmem_ld_x32(tmem_base + lane_base + c0, v);
-    tmem_wait_ld();
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(d);
 #pragma unroll
-    for (int i = 0; i < 32; ++i) p.c[r * p.N + c0 + i] = __uint_as_float(v[i]);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+    for (int i = 0; i < N / 8; ++i) {
+      p.c[row * N + 8 * i + 2 * tq] = d[4 * i];
+      p.c[row * N + 8 * i + 2 * tq + 1] = d[4 * i + 1];
+      p.c[(row + 8) * N + 8 * i + 2 * tq] = d[4 * i + 2];
+      p.c[(row + 8) * N + 8 * i + 2 * tq + 1] = d[4 * i + 3];
+    }
   }
 }
 
@@ -187,11 +165,10 @@ int tfa_selftest_umma(const void* a, const void* b, float* c, int N, int K, int 
   else rc = encode2d(&tmB, b, dtype, N, K, K);             // (K x N), N contiguous
   if (rc) return rc;
 
-  UmmaTestParams p;
+  MmaTestParams p;
   std::memset(&p, 0, sizeof(p));
-  p.N = N; p.K = K; p.mode = mode; p.fmt = (dtype == TFA_BF16) ? 1 : 0;
+  p.N = N; p.K = K; p.mode = mode;
   p.slab_a = 128 * 128;
-  p.lbo_a = 16; p.sbo_a = 1024; p.kstep_a = 32;
   if (mode == 0) { p.slab_b = N * 128; p.lbo_b = 16; p.sbo_b = 1024; p.kstep_b = 32; }
   else           { p.slab_b = K * 128; p.lbo_b = p.slab_b; p.sbo_b = 1024; p.kstep_b = 2048; }
   if (knobs) {
@@ -204,13 +181,11 @@ int tfa_selftest_umma(const void* a, const void* b, float* c, int N, int K, int 
   p.c = c;
   p.dbg = static_cast<DebugRecord*>(tfa_internal_dbg_dev());
   const int smem = 65536 + 1024 + 64;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(selftest_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    attr_set = true;
-  }
-  selftest_umma_kernel<<<1, 128, smem, static_cast<cudaStream_t>(stream)>>>(tmA, tmB, p);
+  auto kern = (N == 64) ? (dtype == TFA_BF16 ? selftest_mma_kernel<64, true> : selftest_mma_kernel<64, false>)
+                        : (dtype == TFA_BF16 ? selftest_mma_kernel<128, true> : selftest_mma_kernel<128, false>);
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return static_cast<int>(e);
+  kern<<<1, 128, smem, static_cast<cudaStream_t>(stream)>>>(tmA, tmB, p);
   tfa_internal_count_launch();
   return static_cast<int>(cudaGetLastError());
 }

@@ -2,7 +2,7 @@
 
 This is the same stub INTEGRATION.md shows for a reference maintainer.  torch is used only to get
 `data_ptr()` / streams of tensors the caller already owns.  There is NO fallback: if libtfa_b200.so
-is missing or the device is not sm_100, calls raise.
+is missing or the device is not sm_90, calls raise.
 """
 from __future__ import annotations
 
