@@ -51,6 +51,7 @@ extern "C" {
 #define TFA_EINVAL_SCALE  (-9)  /* softmax_scale negative, NaN or infinite         */
 #define TFA_EINVAL_HEADS  (-10) /* Hq not a multiple of Hkv                         */
 #define TFA_EINVAL_WORKSPACE (-11) /* split-KV asked for but workspace missing/small */
+#define TFA_EINVAL_SEQLENS (-12)   /* cu_seqlens null / not 4-byte aligned, or max_seqlen_q not in [1, total_q] */
 
 /* Extended argument block (POD), the analogue of Flash_fwd_params (flash.h:29-60).
  * Strides are in ELEMENTS.  The innermost (head_dim) stride must be 1.
@@ -133,6 +134,48 @@ int tfa_attn_fwd(const tfa_attn_args* args);
 int tfa_attn_num_splits(const tfa_attn_args* args);
 /* Workspace needed for `num_splits` (as returned above): num_splits * B*Hq*Sq * (D + 1) * 4 bytes; 0 for 1. */
 size_t tfa_attn_workspace_bytes(const tfa_attn_args* args, int num_splits);
+
+/* ---- variable-length batch (packed sequences, the flash-attn "varlen" interface) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_varlen_fwd.
+ *
+ *   q        : (total_q, Hq, D) through q_stride_s / q_stride_h (elements, unit head_dim stride)
+ *   k, v     : (total_k, Hkv, D) through kv_stride_s / kv_stride_h;  Hq % Hkv == 0.  The strides let q, k and v
+ *              be views of one packed (total, 3, H, D) tensor.
+ *   out      : (total_q, Hq, D) contiguous, dtype of q, or fp32 when out_fp32 != 0
+ *   lse      : (Hq, total_q) contiguous fp32, natural log; may be NULL
+ *   cu_seqlens_q, cu_seqlens_k : int32 DEVICE arrays of B + 1 entries, cu[0] = 0, non-decreasing, cu[B] = total.
+ *              Sequence b is rows [cu_q[b], cu_q[b+1]) of q/out and rows [cu_k[b], cu_k[b+1]) of k/v, and is the
+ *              problem tfa_attn_fwd() solves: query head h reads K/V head h / (Hq/Hkv); causal is bottom-right
+ *              aligned, row i sees keys j <= i + (Sk_b - Sq_b).  Rows that see no key (causal Sq_b > Sk_b, or
+ *              Sk_b == 0) get out = 0 and lse = +inf; a sequence with Sq_b == 0 writes nothing.
+ *   total_q, total_k : >= 1.
+ *   max_seqlen_q : >= every Sq_b, in [1, total_q].  The host never reads cu_seqlens: the kernel does, clamping
+ *              every entry to [0, total], so malformed contents cannot make it write outside out and lse.  Rows of
+ *              a sequence beyond its first max_seqlen_q are not computed and keep what out / lse held (as in
+ *              flash-attn).
+ * One kernel launch per call, nothing read back to the host: the call can be captured in a CUDA graph and replayed
+ * with new cu_seqlens contents of the same totals.  No split-KV. */
+typedef struct tfa_attn_varlen_args {
+  const void* q;
+  const void* k;
+  const void* v;
+  void* out;
+  float* lse;
+  const int32_t* cu_seqlens_q;
+  const int32_t* cu_seqlens_k;
+  int32_t B, Hq, Hkv, D;
+  int32_t total_q, total_k, max_seqlen_q;
+  int64_t q_stride_s, q_stride_h;
+  int64_t kv_stride_s, kv_stride_h;
+  int32_t dtype;
+  int32_t is_causal;
+  float softmax_scale;
+  int32_t out_fp32;
+  void* stream;
+} tfa_attn_varlen_args;
+
+int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

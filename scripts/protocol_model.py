@@ -6,7 +6,9 @@ kernel's control flow statement by statement (same barriers, arrival counts, rin
 release points) and yield at every mbarrier wait.  A random scheduler interleaves them; TMA loads complete after random
 delays, and each warpgroup's wgmma groups complete in order after random delays (wgmma.wait_group N returns once at most
 N groups are still in flight).  One CTA walks a list of work items, as the persistent schedule does; a list of one item
-is the one-CTA-per-item schedule.  Shadow state catches what a deadlock-only test would miss:
+is the one-CTA-per-item schedule.  An item with no KV tiles is skipped by the producer; the softmax warpgroups skip it
+too, except for a variable-length item whose rows see no key (`empty`), for which they write O = 0 and LSE = +inf
+without waiting on any barrier.  Shadow state catches what a deadlock-only test would miss:
 
   * a Q buffer or ring slot overwritten by TMA while an issued, unfinished wgmma still reads it,
   * a wgmma that reads a buffer holding the wrong (item, tile) -- a release that came too early or a parity slip,
@@ -34,8 +36,9 @@ class Bar:
 
 
 class Sim:
-    def __init__(self, items, nstage, rng):
+    def __init__(self, items, nstage, rng, empty=()):
         self.items, self.N, self.rng = items, nstage, rng     # items: KV tiles per work item (0 = skipped)
+        self.empty = set(empty)                               # items with 0 tiles whose rows are still written
         self.q_full = Bar("q_full", 1)
         self.q_empty = Bar("q_empty", 2)                      # one arrival per warpgroup (per warp in the kernel)
         self.kv_full = [Bar(f"kv_full{i}", 1) for i in range(nstage)]
@@ -129,6 +132,9 @@ class Sim:
 
         for item, n in enumerate(self.items):
             if n == 0:
+                if item in self.empty:                        # epilogue only: no barrier is touched
+                    yield lambda: True
+                    self.finished[t].append(item)
                 continue
             yield lambda p=qcnt & 1: self.q_full.done(p)
             qcnt += 1
@@ -187,7 +193,7 @@ class Sim:
         else:
             raise AssertionError("did not finish")
         want = [(it, j) for it, n in enumerate(self.items) for j in range(n)]
-        done = [it for it, n in enumerate(self.items) if n > 0]
+        done = [it for it, n in enumerate(self.items) if n > 0 or it in self.empty]
         for t in range(2):
             assert self.seen[t] == want, f"wg{t} consumed {self.seen[t]}, expected {want}"
             assert self.finished[t] == done
@@ -208,11 +214,29 @@ def random_items(rng):
     return items
 
 
+def random_varlen_items(rng):
+    """Items of a variable-length batch: tiles per item, and the items that lie inside their sequence but see no key
+    (causal Sq_b > Sk_b, or Sk_b = 0).  Items past a sequence's end are skipped by every role, like a 0 here."""
+    items, empty = [], []
+    for i in range(rng.randint(1, 12)):
+        kind = rng.random()
+        if kind < 0.3:
+            items.append(0)
+            empty.append(i)
+        elif kind < 0.45:
+            items.append(0)
+        else:
+            items.append(rng.randint(1, 6))
+    return items, empty
+
+
 def main():
     trials = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     for trial in range(trials):
         rng = random.Random(1000003 + trial)
         Sim(random_items(rng), rng.choice([4, 8]), rng).run()
+        items, empty = random_varlen_items(rng)
+        Sim(items, rng.choice([4, 8]), rng, empty).run()
     print(f"{trials} trials: no violation")
 
 

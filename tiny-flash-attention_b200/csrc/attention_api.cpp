@@ -196,6 +196,73 @@ std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Te
   return {out, lse};
 }
 
+// Variable-length batch (the packed cu_seqlens interface of flash-attn's varlen forward): q (total_q, Hq, D),
+// k, v (total_k, Hkv, D), unit head_dim stride (views of one packed (total, 3, H, D) qkv tensor need no copy);
+// cu_seqlens_q / cu_seqlens_k int32 of B + 1 offsets on q's device.  Returns out (total_q, Hq, D) contiguous and
+// lse (Hq, total_q).  max_seqlen_k is not taken: the kernel has no use for it.
+std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Tensor k, torch::Tensor v,
+                                                     torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
+                                                     int64_t max_seqlen_q, bool is_causal, float softmax_scale) {
+  TFA_CHECK_CUDA(q);
+  TFA_CHECK_CUDA(k);
+  TFA_CHECK_CUDA(v);
+  TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3, "q, k, v must have 3 dimensions (total, heads, head_dim)");
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
+              "q, k, v must have the same dtype");
+  TORCH_CHECK(k.sizes() == v.sizes() && k.strides() == v.strides(), "k and v must have identical shapes and strides");
+  TORCH_CHECK(k.size(2) == q.size(2), "k/v must share head_dim with q");
+  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
+  TORCH_CHECK(q.stride(2) == 1 && k.stride(2) == 1, "q, k, v must have a unit head_dim stride");
+  TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt && cu_seqlens_k.scalar_type() == at::kInt,
+              "cu_seqlens_q and cu_seqlens_k must be int32");
+  TORCH_CHECK(cu_seqlens_q.device() == q.device() && cu_seqlens_k.device() == q.device(),
+              "cu_seqlens_q and cu_seqlens_k must be on q's device");
+  TORCH_CHECK(cu_seqlens_q.dim() == 1 && cu_seqlens_q.is_contiguous() && cu_seqlens_k.dim() == 1 &&
+                  cu_seqlens_k.is_contiguous(),
+              "cu_seqlens_q and cu_seqlens_k must be contiguous 1-D tensors");
+  TORCH_CHECK(cu_seqlens_q.numel() >= 2 && cu_seqlens_k.numel() == cu_seqlens_q.numel(),
+              fmt_msg("cu_seqlens_q and cu_seqlens_k must both hold B + 1 >= 2 offsets, got %lld and %lld",
+                      static_cast<long long>(cu_seqlens_q.numel()), static_cast<long long>(cu_seqlens_k.numel())));
+  const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2), total_k = k.size(0), Hkv = k.size(1);
+  const int64_t B = cu_seqlens_q.numel() - 1;
+  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
+  TORCH_CHECK(total_q >= 1 && total_k >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
+  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(max_seqlen_q >= 1 && max_seqlen_q <= total_q,
+              fmt_msg("max_seqlen_q must be in [1, total_q = %lld], got %lld", static_cast<long long>(total_q),
+                      static_cast<long long>(max_seqlen_q)));
+  TORCH_CHECK(total_q < (1LL << 31) && total_k < (1LL << 31) && B < (1LL << 31), "tensors too large");
+
+  torch::Tensor out, lse;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    out = torch::empty({total_q, Hq, D}, q.options());
+    lse = torch::empty({Hq, total_q}, q.options().dtype(at::kFloat));
+    tfa_attn_varlen_args a;
+    a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.cu_seqlens_q = cu_seqlens_q.data_ptr<int32_t>();
+    a.cu_seqlens_k = cu_seqlens_k.data_ptr<int32_t>();
+    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
+    a.D = static_cast<int32_t>(D);
+    a.total_q = static_cast<int32_t>(total_q); a.total_k = static_cast<int32_t>(total_k);
+    a.max_seqlen_q = static_cast<int32_t>(max_seqlen_q);
+    a.q_stride_s = q.stride(0); a.q_stride_h = q.stride(1);
+    a.kv_stride_s = k.stride(0); a.kv_stride_h = k.stride(1);
+    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.out_fp32 = 0;
+    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    rc = tfa_attn_varlen_fwd(&a);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_cutlass", &flash_attention_v2_cutlass,
         "Flash attention v2 forward, H100-native (sm_90a wgmma/TMA)");
@@ -205,6 +272,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_fp32out", &flash_attention_v2_fp32out, "same op, fp32 output (validation)");
   m.def("flash_attention_v2_general", &flash_attention_v2_general,
         "grouped K/V heads, Sq != Sk (bottom-right causal), optional split-KV: (q, k, v, is_causal, scale, num_splits)");
+  m.def("flash_attention_v2_varlen", &flash_attention_v2_varlen,
+        "packed variable-length batch: (q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, scale)");
   m.def("launch_count", []() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

@@ -31,6 +31,7 @@
 // gives its registers to the others), warpgroups 1 and 2 run Q tile 0 and 1: wgmma, softmax, epilogue.
 // PERSIST = false: one CTA per work item.  PERSIST = true: one CTA per SM walks the items blockIdx.x, +gridDim.x, ...
 // and its producer runs ahead into the next item's Q and K/V while the softmax warpgroups finish the current one.
+// VARLEN = true: a packed variable-length batch; each item reads its sequence's offsets and lengths from cu_seqlens.
 #pragma once
 #include "ptx_sm90.cuh"
 
@@ -67,6 +68,12 @@ struct FwdParams {
   float scale;        // softmax_scale
   float scale_log2;   // softmax_scale * log2(e)
   DebugRecord* dbg;
+  // Variable length (VARLEN = true): batch entry b is the problem of rows [cu_q[b], cu_q[b+1]) of the packed q/out
+  // and rows [cu_k[b], cu_k[b+1]) of the packed k/v; S is max_seqlen_q and Sk / causal_off are unused.  The arrays are
+  // device memory, read by the kernel only; lse is (H, total_q).
+  const int* cu_q;
+  const int* cu_k;
+  int total_q, total_k;
 };
 
 template <int D>
@@ -116,10 +123,15 @@ __host__ __device__ __forceinline__ void decode_work(int block, int npairs, int 
 }
 
 // One work item: both Q tiles walk the same KV tiles [jb, jb + n); rows a tile does not see are masked.
+// q0 / k0 are the sequence's first row in the (packed) q and k/v tensors, Sq / Sk / coff its own lengths and causal
+// offset: the whole tensor's (q0 = k0 = 0) unless VARLEN.  `live`: the item has rows to write.  The producer loads an
+// item iff n > 0, the softmax warpgroups wait on its barriers iff n > 0: n > 0 implies live.
 struct Item {
   int bh, bidx, hidx, hkv, split, jb, row0, n;
+  int q0, k0, Sq, Sk, coff;
+  bool live;
 };
-template <bool CAUSAL>
+template <bool CAUSAL, bool VARLEN>
 __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   Item w;
   int pr;
@@ -129,14 +141,37 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   w.hkv = w.hidx / p.kv_group;
   w.row0 = pr * 128;
   w.jb = w.split * p.split_tiles;
-  const int nkv_total = (p.Sk + 127) >> 7;
-  // causal: the item's last row sees keys <= row0 + 127 + causal_off
-  const int nfull = CAUSAL ? min(nkv_total, (w.row0 + 127 + p.causal_off) / 128 + 1) : nkv_total;
+  if constexpr (VARLEN) {
+    // clamped to the packed tensors: whatever cu_seqlens holds, no row outside [0, total) is read or written
+    const int q0 = min(max(__ldg(p.cu_q + w.bidx), 0), p.total_q);
+    const int q1 = min(max(__ldg(p.cu_q + w.bidx + 1), 0), p.total_q);
+    const int k0 = min(max(__ldg(p.cu_k + w.bidx), 0), p.total_k);
+    const int k1 = min(max(__ldg(p.cu_k + w.bidx + 1), 0), p.total_k);
+    w.q0 = q0;
+    w.k0 = k0;
+    w.Sq = max(q1 - q0, 0);
+    w.Sk = max(k1 - k0, 0);
+    w.coff = w.Sk - w.Sq;           // may be negative: the sequence's first rows see no key
+  } else {
+    w.q0 = 0;
+    w.k0 = 0;
+    w.Sq = p.S;
+    w.Sk = p.Sk;
+    w.coff = p.causal_off;
+  }
+  const int nkv_total = (w.Sk + 127) >> 7;
+  // causal: the item's last row sees keys <= last (none when last < 0, which only a varlen sequence can have)
+  const int last = w.row0 + 127 + w.coff;
+  const int nfull = CAUSAL ? ((VARLEN && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
   w.n = max(0, min(nfull - w.jb, p.split_tiles));   // 0: a split-KV item wholly above the causal diagonal
+  // dense: an item without tiles writes nothing (its rows belong to other splits); varlen: an item inside its sequence
+  // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0)
+  w.live = VARLEN ? w.row0 < w.Sq : w.n > 0;
+  if (VARLEN && !w.live) w.n = 0;    // past the sequence's end: the producer must skip it as the consumers do
   return w;
 }
 
-template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST>
+template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST, bool VARLEN>
 __global__ void __launch_bounds__(384, 1)
 fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
@@ -160,7 +195,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int lane = threadIdx.x & 31;
   const int first = static_cast<int>(blockIdx.x);
   const int stride = PERSIST ? static_cast<int>(gridDim.x) : p.total_items;
-  if (!PERSIST && decode_item<CAUSAL>(first, p).n == 0) return;   // CTA-uniform
+  if (!PERSIST && !decode_item<CAUSAL, VARLEN>(first, p).live) return;   // CTA-uniform
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -183,14 +218,17 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       uint32_t ent = 0;      // running K/V ring entry (K_j and V_j of every item in turn; never reset between items)
       uint32_t qcnt = 0;     // items loaded
       for (int item = first; item < p.total_items; item += stride) {
-        const Item w = decode_item<CAUSAL>(item, p);
+        const Item w = decode_item<CAUSAL, VARLEN>(item, p);
         if (w.n == 0) continue;
         if (qcnt > 0) mbar_wait(q_empty, (qcnt - 1) & 1, p.dbg, SITE_LOAD_Q, qcnt);
         ++qcnt;
         mbar_arrive_expect_tx(q_full, TILE);
+        // varlen: the packed tensors are one batch entry; rows of the next sequence a box takes in are never stored
+        // (queries) or masked (keys)
+        const int wz = VARLEN ? 0 : w.bidx;
 #pragma unroll
         for (int sl = 0; sl < C::SLABS; ++sl)
-          tma_load_4d(sQ + sl * C::SLAB_BYTES, &tmQ, q_full, sl * 64, w.row0, w.hidx, w.bidx);
+          tma_load_4d(sQ + sl * C::SLAB_BYTES, &tmQ, q_full, sl * 64, w.q0 + w.row0, w.hidx, wz);
         for (int j = 0; j < w.n; ++j) {
 #pragma unroll
           for (int kv = 0; kv < 2; ++kv, ++ent) {
@@ -200,8 +238,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             const CUtensorMap* tm = kv ? &tmV : &tmK;
 #pragma unroll
             for (int sl = 0; sl < C::SLABS; ++sl)
-              tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64, (w.jb + j) * C::BN,
-                          w.hkv, w.bidx);
+              tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64,
+                          w.k0 + (w.jb + j) * C::BN, w.hkv, wz);
           }
         }
       }
@@ -218,19 +256,17 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int g = lane >> 2, tq = lane & 3;        // this thread: rows 16 wq + g and + 8, columns 8 i + 2 tq (+1)
   const int r_lo = t * 64 + wq * 16 + g;         // row inside the item (0..127); r_hi = r_lo + 8
   const float c = p.scale_log2;
-  const int S = p.S, Sk = p.Sk;
   const uint32_t sQ_addr = smem_u32(sQ) + t * 64 * 128;   // this tile's rows inside each slab
   const uint32_t sKV_addr = smem_u32(sKV);
 
   uint32_t ent = 0;        // K/V ring entry of K_0 of the current item (same sequence as the producer's)
   uint32_t qcnt = 0;
   for (int item = first; item < p.total_items; item += stride) {
-    const Item w = decode_item<CAUSAL>(item, p);
+    const Item w = decode_item<CAUSAL, VARLEN>(item, p);
     const int n = w.n;
-    if (n == 0) continue;
-    const int row_lo = w.row0 + r_lo, row_hi = row_lo + 8;    // global query rows
-    mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
-    ++qcnt;
+    if (!w.live) continue;
+    const int S = w.Sq, Sk = w.Sk, coff = w.coff;
+    const int row_lo = w.row0 + r_lo, row_hi = row_lo + 8;    // query rows of the sequence
 
     // S = Q K^T over D/16 k-steps; K-major operands advance 32 B per k-step inside a slab, one slab per 4 k-steps
     auto issue_S = [&](float* s, uint32_t kslot) {
@@ -267,10 +303,10 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     // returns alpha for (lo, hi) when O must be rescaled (rare), else {1, 1}
     auto softmax = [&](int j, bool& rescale, float& a_lo, float& a_hi) {
       const int col0 = (w.jb + j) * C::BN;
-      const bool edge = (col0 + C::BN > Sk) || (CAUSAL && col0 + C::BN - 1 > w.row0 + t * 64 + p.causal_off);
+      const bool edge = (col0 + C::BN > Sk) || (CAUSAL && col0 + C::BN - 1 > w.row0 + t * 64 + coff);
       if (edge) {     // tiles crossing the causal diagonal or the end of the keys (warpgroup-uniform)
-        const int lim_lo = (CAUSAL ? min(Sk, row_lo + p.causal_off + 1) : Sk) - col0;
-        const int lim_hi = (CAUSAL ? min(Sk, row_hi + p.causal_off + 1) : Sk) - col0;
+        const int lim_lo = (CAUSAL ? min(Sk, row_lo + coff + 1) : Sk) - col0;
+        const int lim_hi = (CAUSAL ? min(Sk, row_hi + coff + 1) : Sk) - col0;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
 #pragma unroll
@@ -331,59 +367,64 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
     };
 
-    // ---- KV tile 0 ----
-    {
-      const uint32_t kslot = ent % NSTAGE;
-      mbar_wait(&kv_full[kslot], (ent / NSTAGE) & 1, p.dbg, SITE_MMA_K, ent);
-      wgmma_fence();
-      issue_S(s, kslot);
-      wgmma_wait<0>();
-      reg_fence(s);
-      release(&kv_empty[kslot]);
-      if (n == 1) release(q_empty);
-      bool rs;
-      float a0, a1;
-      softmax(0, rs, a0, a1);
-      pack_P();
-    }
-    // ---- KV tiles 1 .. n-1: S_j and PV_{j-1} in flight together ----
-    for (int j = 1; j < n; ++j) {
-      const uint32_t ek = ent + 2 * j, ev = ent + 2 * j - 1;
-      const uint32_t kslot = ek % NSTAGE, vslot = ev % NSTAGE;
-      mbar_wait(&kv_full[kslot], (ek / NSTAGE) & 1, p.dbg, SITE_MMA_K, ek);
-      wgmma_fence();
-      issue_S(s, kslot);
-      mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
-      issue_PV(o, pf, vslot, j > 1);
-      wgmma_wait<1>();                               // S_j done
-      reg_fence(s);
-      release(&kv_empty[kslot]);
-      if (j == n - 1) release(q_empty);
-      bool rs;
-      float a_lo, a_hi;
-      softmax(j, rs, a_lo, a_hi);
-      wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
-      reg_fence(o);
-      release(&kv_empty[vslot]);
-      if (rs) {
-#pragma unroll
-        for (int i = 0; i < D / 8; ++i) {
-          o[4 * i + 0] *= a_lo; o[4 * i + 1] *= a_lo;
-          o[4 * i + 2] *= a_hi; o[4 * i + 3] *= a_hi;
-        }
+    // A varlen item whose rows all see no key has no tiles: it waits on no barrier, its rows get O = 0, LSE = +inf.
+    if (!VARLEN || n > 0) {
+      mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
+      ++qcnt;
+      // ---- KV tile 0 ----
+      {
+        const uint32_t kslot = ent % NSTAGE;
+        mbar_wait(&kv_full[kslot], (ent / NSTAGE) & 1, p.dbg, SITE_MMA_K, ent);
+        wgmma_fence();
+        issue_S(s, kslot);
+        wgmma_wait<0>();
+        reg_fence(s);
+        release(&kv_empty[kslot]);
+        if (n == 1) release(q_empty);
+        bool rs;
+        float a0, a1;
+        softmax(0, rs, a0, a1);
+        pack_P();
       }
-      pack_P();
+      // ---- KV tiles 1 .. n-1: S_j and PV_{j-1} in flight together ----
+      for (int j = 1; j < n; ++j) {
+        const uint32_t ek = ent + 2 * j, ev = ent + 2 * j - 1;
+        const uint32_t kslot = ek % NSTAGE, vslot = ev % NSTAGE;
+        mbar_wait(&kv_full[kslot], (ek / NSTAGE) & 1, p.dbg, SITE_MMA_K, ek);
+        wgmma_fence();
+        issue_S(s, kslot);
+        mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        issue_PV(o, pf, vslot, j > 1);
+        wgmma_wait<1>();                               // S_j done
+        reg_fence(s);
+        release(&kv_empty[kslot]);
+        if (j == n - 1) release(q_empty);
+        bool rs;
+        float a_lo, a_hi;
+        softmax(j, rs, a_lo, a_hi);
+        wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
+        reg_fence(o);
+        release(&kv_empty[vslot]);
+        if (rs) {
+#pragma unroll
+          for (int i = 0; i < D / 8; ++i) {
+            o[4 * i + 0] *= a_lo; o[4 * i + 1] *= a_lo;
+            o[4 * i + 2] *= a_hi; o[4 * i + 3] *= a_hi;
+          }
+        }
+        pack_P();
+      }
+      {
+        const uint32_t ev = ent + 2 * n - 1, vslot = ev % NSTAGE;
+        mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        wgmma_fence();
+        issue_PV(o, pf, vslot, n > 1);
+        wgmma_wait<0>();
+        reg_fence(o);
+        release(&kv_empty[vslot]);
+      }
+      ent += 2 * n;
     }
-    {
-      const uint32_t ev = ent + 2 * n - 1, vslot = ev % NSTAGE;
-      mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
-      wgmma_fence();
-      issue_PV(o, pf, vslot, n > 1);
-      wgmma_wait<0>();
-      reg_fence(o);
-      release(&kv_empty[vslot]);
-    }
-    ent += 2 * n;
 
     // ---------------------------- epilogue ----------------------------
 #pragma unroll
@@ -393,11 +434,21 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
     const float inv_lo = (l_lo > 0.f) ? 1.0f / l_lo : 0.f;
     const float inv_hi = (l_hi > 0.f) ? 1.0f / l_hi : 0.f;
-    const long long tile_off = static_cast<long long>(w.bidx) * p.o_stride_b + static_cast<long long>(w.hidx) * p.o_stride_h;
+    const long long tile_off =
+        (VARLEN ? static_cast<long long>(w.q0) * p.o_stride_s : static_cast<long long>(w.bidx) * p.o_stride_b) +
+        static_cast<long long>(w.hidx) * p.o_stride_h;
     if (p.lse != nullptr && tq == 0) {
-      float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
-      if (row_lo < S) lrow[row_lo] = m_lo * p.scale + logf(l_lo);
-      if (row_hi < S) lrow[row_hi] = m_hi * p.scale + logf(l_hi);
+      if constexpr (VARLEN) {
+        // (H, total_q); a row that saw no key (l == 0) gets +inf.  Not for split-KV partials, whose -inf tells the
+        // combine that the split holds nothing.
+        float* lrow = p.lse + static_cast<long long>(w.hidx) * p.lse_stride_bh + w.q0;
+        if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : INFINITY;
+        if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : INFINITY;
+      } else {
+        float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
+        if (row_lo < S) lrow[row_lo] = m_lo * p.scale + logf(l_lo);
+        if (row_hi < S) lrow[row_hi] = m_hi * p.scale + logf(l_hi);
+      }
     }
 
     if constexpr (OUT_F32) {

@@ -142,7 +142,7 @@ cudaError_t opt_in_smem(K kernel, int bytes) {
   return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
 
-template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32>
+template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool VARLEN>
 int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
                 int variant, cudaStream_t stream) {
   cudaError_t cerr = cudaSuccess;
@@ -152,11 +152,11 @@ int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
     const int sms = num_sms();
     if (sms <= 0) return TFA_EARCH;
     if (nblocks > sms) nblocks = sms;                                   // one CTA per SM
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true>;
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, VARLEN>;
     if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
     kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   } else {
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false>;
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, VARLEN>;
     if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
     kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   }
@@ -164,10 +164,10 @@ int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
   return static_cast<int>(cudaGetLastError());
 }
 
-template <int D>
+template <int D, bool VARLEN>
 int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
              const FwdParams& p, long long nblocks, int variant, cudaStream_t s) {
-#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_>(tq, tk, tv, p, nblocks, variant, s)
+#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_, VARLEN>(tq, tk, tv, p, nblocks, variant, s)
   if (causal) {
     if (bf16) { if (f32) TFA_GO(true, true, true); else TFA_GO(true, true, false); }
     else      { if (f32) TFA_GO(true, false, true); else TFA_GO(true, false, false); }
@@ -176,6 +176,33 @@ int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUte
     else      { if (f32) TFA_GO(false, false, true); else TFA_GO(false, false, false); }
   }
 #undef TFA_GO
+}
+
+// The kernel parameters every forward sets the same way: heads, work-item order, softmax scale, watchdog.
+FwdParams base_params(int Hq, int Hkv, long long npairs, int BH, float scale) {
+  FwdParams p;
+  std::memset(&p, 0, sizeof(p));
+  p.H = Hq;
+  p.kv_group = Hq / Hkv;
+  p.npairs = static_cast<int>(npairs);
+  p.BH = BH;
+  p.head_chunk = p.BH < 8 ? p.BH : 8;
+  p.scale = scale;
+  // scale == 0 is legal (uniform attention over the visible keys): a tiny positive exponent scale keeps
+  // masked scores at -inf (0 * -inf would be NaN) while every visible score still maps to exp2(0) = 1
+  p.scale_log2 = fmaxf(scale * 1.4426950408889634f, 1.0e-30f);
+  p.dbg = g_dbg_dev;
+  return p;
+}
+
+// One forward kernel launch over `nitems` work items.
+template <bool VARLEN>
+int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
+               const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
+  if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
+  p.total_items = static_cast<int>(nitems);
+  if (D == 64) return dispatch<64, VARLEN>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+  return dispatch<128, VARLEN>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
 }
 
 bool arch_ok() {
@@ -338,22 +365,12 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   float* ws_o = static_cast<float*>(a.ws);
   float* ws_lse = ws_o ? ws_o + static_cast<size_t>(nsplit) * rows * a.D : nullptr;
 
-  FwdParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.H = a.Hq;
+  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
   p.S = a.Sq;
   p.Sk = a.Sk;
   p.causal_off = causal_off;
-  p.kv_group = a.Hq / a.Hkv;
-  p.npairs = static_cast<int>(npairs);
   p.nsplit = nsplit;
   p.split_tiles = split_tiles;
-  p.BH = a.B * a.Hq;
-  p.head_chunk = p.BH < 8 ? p.BH : 8;
-  p.scale = a.scale;
-  // scale == 0 is legal (uniform attention over the visible keys): a tiny positive exponent scale keeps
-  // masked scores at -inf (0 * -inf would be NaN) while every visible score still maps to exp2(0) = 1
-  p.scale_log2 = fmaxf(a.scale * 1.4426950408889634f, 1.0e-30f);
   if (nsplit > 1) {
     // partials: contiguous (B, Hq, Sq, D) fp32 per split, normalised, with their LSEs
     p.out = nullptr;
@@ -378,14 +395,10 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   }
   for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
   p.n_extra_dst = n_extra;
-  p.dbg = g_dbg_dev;
 
   const long long nitems = npairs * a.B * a.Hq * nsplit;
-  if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
-  p.total_items = static_cast<int>(nitems);
   const bool kernel_f32 = f32 || nsplit > 1;
-  if (a.D == 64) rc = dispatch<64>(causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
-  else           rc = dispatch<128>(causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
+  rc = launch_fwd<false>(a.D, causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
   if (rc) return rc;
 
   if (nsplit > 1) {
@@ -430,6 +443,57 @@ Problem from_attn_args(const tfa_attn_args& a) {
   return q;
 }
 
+// The packed tensors as one batch entry of total_q query rows and total_k keys (what validate() checks of them).
+Problem from_varlen_args(const tfa_attn_varlen_args& a) {
+  Problem q;
+  q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
+  q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.Sk = a.total_k; q.D = a.D;
+  q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.ksb = 0; q.ksh = a.kv_stride_h; q.kss = a.kv_stride_s;
+  q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
+  q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
+  q.stream = static_cast<cudaStream_t>(a.stream);
+  return q;
+}
+
+int varlen_impl(const tfa_attn_varlen_args& va) {
+  const Problem a = from_varlen_args(va);
+  int rc = validate(a);
+  if (rc) return rc;
+  if (!va.cu_seqlens_q || !va.cu_seqlens_k ||
+      ((reinterpret_cast<uintptr_t>(va.cu_seqlens_q) | reinterpret_cast<uintptr_t>(va.cu_seqlens_k)) & 3u))
+    return TFA_EINVAL_SEQLENS;
+  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
+  if (!arch_ok()) return TFA_EARCH;
+  init_dbg();
+  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
+
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
+  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
+  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
+
+  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once
+  const long long npairs = (static_cast<long long>(va.max_seqlen_q) + 127) / 128;
+  const int variant = choose_kernel(causal, npairs, 0);
+
+  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
+  p.S = va.max_seqlen_q;
+  p.nsplit = 1;
+  p.split_tiles = 0x7fffffff;          // one split holds every KV tile of any sequence
+  p.out = f32 ? nullptr : a.out;
+  p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
+  p.lse = a.lse;
+  p.o_stride_s = static_cast<long long>(a.Hq) * a.D;     // out is (total_q, Hq, D) contiguous
+  p.o_stride_h = a.D;
+  p.lse_stride_bh = a.Sq;                                // lse is (Hq, total_q)
+  p.cu_q = va.cu_seqlens_q;
+  p.cu_k = va.cu_seqlens_k;
+  p.total_q = a.Sq;
+  p.total_k = a.Sk;
+  return launch_fwd<true>(a.D, causal, bf16, f32, tq, tk, tv, p, npairs * a.B * a.Hq, variant, a.stream);
+}
+
 // ---- host-buffer path workspace ----
 struct HostWs {
   void* d[4] = {nullptr, nullptr, nullptr, nullptr};   // q k v o
@@ -464,6 +528,11 @@ int tfa_fwd_ex(const tfa_fwd_args* args) {
 int tfa_attn_fwd(const tfa_attn_args* args) {
   if (!args) return TFA_EINVAL_PTR;
   return fwd_impl(from_attn_args(*args));
+}
+
+int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
+  if (!args) return TFA_EINVAL_PTR;
+  return varlen_impl(*args);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -621,6 +690,8 @@ const char* tfa_error_string(int code) {
     case TFA_EINVAL_SCALE: return "tfa: softmax_scale must be finite and >= 0";
     case TFA_EINVAL_HEADS: return "tfa: query heads must be a multiple of K/V heads";
     case TFA_EINVAL_WORKSPACE: return "tfa: split-KV needs a 16-byte aligned workspace of tfa_attn_workspace_bytes()";
+    case TFA_EINVAL_SEQLENS:
+      return "tfa: cu_seqlens must be non-null 4-byte aligned device pointers and max_seqlen_q in [1, total_q]";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "tfa: unknown error";
   }
 }

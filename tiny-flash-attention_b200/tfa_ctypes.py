@@ -50,6 +50,20 @@ class AttnArgs(ctypes.Structure):
     ]
 
 
+class VarlenArgs(ctypes.Structure):
+    """struct tfa_attn_varlen_args (include/tfa_b200.h)."""
+    _fields_ = [
+        ("q", ctypes.c_void_p), ("k", ctypes.c_void_p), ("v", ctypes.c_void_p), ("out", ctypes.c_void_p),
+        ("lse", ctypes.c_void_p), ("cu_seqlens_q", ctypes.c_void_p), ("cu_seqlens_k", ctypes.c_void_p),
+        ("B", ctypes.c_int32), ("Hq", ctypes.c_int32), ("Hkv", ctypes.c_int32), ("D", ctypes.c_int32),
+        ("total_q", ctypes.c_int32), ("total_k", ctypes.c_int32), ("max_seqlen_q", ctypes.c_int32),
+        ("q_stride_s", ctypes.c_int64), ("q_stride_h", ctypes.c_int64),
+        ("kv_stride_s", ctypes.c_int64), ("kv_stride_h", ctypes.c_int64),
+        ("dtype", ctypes.c_int32), ("is_causal", ctypes.c_int32), ("softmax_scale", ctypes.c_float),
+        ("out_fp32", ctypes.c_int32), ("stream", ctypes.c_void_p),
+    ]
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -71,6 +85,8 @@ def lib():
         L.tfa_attn_num_splits.restype = ci
         L.tfa_attn_workspace_bytes.argtypes = [ctypes.POINTER(AttnArgs), ci]
         L.tfa_attn_workspace_bytes.restype = ctypes.c_size_t
+        L.tfa_attn_varlen_fwd.argtypes = [ctypes.POINTER(VarlenArgs)]
+        L.tfa_attn_varlen_fwd.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -158,6 +174,31 @@ def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, st
     check(L.tfa_attn_fwd(ctypes.byref(a)))
     if return_splits:
         return out, lse, n
+    return out, lse
+
+
+def attn_varlen_fwd(q, k, v, cu_q, cu_k, max_seqlen_q, is_causal, scale, out_fp32=False, out=None, lse=None,
+                    stream=None):
+    """Packed variable-length batch through tfa_attn_varlen_fwd(): q (total_q, Hq, D), k/v (total_k, Hkv, D) device
+    tensors with unit head_dim stride (views of a packed qkv tensor are fine; k and v share strides), cu_q / cu_k
+    int32 device tensors of B + 1 offsets.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be
+    given to write into caller-owned buffers."""
+    import torch
+    assert q.is_cuda and q.dim() == 3 and k.dim() == 3 and k.shape == v.shape and k.stride() == v.stride()
+    assert q.stride(2) == 1 and k.stride(2) == 1
+    assert cu_q.dtype == torch.int32 and cu_k.dtype == torch.int32 and cu_q.numel() == cu_k.numel() >= 2
+    total_q, Hq, D = q.shape
+    total_k, Hkv, _ = k.shape
+    if out is None:
+        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+    if lse is None:
+        lse = torch.empty((Hq, total_q), dtype=torch.float32, device=q.device)
+    st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
+    a = VarlenArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), cu_q.data_ptr(),
+                   cu_k.data_ptr(), cu_q.numel() - 1, Hq, Hkv, D, total_q, total_k, int(max_seqlen_q),
+                   q.stride(0), q.stride(1), k.stride(0), k.stride(1), _dtype_code(q), int(bool(is_causal)),
+                   float(scale), int(bool(out_fp32)), st)
+    check(lib().tfa_attn_varlen_fwd(ctypes.byref(a)))
     return out, lse
 
 
