@@ -52,6 +52,9 @@ extern "C" {
 #define TFA_EINVAL_HEADS  (-10) /* Hq not a multiple of Hkv                         */
 #define TFA_EINVAL_WORKSPACE (-11) /* split-KV asked for but workspace missing/small */
 #define TFA_EINVAL_SEQLENS (-12)   /* cu_seqlens null / not 4-byte aligned, or max_seqlen_q not in [1, total_q] */
+#define TFA_EINVAL_KVCACHE (-13)   /* KV cache: cache_seqlens / block_table null or misaligned, page size not a multiple
+                                      of 128, num_blocks or max_blocks_per_seq < 1, one of k_new / v_new, Snew not in
+                                      [1, capacity] */
 
 /* Extended argument block (POD), the analogue of Flash_fwd_params (flash.h:29-60).
  * Strides are in ELEMENTS.  The innermost (head_dim) stride must be 1.
@@ -176,6 +179,63 @@ typedef struct tfa_attn_varlen_args {
 } tfa_attn_varlen_args;
 
 int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args);
+
+/* ---- attention against a (paged) KV cache: the decode step of a serving loop (flash-attn's flash_attn_with_kvcache,
+ * without rotary) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_kvcache_fwd.
+ *
+ *   q, out   : (B, Sq, Hq, D) through q_stride_* (elements, unit head_dim stride); out uses q's strides and is q's
+ *              dtype, or fp32 when out_fp32 != 0.  Sq >= 1: 1 for decode, a few for speculative verification.
+ *   lse      : (B, Hq, Sq) contiguous fp32, natural log; may be NULL
+ *   k_cache, v_cache : (num_blocks, page_block_size, Hkv, D) through cache_stride_* (block, row, head), shared by both;
+ *              Hq % Hkv == 0.
+ *   block_table : int32 DEVICE array (B, max_blocks_per_seq) with row stride block_table_stride: logical page p of
+ *              sequence b is physical block block_table[b * stride + p].  page_block_size must be a multiple of 128.
+ *              NULL: a contiguous cache (B, capacity, Hkv, D) -- pass num_blocks = B, max_blocks_per_seq = 1 and
+ *              page_block_size = capacity (any value >= 1).
+ *   cache_seqlens : int32 DEVICE array (B): keys already cached per sequence.
+ *   k_new, v_new : optional (B, Snew, Hkv, D) through new_stride_* (both or neither).  They are written into the cache
+ *              at keys [L_b, L_b + Snew) before the attention, in place; cache_seqlens is not incremented.
+ *   capacity = max_blocks_per_seq * page_block_size;  L_b = clamp(cache_seqlens[b], 0, capacity - Snew) (Snew = 0
+ *              without k_new).  Sequence b attends to its first K_b = L_b + Snew keys: query head h reads K/V head
+ *              h / (Hq/Hkv), causal is bottom-right aligned (row i sees keys j <= i + K_b - Sq), rows that see no key
+ *              get out = 0 and lse = +inf.  Cache slots past K_b may hold anything (NaN included) and do not change the
+ *              result.
+ *   num_splits, workspace : as tfa_attn_args.  tfa_attn_num_splits() / tfa_attn_workspace_bytes() on the dense
+ *              problem (B, Hq, Sq, Sk = capacity) give the split count and the workspace it needs.
+ * The host never reads cache_seqlens or block_table: the call (append included) can be captured in a CUDA graph and
+ * replayed with new contents.  The kernels clamp the lengths; a block-table entry outside [0, num_blocks) is never
+ * written through (the append drops that token) and reads through it return zeros, so malformed contents cannot make
+ * a store leave out, lse or the cache.  Launches: 1, + 1 with k_new, + 1 with split-KV. */
+typedef struct tfa_attn_kvcache_args {
+  const void* q;
+  void* k_cache;
+  void* v_cache;
+  const void* k_new;        /* may be NULL (then v_new must be NULL too) */
+  const void* v_new;
+  void* out;
+  float* lse;
+  const int32_t* cache_seqlens;
+  const int32_t* block_table;  /* may be NULL: contiguous cache */
+  int32_t B, Hq, Hkv, Sq, D;
+  int32_t num_blocks, page_block_size, max_blocks_per_seq;
+  int32_t Snew;             /* rows of k_new / v_new; ignored without them */
+  int64_t q_stride_b, q_stride_s, q_stride_h;
+  int64_t cache_stride_block, cache_stride_s, cache_stride_h;
+  int64_t block_table_stride;
+  int64_t new_stride_b, new_stride_s, new_stride_h;
+  int32_t dtype;
+  int32_t is_causal;
+  float softmax_scale;
+  int32_t out_fp32;
+  int32_t num_splits;
+  void* workspace;
+  size_t workspace_bytes;
+  void* stream;
+} tfa_attn_kvcache_args;
+
+int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

@@ -8,9 +8,14 @@ delays, and each warpgroup's wgmma groups complete in order after random delays 
 N groups are still in flight).  One CTA walks a list of work items, as the persistent schedule does; a list of one item
 is the one-CTA-per-item schedule.  An item with no KV tiles is skipped by the producer; the softmax warpgroups skip it
 too, except for a variable-length item whose rows see no key (`empty`), for which they write O = 0 and LSE = +inf
-without waiting on any barrier.  Shadow state catches what a deadlock-only test would miss:
+without waiting on any barrier.  For a KV-cache item (`vtail`) both warpgroups also WRITE into the ring: they zero
+the V rows past the sequence's keys in the slot of its last tile before PV reads it.  The stores take time (they span
+a scheduling point), and are legal only between that slot's kv_full and the warpgroup's release.  Shadow state
+catches what a deadlock-only test would miss:
 
-  * a Q buffer or ring slot overwritten by TMA while an issued, unfinished wgmma still reads it,
+  * a Q buffer or ring slot overwritten by TMA while an issued, unfinished wgmma still reads it, or while a warpgroup
+    still stores into it,
+  * a warpgroup storing into a slot that no longer holds the tile it waited for,
   * a wgmma that reads a buffer holding the wrong (item, tile) -- a release that came too early or a parity slip,
   * every warpgroup consumes every item's K/V tiles exactly once and in order, and finishes every item.
 
@@ -36,9 +41,10 @@ class Bar:
 
 
 class Sim:
-    def __init__(self, items, nstage, rng, empty=()):
+    def __init__(self, items, nstage, rng, empty=(), vtail=()):
         self.items, self.N, self.rng = items, nstage, rng     # items: KV tiles per work item (0 = skipped)
         self.empty = set(empty)                               # items with 0 tiles whose rows are still written
+        self.vtail = set(vtail)                               # items whose last V tile the consumers zero in place
         self.q_full = Bar("q_full", 1)
         self.q_empty = Bar("q_empty", 2)                      # one arrival per warpgroup (per warp in the kernel)
         self.kv_full = [Bar(f"kv_full{i}", 1) for i in range(nstage)]
@@ -48,6 +54,7 @@ class Sim:
         self.kv_buf = [None] * nstage                         # (item, j, 'K'|'V')
         self.q_readers = 0
         self.kv_readers = [0] * nstage
+        self.kv_writers = [0] * nstage                        # warpgroups storing into the slot
         self.tma_q = []                                       # in-flight loads: [remaining, fn]
         self.mma_q = [[], []]                                 # per warpgroup, in order: [remaining, fn_done]
         self.seen = [[], []]                                  # (item, j) consumed, per warpgroup
@@ -94,10 +101,12 @@ class Sim:
                     slot = ent % N
                     yield lambda s=slot, p=((ent // N) & 1) ^ 1: self.kv_empty[s].done(p)
                     assert self.kv_readers[slot] == 0, f"slot {slot} overwritten while a wgmma reads it"
+                    assert self.kv_writers[slot] == 0, f"slot {slot} overwritten while a warpgroup stores into it"
                     self.kv_buf[slot] = "busy"
 
                     def kv_landed(slot=slot, tag=(item, j, kv)):
                         assert self.kv_readers[slot] == 0, "slot written under a reader"
+                        assert self.kv_writers[slot] == 0, "slot written under a warpgroup's stores"
                         self.kv_buf[slot] = tag
                         self.kv_full[slot].arrive()
                     self.tma(kv_landed)
@@ -129,6 +138,14 @@ class Sim:
 
         def wait_full(e):
             yield lambda s=e % N, p=(e // N) & 1: self.kv_full[s].done(p)
+
+        def store_into(slot, tag):
+            """The warpgroup's zeroing stores into a ring slot: they start and end at different scheduling points."""
+            assert self.kv_buf[slot] == tag, f"wg{t}: stores into slot {slot} holding {self.kv_buf[slot]}, not {tag}"
+            self.kv_writers[slot] += 1
+            yield lambda: True
+            assert self.kv_buf[slot] == tag, f"wg{t}: slot {slot} refilled under its stores ({self.kv_buf[slot]})"
+            self.kv_writers[slot] -= 1
 
         for item, n in enumerate(self.items):
             if n == 0:
@@ -164,6 +181,8 @@ class Sim:
                 self.kv_empty[ev % N].arrive()
             ev = ent + 2 * n - 1
             yield from wait_full(ev)
+            if item in self.vtail:                            # zero the V rows past the keys, then PV reads the slot
+                yield from store_into(ev % N, (item, n - 1, "V"))
             issue([("KV", ev % N, (item, n - 1, "V"))])
             yield from wait_group(0)
             self.kv_empty[ev % N].arrive()
@@ -230,6 +249,21 @@ def random_varlen_items(rng):
     return items, empty
 
 
+def random_cache_items(rng):
+    """Items of a KV-cache problem: tiles per item (0 = a split past the sequence's keys, or a row block that sees
+    none: its rows are still written), and the items whose last tile holds the sequence's last key with slots past
+    it, whose V rows the consumers zero."""
+    items, empty, vtail = [], [], []
+    for i in range(rng.randint(1, 12)):
+        n = rng.choice([0, 0, 1, 2, 3, 5])
+        items.append(n)
+        if n == 0:
+            empty.append(i)
+        elif rng.random() < 0.7:
+            vtail.append(i)
+    return items, empty, vtail
+
+
 def main():
     trials = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     for trial in range(trials):
@@ -237,6 +271,8 @@ def main():
         Sim(random_items(rng), rng.choice([4, 8]), rng).run()
         items, empty = random_varlen_items(rng)
         Sim(items, rng.choice([4, 8]), rng, empty).run()
+        items, empty, vtail = random_cache_items(rng)
+        Sim(items, rng.choice([4, 8]), rng, empty, vtail).run()
     print(f"{trials} trials: no violation")
 
 

@@ -18,7 +18,9 @@
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
+#include <algorithm>
 #include <cstdio>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -263,6 +265,117 @@ std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Ten
   return {out, lse};
 }
 
+// Attention against a KV cache (flash-attn's flash_attn_with_kvcache without rotary): q (B, Sq, Hq, D);
+// k_cache / v_cache (num_blocks, page_block_size, Hkv, D) with block_table int32 (B, max_blocks_per_seq), or a
+// contiguous (B, capacity, Hkv, D) cache with block_table None; cache_seqlens int32 (B); k_new / v_new None or
+// (B, Snew, Hkv, D), written into the cache in place at keys [cache_seqlens[b], + Snew) before the attention.
+// Returns out (B, Sq, Hq, D) and lse (B, Hq, Sq).  num_splits as flash_attention_v2_general.
+std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache,
+                                                      torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table,
+                                                      std::optional<torch::Tensor> k_new,
+                                                      std::optional<torch::Tensor> v_new, bool is_causal,
+                                                      float softmax_scale, int64_t num_splits) {
+  TFA_CHECK_CUDA(q);
+  TFA_CHECK_CUDA(k_cache);
+  TFA_CHECK_CUDA(v_cache);
+  TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "q, k_cache, v_cache must have 4 dimensions");
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
+  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
+              "q, k_cache, v_cache must have the same dtype");
+  TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
+              "k_cache and v_cache must have identical shapes and strides");
+  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "q and the caches must share a device");
+  TORCH_CHECK(q.stride(3) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
+  TORCH_CHECK(k_cache.size(3) == q.size(3), "the caches must share head_dim with q");
+  TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
+                  cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == q.size(0),
+              "cache_seqlens must be a contiguous int32 (B,) tensor on q's device");
+  const int64_t B = q.size(0), Sq = q.size(1), Hq = q.size(2), D = q.size(3);
+  const int64_t nblk = k_cache.size(0), page = k_cache.size(1), Hkv = k_cache.size(2);
+  int64_t mbps = 1, bts = 1;
+  if (block_table.has_value()) {
+    const torch::Tensor& bt = *block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == B &&
+                    bt.stride(1) == 1,
+                "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
+    TORCH_CHECK(page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
+                                         static_cast<long long>(page)));
+    mbps = bt.size(1);
+    bts = bt.stride(0);
+  } else {
+    TORCH_CHECK(nblk == B, "without block_table the caches must be (B, capacity, Hkv, D)");
+  }
+  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
+  int64_t snew = 0;
+  if (k_new.has_value()) {
+    const torch::Tensor &kn = *k_new, &vn = *v_new;
+    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
+                    vn.scalar_type() == q.scalar_type(),
+                "k_new and v_new must be on q's device with q's dtype");
+    TORCH_CHECK(kn.dim() == 4 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == B &&
+                    kn.size(2) == Hkv && kn.size(3) == D && kn.stride(3) == 1,
+                "k_new and v_new must be (B, Snew, Hkv, D) with identical strides and a unit head_dim stride");
+    snew = kn.size(1);
+    TORCH_CHECK(snew >= 1 && snew <= mbps * page, "Snew must be in [1, capacity]");
+  }
+  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
+  TORCH_CHECK(B >= 1 && Sq >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
+  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(num_splits >= 0 && num_splits <= 1024, "num_splits must be in [0, 1024]");
+
+  torch::Tensor out, lse, ws;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    out = torch::empty_like(q);
+    if (out.strides() != q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
+      q = q.contiguous();
+      out = torch::empty_like(q);
+    }
+    lse = torch::empty({B, Hq, Sq}, q.options().dtype(at::kFloat));
+    tfa_attn_kvcache_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr();
+    a.k_new = snew ? k_new->data_ptr() : nullptr;
+    a.v_new = snew ? v_new->data_ptr() : nullptr;
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.cache_seqlens = cache_seqlens.data_ptr<int32_t>();
+    a.block_table = block_table.has_value() ? block_table->data_ptr<int32_t>() : nullptr;
+    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
+    a.Sq = static_cast<int32_t>(Sq); a.D = static_cast<int32_t>(D);
+    a.num_blocks = static_cast<int32_t>(nblk); a.page_block_size = static_cast<int32_t>(page);
+    a.max_blocks_per_seq = static_cast<int32_t>(mbps); a.Snew = static_cast<int32_t>(snew);
+    a.q_stride_b = q.stride(0); a.q_stride_s = q.stride(1); a.q_stride_h = q.stride(2);
+    a.cache_stride_block = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1); a.cache_stride_h = k_cache.stride(2);
+    a.block_table_stride = bts;
+    if (snew) { a.new_stride_b = k_new->stride(0); a.new_stride_s = k_new->stride(1); a.new_stride_h = k_new->stride(2); }
+    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.num_splits = static_cast<int32_t>(num_splits);
+    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    // split count and workspace: those of the dense problem with Sk = capacity
+    tfa_attn_args d;
+    std::memset(&d, 0, sizeof(d));
+    d.B = a.B; d.Hq = a.Hq; d.Hkv = a.Hkv; d.Sq = a.Sq; d.D = a.D;
+    d.Sk = static_cast<int32_t>(std::min<int64_t>(mbps * page, 0x7fffffff));
+    d.is_causal = a.is_causal;
+    d.num_splits = a.num_splits;
+    const int nsplit = tfa_attn_num_splits(&d);
+    if (nsplit > 1) {
+      const size_t need = tfa_attn_workspace_bytes(&d, nsplit);
+      ws = torch::empty({static_cast<int64_t>((need + 3) / 4)}, q.options().dtype(at::kFloat));
+      a.workspace = ws.data_ptr();
+      a.workspace_bytes = need;
+      a.num_splits = nsplit;
+    }
+    rc = tfa_attn_kvcache_fwd(&a);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_cutlass", &flash_attention_v2_cutlass,
         "Flash attention v2 forward, H100-native (sm_90a wgmma/TMA)");
@@ -274,6 +387,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "grouped K/V heads, Sq != Sk (bottom-right causal), optional split-KV: (q, k, v, is_causal, scale, num_splits)");
   m.def("flash_attention_v2_varlen", &flash_attention_v2_varlen,
         "packed variable-length batch: (q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, scale)");
-  m.def("launch_count", []() { return tfa_launch_count(); }, "kernels launched by the library so far");
+  m.def("flash_attention_v2_kvcache", &flash_attention_v2_kvcache,
+        "attention against a (paged) KV cache with an optional in-place append: (q, k_cache, v_cache, cache_seqlens, "
+        "block_table, k_new, v_new, is_causal, scale, num_splits)");
+  m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

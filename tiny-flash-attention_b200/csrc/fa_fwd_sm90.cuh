@@ -31,11 +31,44 @@
 // gives its registers to the others), warpgroups 1 and 2 run Q tile 0 and 1: wgmma, softmax, epilogue.
 // PERSIST = false: one CTA per work item.  PERSIST = true: one CTA per SM walks the items blockIdx.x, +gridDim.x, ...
 // and its producer runs ahead into the next item's Q and K/V while the softmax warpgroups finish the current one.
-// VARLEN = true: a packed variable-length batch; each item reads its sequence's offsets and lengths from cu_seqlens.
+// MODE (the problem the grid solves): kDense = (B, H, S, D) tensors; kVarlen = a packed variable-length batch, each
+// item reads its sequence's offsets and lengths from cu_seqlens; kCache = decode against a (paged) KV cache, each item
+// reads its sequence's cached length from cache_seqlens and its K/V boxes' pages from a block table.
 #pragma once
 #include "ptx_sm90.cuh"
 
 namespace tfa {
+
+enum : int { kDense = 0, kVarlen = 1, kCache = 2 };
+
+// ---- KV-cache address math, host-callable so that a CPU test can check it exhaustively (tests/test_kvcache.py) ----
+// Keys attended by sequence b: its cached length clamped to [0, capacity - snew], plus the snew appended keys.  The
+// clamp keeps every append inside the sequence's capacity whatever cache_seqlens holds.
+__host__ __device__ __forceinline__ int cache_len(int raw, int capacity, int snew) {
+  return min(max(raw, 0), capacity - snew);
+}
+// Logical key `key` (0 <= key < capacity) of sequence b -> (physical block, row inside it).  Without a block table
+// the cache is contiguous, one page of `page` = capacity rows per sequence, and the block is b.  The entry is
+// returned as stored: the TMA loads bounds-check it in hardware, the append checks it with block_ok().
+__host__ __device__ __forceinline__ void page_lookup(const int* block_table, long long bt_stride, int b, int key,
+                                                     int page, int& blk, int& row) {
+  const int pg = key / page;
+  blk = block_table ? block_table[b * bt_stride + pg] : b;
+  row = key - pg * page;
+}
+__host__ __device__ __forceinline__ bool block_ok(int blk, int num_blocks) { return blk >= 0 && blk < num_blocks; }
+// Element offset, in a cache with (block, row, head) element strides cs_b / cs_s / cs_h, of appended token i of
+// sequence b at head h, or -1 when its block-table entry lies outside [0, num_blocks) (the token is then dropped).
+__host__ __device__ __forceinline__ long long append_offset(const int* cache_seqlens, const int* block_table,
+                                                            long long bt_stride, int b, int i, int h, int page,
+                                                            int capacity, int snew, int num_blocks, long long cs_b,
+                                                            long long cs_s, long long cs_h) {
+  const int key = cache_len(cache_seqlens[b], capacity, snew) + i;
+  int blk, row;
+  page_lookup(block_table, bt_stride, b, key, page, blk, row);
+  if (!block_ok(blk, num_blocks)) return -1;
+  return blk * cs_b + row * cs_s + h * cs_h;
+}
 
 struct FwdParams {
   void* out;          // 16-bit output, element strides below
@@ -74,6 +107,13 @@ struct FwdParams {
   const int* cu_q;
   const int* cu_k;
   int total_q, total_k;
+  // KV cache (MODE == kCache): q / out / lse are the dense (B, H, S) problem; sequence b attends to the first
+  // cache_len(cache_seqlens[b]) + snew keys of its cache, whose key r lives at page_lookup(block_table, b, r).  The
+  // K/V tensor maps are (D, page, Hkv, num_blocks).  Sk / causal_off are unused.
+  const int* cache_seqlens;
+  const int* block_table;     // nullptr: contiguous cache, page = capacity
+  long long bt_stride;
+  int page, capacity, snew;
 };
 
 template <int D>
@@ -124,15 +164,17 @@ __host__ __device__ __forceinline__ void decode_work(int block, int npairs, int 
 
 // One work item: both Q tiles walk the same KV tiles [jb, jb + n); rows a tile does not see are masked.
 // q0 / k0 are the sequence's first row in the (packed) q and k/v tensors, Sq / Sk / coff its own lengths and causal
-// offset: the whole tensor's (q0 = k0 = 0) unless VARLEN.  `live`: the item has rows to write.  The producer loads an
-// item iff n > 0, the softmax warpgroups wait on its barriers iff n > 0: n > 0 implies live.
+// offset: the whole tensor's (q0 = k0 = 0) for kDense, the cached length for kCache.  `live`: the item has rows to
+// write.  The producer loads an item iff n > 0, the softmax warpgroups wait on its barriers iff n > 0: n > 0 implies
+// live.
 struct Item {
   int bh, bidx, hidx, hkv, split, jb, row0, n;
   int q0, k0, Sq, Sk, coff;
   bool live;
 };
-template <bool CAUSAL, bool VARLEN>
+template <bool CAUSAL, int MODE>
 __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
+  constexpr bool VARLEN = MODE == kVarlen;
   Item w;
   int pr;
   decode_work(item, p.npairs, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
@@ -152,6 +194,12 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.Sq = max(q1 - q0, 0);
     w.Sk = max(k1 - k0, 0);
     w.coff = w.Sk - w.Sq;           // may be negative: the sequence's first rows see no key
+  } else if constexpr (MODE == kCache) {
+    w.q0 = 0;
+    w.k0 = 0;
+    w.Sq = p.S;
+    w.Sk = cache_len(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew) + p.snew;
+    w.coff = w.Sk - w.Sq;           // may be negative, as for varlen
   } else {
     w.q0 = 0;
     w.k0 = 0;
@@ -160,21 +208,24 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.coff = p.causal_off;
   }
   const int nkv_total = (w.Sk + 127) >> 7;
-  // causal: the item's last row sees keys <= last (none when last < 0, which only a varlen sequence can have)
+  // causal: the item's last row sees keys <= last (none when last < 0, which only varlen and cache sequences can have)
   const int last = w.row0 + 127 + w.coff;
-  const int nfull = CAUSAL ? ((VARLEN && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
+  const int nfull = CAUSAL ? ((MODE != kDense && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
   w.n = max(0, min(nfull - w.jb, p.split_tiles));   // 0: a split-KV item wholly above the causal diagonal
   // dense: an item without tiles writes nothing (its rows belong to other splits); varlen: an item inside its sequence
-  // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0)
-  w.live = VARLEN ? w.row0 < w.Sq : w.n > 0;
+  // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0); cache: every item writes its rows,
+  // a split without tiles too (LSE = -inf), so the combine can read every split's partial
+  w.live = VARLEN ? w.row0 < w.Sq : (MODE == kCache || w.n > 0);
   if (VARLEN && !w.live) w.n = 0;    // past the sequence's end: the producer must skip it as the consumers do
   return w;
 }
 
-template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST, bool VARLEN>
+template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST, int MODE>
 __global__ void __launch_bounds__(384, 1)
 fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
+  constexpr bool VARLEN = MODE == kVarlen;
+  constexpr bool CACHE = MODE == kCache;
   using C = FwdCfg<D>;
   constexpr int TILE = C::TILE_BYTES;
   constexpr int NSTAGE = C::NSTAGE;
@@ -195,7 +246,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int lane = threadIdx.x & 31;
   const int first = static_cast<int>(blockIdx.x);
   const int stride = PERSIST ? static_cast<int>(gridDim.x) : p.total_items;
-  if (!PERSIST && !decode_item<CAUSAL, VARLEN>(first, p).live) return;   // CTA-uniform
+  if (!PERSIST && !decode_item<CAUSAL, MODE>(first, p).live) return;   // CTA-uniform
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -218,7 +269,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       uint32_t ent = 0;      // running K/V ring entry (K_j and V_j of every item in turn; never reset between items)
       uint32_t qcnt = 0;     // items loaded
       for (int item = first; item < p.total_items; item += stride) {
-        const Item w = decode_item<CAUSAL, VARLEN>(item, p);
+        const Item w = decode_item<CAUSAL, MODE>(item, p);
         if (w.n == 0) continue;
         if (qcnt > 0) mbar_wait(q_empty, (qcnt - 1) & 1, p.dbg, SITE_LOAD_Q, qcnt);
         ++qcnt;
@@ -230,6 +281,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         for (int sl = 0; sl < C::SLABS; ++sl)
           tma_load_4d(sQ + sl * C::SLAB_BYTES, &tmQ, q_full, sl * 64, w.q0 + w.row0, w.hidx, wz);
         for (int j = 0; j < w.n; ++j) {
+          // cache: the tile's 128 keys lie in one page (page % 128 == 0, or one page per sequence)
+          int ky = w.k0 + (w.jb + j) * C::BN, kw = wz;
+          if constexpr (CACHE) page_lookup(p.block_table, p.bt_stride, w.bidx, ky, p.page, kw, ky);
 #pragma unroll
           for (int kv = 0; kv < 2; ++kv, ++ent) {
             const uint32_t slot = ent % NSTAGE;
@@ -238,8 +292,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             const CUtensorMap* tm = kv ? &tmV : &tmK;
 #pragma unroll
             for (int sl = 0; sl < C::SLABS; ++sl)
-              tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64,
-                          w.k0 + (w.jb + j) * C::BN, w.hkv, wz);
+              tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64, ky, w.hkv, kw);
           }
         }
       }
@@ -262,7 +315,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint32_t ent = 0;        // K/V ring entry of K_0 of the current item (same sequence as the producer's)
   uint32_t qcnt = 0;
   for (int item = first; item < p.total_items; item += stride) {
-    const Item w = decode_item<CAUSAL, VARLEN>(item, p);
+    const Item w = decode_item<CAUSAL, MODE>(item, p);
     const int n = w.n;
     if (!w.live) continue;
     const int S = w.Sq, Sk = w.Sk, coff = w.coff;
@@ -289,6 +342,26 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     auto release = [&](uint64_t* bar) {
       __syncwarp();
       if (lane == 0) mbar_arrive(bar);
+    };
+    // cache: the slots of a page past the sequence's keys may hold anything, NaN included, and P = 0 does not cancel
+    // 0 * NaN in the PV product.  So before PV reads the tile holding key Sk - 1, this warpgroup zeroes the V rows
+    // [Sk, tile end) in shared memory (whole 128-byte swizzle rows of each slab, so the swizzle does not matter).  Both
+    // warpgroups write the same zeros; the slot is released only after both have read it.  Between the kv_full wait
+    // and the release, so the producer cannot refill the slot under the stores (scripts/protocol_model.py).
+    auto zero_v_tail = [&](uint32_t vslot, int jt) {
+      if constexpr (CACHE) {
+        const int valid = Sk - (w.jb + jt) * C::BN;          // warpgroup-uniform
+        if (valid < C::BN) {
+          uint8_t* vt = sKV + vslot * TILE;
+          const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+          for (int idx = valid * 8 + (threadIdx.x & 127); idx < C::BN * 8; idx += 128) {
+#pragma unroll
+            for (int sl = 0; sl < C::SLABS; ++sl) *reinterpret_cast<uint4*>(vt + sl * C::SLAB_BYTES + idx * 16) = z;
+          }
+          fence_proxy_async_smem();                          // generic-proxy stores -> the wgmma's operand reads
+          named_bar_sync(1 + t, 128);
+        }
+      }
     };
 
     float s[64];             // S tile: 16 column groups of 8 keys x {row_lo: [0],[1], row_hi: [2],[3]}
@@ -367,8 +440,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
     };
 
-    // A varlen item whose rows all see no key has no tiles: it waits on no barrier, its rows get O = 0, LSE = +inf.
-    if (!VARLEN || n > 0) {
+    // A varlen or cache item whose rows all see no key has no tiles: it waits on no barrier, its rows get O = 0 and
+    // LSE = +inf (-inf for a split-KV partial).
+    if (MODE == kDense || n > 0) {
       mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
       ++qcnt;
       // ---- KV tile 0 ----
@@ -394,6 +468,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         wgmma_fence();
         issue_S(s, kslot);
         mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        zero_v_tail(vslot, j - 1);
         issue_PV(o, pf, vslot, j > 1);
         wgmma_wait<1>();                               // S_j done
         reg_fence(s);
@@ -417,6 +492,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       {
         const uint32_t ev = ent + 2 * n - 1, vslot = ev % NSTAGE;
         mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        zero_v_tail(vslot, n - 1);
         wgmma_fence();
         issue_PV(o, pf, vslot, n > 1);
         wgmma_wait<0>();
@@ -444,6 +520,12 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         float* lrow = p.lse + static_cast<long long>(w.hidx) * p.lse_stride_bh + w.q0;
         if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : INFINITY;
         if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : INFINITY;
+      } else if constexpr (CACHE) {
+        // (B, H, S) as dense; a row that saw no key gets +inf, or -inf in a split-KV partial (as above)
+        const float none = p.nsplit > 1 ? -INFINITY : INFINITY;
+        float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
+        if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : none;
+        if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : none;
       } else {
         float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
         if (row_lo < S) lrow[row_lo] = m_lo * p.scale + logf(l_lo);

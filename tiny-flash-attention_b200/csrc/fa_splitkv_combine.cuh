@@ -1,5 +1,5 @@
-// fa_splitkv_combine.cuh -- the two small HBM-bound kernels either side of the attention forward when the problem
-// is not the reference's square one (SURVEY.md 8f rows 2-3):
+// fa_splitkv_combine.cuh -- the small HBM-bound kernels either side of the attention forward when the problem
+// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below):
 //
 //   * splitkv_combine_kernel: merges the per-split partial results of the split-KV forward,
 //       O = sum_s exp(lse_s - LSE) * O_s ,  LSE = log sum_s exp(lse_s)
@@ -15,6 +15,7 @@
 // Roofline: HBM.  Algorithmic bytes per row: combine nsplit_valid*(4D+4) + 2D + 4, fill 2D + 4.
 #pragma once
 #include "ptx_sm90.cuh"
+#include "fa_fwd_sm90.cuh"    // the KV-cache address helpers the append shares with the forward
 
 namespace tfa {
 
@@ -105,6 +106,46 @@ __global__ void __launch_bounds__(256) empty_rows_fill_kernel(const FillParams p
   if constexpr (OUT_F32) *reinterpret_cast<float4*>(static_cast<float*>(p.out) + off) = make_float4(0.f, 0.f, 0.f, 0.f);
   else *reinterpret_cast<uint2*>(static_cast<uint16_t*>(p.out) + off) = make_uint2(0u, 0u);
   if (p.lse != nullptr && sub == 0) p.lse[bh * p.lse_stride_bh + i] = INFINITY;
+}
+
+// kvcache_append_kernel: writes k_new / v_new (B, snew, Hkv, D) into the (paged) KV cache at keys
+// [L_b, L_b + snew) of each sequence, L_b = cache_len(cache_seqlens[b]), before the forward reads the cache.  One thread
+// copies one 16-byte chunk of K and the same chunk of V.  cache_seqlens is not incremented.  A token whose block-table
+// entry lies outside [0, num_blocks) is dropped: no store leaves the cache.  Algorithmic bytes: 2 * 2 * B*snew*Hkv*D
+// read and written.
+struct AppendParams {
+  const void* k_new;
+  const void* v_new;
+  void* k_cache;
+  void* v_cache;
+  long long n_sb, n_ss, n_sh;     // element strides of k_new / v_new
+  long long c_sb, c_ss, c_sh;     // element strides of the caches: block, row, head
+  const int* cache_seqlens;
+  const int* block_table;         // nullptr: contiguous cache
+  long long bt_stride;
+  int page, capacity, snew, num_blocks, Hkv;
+  long long chunks;               // B * snew * Hkv * D / 8
+};
+
+template <int D>
+__global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendParams p) {
+  constexpr int CPR = D / 8;                   // 16-byte chunks per row
+  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (c >= p.chunks) return;
+  const int sub = static_cast<int>(c % CPR);
+  long long r = c / CPR;
+  const int h = static_cast<int>(r % p.Hkv);
+  r /= p.Hkv;
+  const int i = static_cast<int>(r % p.snew);
+  const int b = static_cast<int>(r / p.snew);
+  const long long dst = append_offset(p.cache_seqlens, p.block_table, p.bt_stride, b, i, h, p.page, p.capacity,
+                                      p.snew, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
+  if (dst < 0) return;
+  const long long src = b * p.n_sb + i * p.n_ss + h * p.n_sh + sub * 8;
+  const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
+  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + dst + sub * 8) = vx;
 }
 
 }  // namespace tfa

@@ -142,7 +142,7 @@ cudaError_t opt_in_smem(K kernel, int bytes) {
   return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
 
-template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool VARLEN>
+template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, int MODE>
 int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
                 int variant, cudaStream_t stream) {
   cudaError_t cerr = cudaSuccess;
@@ -152,11 +152,11 @@ int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
     const int sms = num_sms();
     if (sms <= 0) return TFA_EARCH;
     if (nblocks > sms) nblocks = sms;                                   // one CTA per SM
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, VARLEN>;
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, MODE>;
     if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
     kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   } else {
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, VARLEN>;
+    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
     if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
     kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   }
@@ -164,10 +164,10 @@ int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap&
   return static_cast<int>(cudaGetLastError());
 }
 
-template <int D, bool VARLEN>
+template <int D, int MODE>
 int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
              const FwdParams& p, long long nblocks, int variant, cudaStream_t s) {
-#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_, VARLEN>(tq, tk, tv, p, nblocks, variant, s)
+#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_, MODE>(tq, tk, tv, p, nblocks, variant, s)
   if (causal) {
     if (bf16) { if (f32) TFA_GO(true, true, true); else TFA_GO(true, true, false); }
     else      { if (f32) TFA_GO(true, false, true); else TFA_GO(true, false, false); }
@@ -195,14 +195,14 @@ FwdParams base_params(int Hq, int Hkv, long long npairs, int BH, float scale) {
   return p;
 }
 
-// One forward kernel launch over `nitems` work items.
-template <bool VARLEN>
+// One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache).
+template <int MODE>
 int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
   if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
   p.total_items = static_cast<int>(nitems);
-  if (D == 64) return dispatch<64, VARLEN>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
-  return dispatch<128, VARLEN>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+  if (D == 64) return dispatch<64, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+  return dispatch<128, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
 }
 
 bool arch_ok() {
@@ -398,7 +398,7 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
 
   const long long nitems = npairs * a.B * a.Hq * nsplit;
   const bool kernel_f32 = f32 || nsplit > 1;
-  rc = launch_fwd<false>(a.D, causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
+  rc = launch_fwd<tfa::kDense>(a.D, causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
   if (rc) return rc;
 
   if (nsplit > 1) {
@@ -491,7 +491,148 @@ int varlen_impl(const tfa_attn_varlen_args& va) {
   p.cu_k = va.cu_seqlens_k;
   p.total_q = a.Sq;
   p.total_k = a.Sk;
-  return launch_fwd<true>(a.D, causal, bf16, f32, tq, tk, tv, p, npairs * a.B * a.Hq, variant, a.stream);
+  return launch_fwd<tfa::kVarlen>(a.D, causal, bf16, f32, tq, tk, tv, p, npairs * a.B * a.Hq, variant, a.stream);
+}
+
+// The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
+Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
+  Problem q;
+  q.q = a.q; q.k = a.k_cache; q.v = a.v_cache; q.out = a.out; q.lse = a.lse;
+  q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.Sq; q.D = a.D;
+  const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
+  q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
+  q.qsb = a.q_stride_b; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
+  q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
+  q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
+  q.stream = static_cast<cudaStream_t>(a.stream);
+  return q;
+}
+
+int validate_kvcache(const tfa_attn_kvcache_args& ka) {
+  if (!ka.cache_seqlens || (reinterpret_cast<uintptr_t>(ka.cache_seqlens) & 3u) ||
+      (reinterpret_cast<uintptr_t>(ka.block_table) & 3u))
+    return TFA_EINVAL_KVCACHE;
+  if (ka.num_blocks < 1 || ka.max_blocks_per_seq < 1 || ka.page_block_size < 1) return TFA_EINVAL_KVCACHE;
+  if (ka.block_table) {
+    if (ka.page_block_size % 128 || ka.block_table_stride < ka.max_blocks_per_seq) return TFA_EINVAL_KVCACHE;
+  } else if (ka.max_blocks_per_seq != 1 || ka.num_blocks < ka.B) {
+    return TFA_EINVAL_KVCACHE;           // contiguous: one page (block b) per sequence
+  }
+  if ((ka.k_new == nullptr) != (ka.v_new == nullptr)) return TFA_EINVAL_KVCACHE;
+  if (ka.k_new) {
+    const long long cap = static_cast<long long>(ka.max_blocks_per_seq) * ka.page_block_size;
+    if (ka.Snew < 1 || ka.Snew > cap) return TFA_EINVAL_KVCACHE;
+    if ((reinterpret_cast<uintptr_t>(ka.k_new) | reinterpret_cast<uintptr_t>(ka.v_new)) & 15u) return TFA_EINVAL_PTR;
+    if ((ka.new_stride_s % 8) || (ka.new_stride_h % 8) || (ka.new_stride_b % 8) || ka.new_stride_s < 0 ||
+        ka.new_stride_h < 0 || ka.new_stride_b < 0)
+      return TFA_EINVAL_STRIDE;
+  }
+  return 0;
+}
+
+int kvcache_impl(const tfa_attn_kvcache_args& ka) {
+  Problem a = from_kvcache_args(ka);
+  int rc = validate_kvcache(ka);        // first: a table of 0 pages is a cache error, not a 0-key shape error
+  if (rc) return rc;
+  if ((rc = validate(a))) return rc;
+  if (!arch_ok()) return TFA_EARCH;
+  init_dbg();
+  cudaStream_t stream = a.stream;
+  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
+  const int capacity = a.Sk;
+  const int snew = ka.k_new ? ka.Snew : 0;
+  const int page = ka.block_table ? ka.page_block_size : capacity;
+
+  int nsplit = resolve_splits(a, a.num_splits, num_sms());
+  if (nsplit > 1) {
+    const size_t need = splitkv_ws_bytes(a, nsplit);
+    const bool ws_ok = a.ws != nullptr && !(reinterpret_cast<uintptr_t>(a.ws) & 15u) && a.ws_bytes >= need;
+    if (!ws_ok) {
+      if (a.num_splits == 0) nsplit = 1;               // auto: no workspace, no split
+      else return TFA_EINVAL_WORKSPACE;
+    }
+  }
+
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
+  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+
+  if (snew > 0) {
+    tfa::AppendParams ap;
+    ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
+    ap.n_sb = ka.new_stride_b; ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
+    ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
+    ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
+    ap.page = page; ap.capacity = capacity; ap.snew = snew; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
+    ap.chunks = static_cast<long long>(a.B) * snew * a.Hkv * (a.D / 8);
+    const long long blocks = (ap.chunks + 255) / 256;
+    if (blocks > 0x7fffffffLL) return TFA_EINVAL_SHAPE;
+    if (a.D == 64) tfa::kvcache_append_kernel<64><<<static_cast<int>(blocks), 256, 0, stream>>>(ap);
+    else           tfa::kvcache_append_kernel<128><<<static_cast<int>(blocks), 256, 0, stream>>>(ap);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if ((rc = static_cast<int>(cudaGetLastError()))) return rc;
+  }
+
+  const long long npairs = (static_cast<long long>(a.Sq) + 127) / 128;
+  const int nkv_total = (capacity + 127) / 128;
+  const int split_tiles = (nkv_total + nsplit - 1) / nsplit;
+  const int variant = choose_kernel(causal, npairs, 0);
+  const long long rows = static_cast<long long>(a.B) * a.Hq * a.Sq;
+  float* ws_o = static_cast<float*>(a.ws);
+  float* ws_lse = ws_o ? ws_o + static_cast<size_t>(nsplit) * rows * a.D : nullptr;
+
+  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
+  p.S = a.Sq;
+  p.nsplit = nsplit;
+  p.split_tiles = split_tiles;
+  if (nsplit > 1) {
+    // partials: contiguous (B, Hq, Sq, D) fp32 per split, as fwd_impl's
+    p.out_f32 = ws_o;
+    p.lse = ws_lse;
+    p.o_stride_s = a.D;
+    p.o_stride_h = static_cast<long long>(a.Sq) * a.D;
+    p.o_stride_b = p.o_stride_h * a.Hq;
+    p.part_stride = rows * a.D;
+    p.lse_stride_bh = a.Sq;
+    p.lse_part_stride = rows;
+  } else {
+    p.out = f32 ? nullptr : a.out;
+    p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
+    p.lse = a.lse;
+    p.o_stride_b = a.qsb;
+    p.o_stride_h = a.qsh;
+    p.o_stride_s = a.qss;
+    p.lse_stride_bh = a.Sq;
+  }
+  p.cache_seqlens = ka.cache_seqlens;
+  p.block_table = ka.block_table;
+  p.bt_stride = ka.block_table_stride;
+  p.page = page;
+  p.capacity = capacity;
+  p.snew = snew;
+  rc = launch_fwd<tfa::kCache>(a.D, causal, bf16, f32 || nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * nsplit,
+                               variant, stream);
+  if (rc) return rc;
+
+  if (nsplit > 1) {
+    // every split wrote its rows (LSE = -inf where it saw no key): causal = 0 makes the combine read all of them
+    tfa::CombineParams cp;
+    cp.o_part = ws_o;
+    cp.lse_part = ws_lse;
+    cp.out = a.out;
+    cp.lse = a.lse;
+    cp.o_stride_b = a.qsb; cp.o_stride_h = a.qsh; cp.o_stride_s = a.qss;
+    cp.lse_stride_bh = a.Sq;
+    cp.rows = rows;
+    cp.H = a.Hq; cp.S = a.Sq;
+    cp.nsplit = nsplit; cp.split_tiles = split_tiles;
+    cp.nkv_total = nkv_total;
+    cp.causal = 0; cp.causal_off = 0;
+    rc = (a.D == 64) ? launch_combine<64>(cp, bf16, f32, stream) : launch_combine<128>(cp, bf16, f32, stream);
+  }
+  return rc;
 }
 
 // ---- host-buffer path workspace ----
@@ -533,6 +674,11 @@ int tfa_attn_fwd(const tfa_attn_args* args) {
 int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
   if (!args) return TFA_EINVAL_PTR;
   return varlen_impl(*args);
+}
+
+int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
+  if (!args) return TFA_EINVAL_PTR;
+  return kvcache_impl(*args);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -666,6 +812,20 @@ int tfa_internal_decode_work(int block, int npairs, int nsplit, int head_chunk, 
   return 0;
 }
 
+// development aid (not in the public header): the KV-cache address helpers of fa_fwd_sm90.cuh, callable on the host
+// with host arrays.  out2 = {physical block, row} of key `key` of sequence b.
+int tfa_internal_page_lookup(const int* block_table, long long bt_stride, int b, int key, int page, int* out2) {
+  tfa::page_lookup(block_table, bt_stride, b, key, page, out2[0], out2[1]);
+  return 0;
+}
+int tfa_internal_cache_len(int raw, int capacity, int snew) { return tfa::cache_len(raw, capacity, snew); }
+long long tfa_internal_append_offset(const int* cache_seqlens, const int* block_table, long long bt_stride, int b, int i,
+                                     int h, int page, int capacity, int snew, int num_blocks, long long cs_b,
+                                     long long cs_s, long long cs_h) {
+  return tfa::append_offset(cache_seqlens, block_table, bt_stride, b, i, h, page, capacity, snew, num_blocks, cs_b,
+                            cs_s, cs_h);
+}
+
 int tfa_debug_record(unsigned int out[8]) {
   if (!out) return TFA_EINVAL_PTR;
   if (!g_dbg_host) { std::memset(out, 0, 8 * sizeof(unsigned int)); return 0; }
@@ -692,6 +852,9 @@ const char* tfa_error_string(int code) {
     case TFA_EINVAL_WORKSPACE: return "tfa: split-KV needs a 16-byte aligned workspace of tfa_attn_workspace_bytes()";
     case TFA_EINVAL_SEQLENS:
       return "tfa: cu_seqlens must be non-null 4-byte aligned device pointers and max_seqlen_q in [1, total_q]";
+    case TFA_EINVAL_KVCACHE:
+      return "tfa: kv cache needs non-null 4-byte aligned cache_seqlens (block_table: aligned, page_block_size a "
+             "multiple of 128), num_blocks and max_blocks_per_seq >= 1, and k_new with v_new, Snew in [1, capacity]";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "tfa: unknown error";
   }
 }

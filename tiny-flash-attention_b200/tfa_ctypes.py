@@ -64,6 +64,25 @@ class VarlenArgs(ctypes.Structure):
     ]
 
 
+class KvcacheArgs(ctypes.Structure):
+    """struct tfa_attn_kvcache_args (include/tfa_b200.h)."""
+    _fields_ = [
+        ("q", ctypes.c_void_p), ("k_cache", ctypes.c_void_p), ("v_cache", ctypes.c_void_p),
+        ("k_new", ctypes.c_void_p), ("v_new", ctypes.c_void_p), ("out", ctypes.c_void_p), ("lse", ctypes.c_void_p),
+        ("cache_seqlens", ctypes.c_void_p), ("block_table", ctypes.c_void_p),
+        ("B", ctypes.c_int32), ("Hq", ctypes.c_int32), ("Hkv", ctypes.c_int32), ("Sq", ctypes.c_int32),
+        ("D", ctypes.c_int32), ("num_blocks", ctypes.c_int32), ("page_block_size", ctypes.c_int32),
+        ("max_blocks_per_seq", ctypes.c_int32), ("Snew", ctypes.c_int32),
+        ("q_stride_b", ctypes.c_int64), ("q_stride_s", ctypes.c_int64), ("q_stride_h", ctypes.c_int64),
+        ("cache_stride_block", ctypes.c_int64), ("cache_stride_s", ctypes.c_int64), ("cache_stride_h", ctypes.c_int64),
+        ("block_table_stride", ctypes.c_int64),
+        ("new_stride_b", ctypes.c_int64), ("new_stride_s", ctypes.c_int64), ("new_stride_h", ctypes.c_int64),
+        ("dtype", ctypes.c_int32), ("is_causal", ctypes.c_int32), ("softmax_scale", ctypes.c_float),
+        ("out_fp32", ctypes.c_int32), ("num_splits", ctypes.c_int32),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t), ("stream", ctypes.c_void_p),
+    ]
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -87,6 +106,8 @@ def lib():
         L.tfa_attn_workspace_bytes.restype = ctypes.c_size_t
         L.tfa_attn_varlen_fwd.argtypes = [ctypes.POINTER(VarlenArgs)]
         L.tfa_attn_varlen_fwd.restype = ci
+        L.tfa_attn_kvcache_fwd.argtypes = [ctypes.POINTER(KvcacheArgs)]
+        L.tfa_attn_kvcache_fwd.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -199,6 +220,56 @@ def attn_varlen_fwd(q, k, v, cu_q, cu_k, max_seqlen_q, is_causal, scale, out_fp3
                    q.stride(0), q.stride(1), k.stride(0), k.stride(1), _dtype_code(q), int(bool(is_causal)),
                    float(scale), int(bool(out_fp32)), st)
     check(lib().tfa_attn_varlen_fwd(ctypes.byref(a)))
+    return out, lse
+
+
+def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
+                     scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False):
+    """Attention against a KV cache through tfa_attn_kvcache_fwd(): q (B, Sq, Hq, D) with unit head_dim stride;
+    k_cache / v_cache (num_blocks, page, Hkv, D) with a block_table (B, max_blocks_per_seq) int32, or (B, capacity,
+    Hkv, D) with block_table None; cache_seqlens (B,) int32; optional k_new / v_new (B, Snew, Hkv, D) appended in
+    place.  num_splits: 1 none, n > 1 as asked, 0 library heuristic (a workspace is allocated here when it splits).
+    Returns out (q's shape and strides) and lse (B, Hq, Sq)."""
+    import torch
+    assert q.is_cuda and q.dim() == 4 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
+    assert k_cache.stride() == v_cache.stride() and q.stride(3) == 1 and k_cache.stride(3) == 1
+    assert cache_seqlens.dtype == torch.int32
+    B, Sq, Hq, D = q.shape
+    nblk, page, Hkv, _ = k_cache.shape
+    if block_table is not None:
+        assert block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
+        mbps, bts, bt_ptr = block_table.shape[1], block_table.stride(0), block_table.data_ptr()
+    else:
+        mbps, bts, bt_ptr = 1, 1, None
+    snew, nptr, vptr, ns = 0, None, None, (0, 0, 0)
+    if k_new is not None:
+        assert k_new.shape == v_new.shape and k_new.stride() == v_new.stride() and k_new.stride(3) == 1
+        snew, nptr, vptr, ns = k_new.shape[1], k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:3]
+    if scale is None:
+        scale = D ** -0.5
+    if out is None:
+        out = torch.empty_strided(q.shape, q.stride(), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+    if lse is None:
+        lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=q.device)
+    st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
+    a = KvcacheArgs(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), nptr, vptr, out.data_ptr(), lse.data_ptr(),
+                    cache_seqlens.data_ptr(), bt_ptr, B, Hq, Hkv, Sq, D, nblk, page, mbps, snew,
+                    q.stride(0), q.stride(1), q.stride(2), k_cache.stride(0), k_cache.stride(1), k_cache.stride(2),
+                    bts, ns[0], ns[1], ns[2], _dtype_code(q), int(bool(is_causal)), float(scale),
+                    int(bool(out_fp32)), int(num_splits), None, 0, st)
+    L = lib()
+    # the split count and workspace of the dense problem with Sk = capacity
+    dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
+                     int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
+    n = int(L.tfa_attn_num_splits(ctypes.byref(dense)))
+    if n > 1:
+        need = int(L.tfa_attn_workspace_bytes(ctypes.byref(dense), n))
+        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=q.device)
+        a.workspace, a.workspace_bytes, a.num_splits = ws.data_ptr(), need, n
+        _WORKSPACES[(q.device.index, int(st))] = ws      # alive until the next call on this stream, as attn_fwd()
+    check(L.tfa_attn_kvcache_fwd(ctypes.byref(a)))
+    if return_splits:
+        return out, lse, n
     return out, lse
 
 
