@@ -45,15 +45,36 @@ std::string fmt_msg(const char* fmt, long long a = 0, long long b = 0, long long
   return std::string(buf);
 }
 
+// q is fp16 or bf16, and the other two tensors share its dtype and device; `names` names all three in the messages.
+void check_dtype_device(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v,
+                        const std::string& names) {
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
+              names + " must have the same dtype");
+  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), names + " must be on the same device");
+}
+
 void check_common(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v) {
   TORCH_CHECK(q.dim() == 4, fmt_msg("q must have 4 dimensions, got %lld", static_cast<long long>(q.dim())));
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16,
-              "q must be float16 or bfloat16");
-  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
-              "q, k, v must have the same dtype");
+  check_dtype_device(q, k, v, "q, k, v");
   TORCH_CHECK(k.sizes() == q.sizes() && v.sizes() == q.sizes(),
               "q, k, v must have identical shapes (self-attention, Sq == Sk)");
-  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
+}
+
+// Split-KV of a dense problem: asks the library for the split count and, when it splits, allocates the workspace on
+// q's device and sets num_splits / workspace / workspace_bytes in `a`.  Returns the workspace (undefined for one
+// pass); the caller keeps it until the launch is enqueued.
+torch::Tensor split_workspace(tfa_attn_args& a, const torch::Tensor& q) {
+  torch::Tensor ws;
+  const int nsplit = tfa_attn_num_splits(&a);
+  if (nsplit > 1) {
+    const size_t need = tfa_attn_workspace_bytes(&a, nsplit);
+    ws = torch::empty({static_cast<int64_t>((need + 3) / 4)}, q.options().dtype(at::kFloat));
+    a.workspace = ws.data_ptr();
+    a.workspace_bytes = need;
+    a.num_splits = nsplit;
+  }
+  return ws;
 }
 
 void raise_on_error(int rc) {
@@ -151,12 +172,9 @@ std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Te
   TFA_CHECK_INPUT(k);
   TFA_CHECK_INPUT(v);
   TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q, k, v must have 4 dimensions");
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
-  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
-              "q, k, v must have the same dtype");
+  check_dtype_device(q, k, v, "q, k, v");
   TORCH_CHECK(k.sizes() == v.sizes(), "k and v must have identical shapes");
   TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), "k/v must share batch and head_dim with q");
-  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
   const int64_t B = q.size(0), Hq = q.size(1), Sq = q.size(2), D = q.size(3), Hkv = k.size(1), Sk = k.size(2);
   TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
   TORCH_CHECK(B >= 1 && Hq >= 1 && Hkv >= 1 && Sq >= 1 && Sk >= 1, "empty tensors are not supported");
@@ -184,14 +202,7 @@ std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Te
     a.num_splits = static_cast<int32_t>(num_splits);
     a.workspace = nullptr; a.workspace_bytes = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    const int nsplit = tfa_attn_num_splits(&a);
-    if (nsplit > 1) {
-      const size_t need = tfa_attn_workspace_bytes(&a, nsplit);
-      ws = torch::empty({static_cast<int64_t>((need + 3) / 4)}, q.options().dtype(at::kFloat));
-      a.workspace = ws.data_ptr();
-      a.workspace_bytes = need;
-      a.num_splits = nsplit;
-    }
+    ws = split_workspace(a, q);
     rc = tfa_attn_fwd(&a);
   }
   raise_on_error(rc);
@@ -209,12 +220,9 @@ std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Ten
   TFA_CHECK_CUDA(k);
   TFA_CHECK_CUDA(v);
   TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3, "q, k, v must have 3 dimensions (total, heads, head_dim)");
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
-  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
-              "q, k, v must have the same dtype");
+  check_dtype_device(q, k, v, "q, k, v");
   TORCH_CHECK(k.sizes() == v.sizes() && k.strides() == v.strides(), "k and v must have identical shapes and strides");
   TORCH_CHECK(k.size(2) == q.size(2), "k/v must share head_dim with q");
-  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
   TORCH_CHECK(q.stride(2) == 1 && k.stride(2) == 1, "q, k, v must have a unit head_dim stride");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt && cu_seqlens_k.scalar_type() == at::kInt,
               "cu_seqlens_q and cu_seqlens_k must be int32");
@@ -279,12 +287,9 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
   TFA_CHECK_CUDA(k_cache);
   TFA_CHECK_CUDA(v_cache);
   TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "q, k_cache, v_cache must have 4 dimensions");
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
-  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
-              "q, k_cache, v_cache must have the same dtype");
+  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
               "k_cache and v_cache must have identical shapes and strides");
-  TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(), "q and the caches must share a device");
   TORCH_CHECK(q.stride(3) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
   TORCH_CHECK(k_cache.size(3) == q.size(3), "the caches must share head_dim with q");
   TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
@@ -362,14 +367,8 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
     d.Sk = static_cast<int32_t>(std::min<int64_t>(mbps * page, 0x7fffffff));
     d.is_causal = a.is_causal;
     d.num_splits = a.num_splits;
-    const int nsplit = tfa_attn_num_splits(&d);
-    if (nsplit > 1) {
-      const size_t need = tfa_attn_workspace_bytes(&d, nsplit);
-      ws = torch::empty({static_cast<int64_t>((need + 3) / 4)}, q.options().dtype(at::kFloat));
-      a.workspace = ws.data_ptr();
-      a.workspace_bytes = need;
-      a.num_splits = nsplit;
-    }
+    ws = split_workspace(d, q);
+    a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
     rc = tfa_attn_kvcache_fwd(&a);
   }
   raise_on_error(rc);

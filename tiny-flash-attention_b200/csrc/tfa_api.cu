@@ -129,12 +129,6 @@ int choose_kernel(bool causal, long long npairs, int n_extra) {
   return npairs <= 8 ? KV_PERSIST : KV_CLASSIC;
 }
 
-// the problem as choose_kernel sees it: Q-tile pairs per head
-int variant_for(bool causal, int Sq, int n_extra) {
-  const long long npairs = (static_cast<long long>(Sq) + 127) / 128;
-  return choose_kernel(causal, npairs, n_extra);
-}
-
 // cudaFuncSetAttribute is per device (context) and costs well under a microsecond: set it on every launch instead of
 // caching "done once" per process, which breaks the first launch on a second GPU of the same process.
 template <typename K>
@@ -142,26 +136,38 @@ cudaError_t opt_in_smem(K kernel, int bytes) {
   return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
 
+// Every launch ends here: count it (tfa_launch_count) and report a launch error.
+int count_launch() {
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return static_cast<int>(cudaGetLastError());
+}
+
+// The fill, combine and append kernels: 256 threads per block, each block taking `per_block` of the `n` rows or chunks.
+template <typename P>
+int launch_small(void (*kern)(P), long long n, int per_block, const P& prm, cudaStream_t stream) {
+  const long long blocks = (n + per_block - 1) / per_block;
+  if (blocks > 0x7fffffffLL) return TFA_EINVAL_SHAPE;
+  kern<<<static_cast<int>(blocks), 256, 0, stream>>>(prm);
+  return count_launch();
+}
+
 template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, int MODE>
 int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
                 int variant, cudaStream_t stream) {
-  cudaError_t cerr = cudaSuccess;
   g_last_variant.store(variant, std::memory_order_relaxed);
+  const bool persist = variant == KV_PERSIST;
   long long nblocks = nitems;
-  if (variant == KV_PERSIST) {
+  if (persist) {
     const int sms = num_sms();
     if (sms <= 0) return TFA_EARCH;
     if (nblocks > sms) nblocks = sms;                                   // one CTA per SM
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, MODE>;
-    if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
-    kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  } else {
-    auto kern = tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
-    if ((cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES)) != cudaSuccess) return static_cast<int>(cerr);
-    kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
   }
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return static_cast<int>(cudaGetLastError());
+  auto kern = persist ? tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, MODE>
+                      : tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
+  const cudaError_t cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES);
+  if (cerr != cudaSuccess) return static_cast<int>(cerr);
+  kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  return count_launch();
 }
 
 template <int D, int MODE>
@@ -176,23 +182,6 @@ int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUte
     else      { if (f32) TFA_GO(false, false, true); else TFA_GO(false, false, false); }
   }
 #undef TFA_GO
-}
-
-// The kernel parameters every forward sets the same way: heads, work-item order, softmax scale, watchdog.
-FwdParams base_params(int Hq, int Hkv, long long npairs, int BH, float scale) {
-  FwdParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.H = Hq;
-  p.kv_group = Hq / Hkv;
-  p.npairs = static_cast<int>(npairs);
-  p.BH = BH;
-  p.head_chunk = p.BH < 8 ? p.BH : 8;
-  p.scale = scale;
-  // scale == 0 is legal (uniform attention over the visible keys): a tiny positive exponent scale keeps
-  // masked scores at -inf (0 * -inf would be NaN) while every visible score still maps to exp2(0) = 1
-  p.scale_log2 = fmaxf(scale * 1.4426950408889634f, 1.0e-30f);
-  p.dbg = g_dbg_dev;
-  return p;
 }
 
 // One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache).
@@ -226,7 +215,8 @@ struct Problem {
   void* out;
   float* lse;
   int B, Hq, Hkv, Sq, Sk, D;
-  long long qsb, qsh, qss, ksb, ksh, kss;   // element strides of q/out and of k/v
+  long long qsb, qsh, qss, ksb, ksh, kss;   // element strides of q and of k/v
+  long long osb, osh, oss, lse_stride_bh;   // where results go: element strides of out, lse elements per (b, h)
   int dtype, causal;
   float scale;
   int out_fp32;
@@ -274,33 +264,122 @@ int resolve_splits(const Problem& a, int want, int sms) {
   return (nkv + tiles - 1) / tiles;                                     // drop empty tail splits
 }
 
+// Split-KV workspace: `nsplit` normalised fp32 partials of the (B, Hq, S, D) output, then their nsplit (B, Hq, S)
+// LSEs (set_output partitions it).  It is sized for the caller's Sq; a dense causal call with Sq > Sk fills it for the
+// Sk rows that see a key.
 size_t splitkv_ws_bytes(const Problem& a, int nsplit) {
   if (nsplit <= 1) return 0;
   return static_cast<size_t>(nsplit) * a.B * a.Hq * a.Sq * (static_cast<size_t>(a.D) + 1) * sizeof(float);
 }
 
+struct SplitPlan {
+  int nsplit;        // work items per Q-tile pair; > 1: partials in the workspace, merged by the combine
+  int split_tiles;   // KV tiles per split
+};
+
+// The split count of a dense or cache call.  Under auto (num_splits == 0) a missing, small or misaligned workspace
+// means one pass; an asked-for count without its workspace is an error.
+int plan_splits(const Problem& a, SplitPlan& plan) {
+  int nsplit = resolve_splits(a, a.num_splits, num_sms());
+  if (nsplit > 1) {
+    const size_t need = splitkv_ws_bytes(a, nsplit);
+    const bool ws_ok = a.ws != nullptr && !(reinterpret_cast<uintptr_t>(a.ws) & 15u) && a.ws_bytes >= need;
+    if (!ws_ok) {
+      if (a.num_splits != 0) return TFA_EINVAL_WORKSPACE;
+      nsplit = 1;                                      // auto: no workspace, no split
+    }
+  }
+  const int nkv_total = (a.Sk + 127) / 128;
+  plan.nsplit = nsplit;
+  plan.split_tiles = (nkv_total + nsplit - 1) / nsplit;
+  return 0;
+}
+
+// Where the forward over S query rows per (batch, head) writes: the caller's out / lse in one pass; with split-KV,
+// contiguous (B, Hq, S, D) fp32 partials per split with their LSEs, which the combine merges into out / lse.
+void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
+  if (nsplit > 1) {
+    const long long rows = static_cast<long long>(a.B) * a.Hq * S;
+    float* ws_o = static_cast<float*>(a.ws);
+    p.out = nullptr;
+    p.out_f32 = ws_o;
+    p.lse = ws_o + static_cast<size_t>(nsplit) * rows * a.D;
+    p.o_stride_s = a.D;
+    p.o_stride_h = static_cast<long long>(S) * a.D;
+    p.o_stride_b = p.o_stride_h * a.Hq;
+    p.part_stride = rows * a.D;
+    p.lse_stride_bh = S;
+    p.lse_part_stride = rows;
+  } else {
+    const bool f32 = a.out_fp32 != 0;
+    p.out = f32 ? nullptr : a.out;
+    p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
+    p.lse = a.lse;
+    p.o_stride_b = a.osb;
+    p.o_stride_h = a.osh;
+    p.o_stride_s = a.oss;
+    p.part_stride = 0;
+    p.lse_stride_bh = a.lse_stride_bh;
+    p.lse_part_stride = 0;
+  }
+}
+
+// the fill and combine kernels take D / 4 threads per row
 template <int D>
 int launch_fill(const tfa::FillParams& fp, bool f32, cudaStream_t stream) {
-  constexpr int RPB = 256 / (D / 4);
-  const long long blocks = (fp.rows + RPB - 1) / RPB;
-  if (blocks > 0x7fffffffLL) return TFA_EINVAL_SHAPE;
-  if (f32) tfa::empty_rows_fill_kernel<D, true><<<static_cast<int>(blocks), 256, 0, stream>>>(fp);
-  else     tfa::empty_rows_fill_kernel<D, false><<<static_cast<int>(blocks), 256, 0, stream>>>(fp);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return static_cast<int>(cudaGetLastError());
+  return launch_small(f32 ? tfa::empty_rows_fill_kernel<D, true> : tfa::empty_rows_fill_kernel<D, false>, fp.rows,
+                      256 / (D / 4), fp, stream);
 }
 
 template <int D>
 int launch_combine(const tfa::CombineParams& cp, bool bf16, bool f32, cudaStream_t stream) {
-  constexpr int RPB = 256 / (D / 4);
-  const long long blocks = (cp.rows + RPB - 1) / RPB;
-  if (blocks > 0x7fffffffLL) return TFA_EINVAL_SHAPE;
-  const int nb = static_cast<int>(blocks);
-  if (f32)       tfa::splitkv_combine_kernel<D, true, true><<<nb, 256, 0, stream>>>(cp);
-  else if (bf16) tfa::splitkv_combine_kernel<D, true, false><<<nb, 256, 0, stream>>>(cp);
-  else           tfa::splitkv_combine_kernel<D, false, false><<<nb, 256, 0, stream>>>(cp);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return static_cast<int>(cudaGetLastError());
+  auto kern = f32 ? tfa::splitkv_combine_kernel<D, true, true>
+                  : bf16 ? tfa::splitkv_combine_kernel<D, true, false> : tfa::splitkv_combine_kernel<D, false, false>;
+  return launch_small(kern, cp.rows, 256 / (D / 4), cp, stream);
+}
+
+// The rest of every forward call.  `p` arrives zeroed with its mode's fields set (Sk / causal_off / extra_dst, cu_q /
+// cu_k, or the cache fields); this sets the fields all modes share, chooses the kernel, launches the forward over S
+// query rows per (batch, head) and, with split-KV, the combine.  With `combine_causal` the combine skips the splits
+// above a row's causal diagonal, which wrote nothing.
+template <int MODE>
+int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, const CUtensorMap& tk,
+                const CUtensorMap& tv, SplitPlan plan, bool combine_causal) {
+  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
+  const long long npairs = (static_cast<long long>(S) + 127) / 128;
+  p.H = a.Hq;
+  p.kv_group = a.Hq / a.Hkv;
+  p.npairs = static_cast<int>(npairs);
+  p.BH = a.B * a.Hq;
+  p.head_chunk = p.BH < 8 ? p.BH : 8;
+  p.scale = a.scale;
+  // scale == 0 is legal (uniform attention over the visible keys): a tiny positive exponent scale keeps
+  // masked scores at -inf (0 * -inf would be NaN) while every visible score still maps to exp2(0) = 1
+  p.scale_log2 = fmaxf(a.scale * 1.4426950408889634f, 1.0e-30f);
+  p.dbg = g_dbg_dev;
+  p.S = S;
+  p.nsplit = plan.nsplit;
+  p.split_tiles = plan.split_tiles;
+  set_output(p, a, S, plan.nsplit);
+
+  const int variant = choose_kernel(causal, npairs, p.n_extra_dst);
+  int rc = launch_fwd<MODE>(a.D, causal, bf16, f32 || plan.nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * plan.nsplit,
+                            variant, a.stream);
+  if (rc || plan.nsplit == 1) return rc;
+
+  tfa::CombineParams cp;
+  cp.o_part = p.out_f32;
+  cp.lse_part = p.lse;
+  cp.out = a.out;
+  cp.lse = a.lse;
+  cp.o_stride_b = a.osb; cp.o_stride_h = a.osh; cp.o_stride_s = a.oss;
+  cp.lse_stride_bh = a.lse_stride_bh;
+  cp.rows = static_cast<long long>(a.B) * a.Hq * S;
+  cp.H = a.Hq; cp.S = S;
+  cp.nsplit = plan.nsplit; cp.split_tiles = plan.split_tiles;
+  cp.nkv_total = (a.Sk + 127) / 128;
+  cp.causal = combine_causal ? 1 : 0; cp.causal_off = p.causal_off;
+  return (a.D == 64) ? launch_combine<64>(cp, bf16, f32, a.stream) : launch_combine<128>(cp, bf16, f32, a.stream);
 }
 
 int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
@@ -308,123 +387,56 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   if (rc) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-  cudaStream_t stream = a.stream;
-  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
+  const bool causal = a.causal != 0, f32 = a.out_fp32 != 0;
   const bool plain = (a.Sq == a.Sk) && (a.Hq == a.Hkv);
   if (n_extra > 0) {
-    // fused exchange: 16-bit output of the reference-shaped problem only
+    // fused exchange: 16-bit output of the reference-shaped problem only, in one pass (tfa_fwd_args has no split
+    // count: from_fwd_args asks for one)
     if (n_extra > 7 || extra_dst == nullptr || f32 || !plain || a.num_splits > 1)
       return TFA_EINVAL_SHAPE;
     for (int i = 0; i < n_extra; ++i)
       if (extra_dst[i] == nullptr || (reinterpret_cast<uintptr_t>(extra_dst[i]) & 15u)) return TFA_EINVAL_PTR;
   }
 
-  int nsplit = (n_extra > 0) ? 1 : resolve_splits(a, a.num_splits, num_sms());
-  if (nsplit > 1) {
-    const size_t need = splitkv_ws_bytes(a, nsplit);
-    const bool ws_ok = a.ws != nullptr && !(reinterpret_cast<uintptr_t>(a.ws) & 15u) && a.ws_bytes >= need;
-    if (!ws_ok) {
-      if (a.num_splits == 0) nsplit = 1;               // auto: no workspace, no split
-      else return TFA_EINVAL_WORKSPACE;
-    }
-  }
-
-  const long long lse_stride_bh = a.Sq;                // of the caller's (B, Hq, Sq) tensor
-  const size_t osz = f32 ? 4 : 2;
+  SplitPlan plan;
+  if ((rc = plan_splits(a, plan))) return rc;
 
   // causal with more queries than keys: rows [0, Sq-Sk) see nothing; the rest is a square causal problem
   if (causal && a.Sk < a.Sq) {
     const int n_empty = a.Sq - a.Sk;
     tfa::FillParams fp;
     fp.out = a.out; fp.lse = a.lse;
-    fp.o_stride_b = a.qsb; fp.o_stride_h = a.qsh; fp.o_stride_s = a.qss;
-    fp.lse_stride_bh = lse_stride_bh;
+    fp.o_stride_b = a.osb; fp.o_stride_h = a.osh; fp.o_stride_s = a.oss;
+    fp.lse_stride_bh = a.lse_stride_bh;
     fp.rows = static_cast<long long>(a.B) * a.Hq * n_empty;
     fp.H = a.Hq; fp.n_empty = n_empty;
-    rc = (a.D == 64) ? launch_fill<64>(fp, f32, stream) : launch_fill<128>(fp, f32, stream);
+    rc = (a.D == 64) ? launch_fill<64>(fp, f32, a.stream) : launch_fill<128>(fp, f32, a.stream);
     if (rc) return rc;
     a.q = static_cast<const char*>(a.q) + static_cast<size_t>(n_empty) * a.qss * 2;
-    a.out = static_cast<char*>(a.out) + static_cast<size_t>(n_empty) * a.qss * osz;
+    a.out = static_cast<char*>(a.out) + static_cast<size_t>(n_empty) * a.oss * (f32 ? 4 : 2);
     if (a.lse) a.lse += n_empty;
     a.Sq = a.Sk;
   }
-  const int causal_off = causal ? a.Sk - a.Sq : 0;     // >= 0 from here on
-
-  const long long npairs = (static_cast<long long>(a.Sq) + 127) / 128;
-  const int nkv_total = (a.Sk + 127) / 128;
-  const int split_tiles = (nkv_total + nsplit - 1) / nsplit;
 
   CUtensorMap tq, tk, tv;
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
   if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
   if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
 
-  const int variant = variant_for(causal, a.Sq, n_extra);
-
-  const long long rows = static_cast<long long>(a.B) * a.Hq * a.Sq;
-  float* ws_o = static_cast<float*>(a.ws);
-  float* ws_lse = ws_o ? ws_o + static_cast<size_t>(nsplit) * rows * a.D : nullptr;
-
-  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
-  p.S = a.Sq;
+  FwdParams p{};
   p.Sk = a.Sk;
-  p.causal_off = causal_off;
-  p.nsplit = nsplit;
-  p.split_tiles = split_tiles;
-  if (nsplit > 1) {
-    // partials: contiguous (B, Hq, Sq, D) fp32 per split, normalised, with their LSEs
-    p.out = nullptr;
-    p.out_f32 = ws_o;
-    p.lse = ws_lse;
-    p.o_stride_s = a.D;
-    p.o_stride_h = static_cast<long long>(a.Sq) * a.D;
-    p.o_stride_b = p.o_stride_h * a.Hq;
-    p.part_stride = rows * a.D;
-    p.lse_stride_bh = a.Sq;
-    p.lse_part_stride = rows;
-  } else {
-    p.out = f32 ? nullptr : a.out;
-    p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
-    p.lse = a.lse;
-    p.o_stride_b = a.qsb;
-    p.o_stride_h = a.qsh;
-    p.o_stride_s = a.qss;
-    p.part_stride = 0;
-    p.lse_stride_bh = lse_stride_bh;
-    p.lse_part_stride = 0;
-  }
+  p.causal_off = causal ? a.Sk - a.Sq : 0;             // >= 0 after the shift
   for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
   p.n_extra_dst = n_extra;
-
-  const long long nitems = npairs * a.B * a.Hq * nsplit;
-  const bool kernel_f32 = f32 || nsplit > 1;
-  rc = launch_fwd<tfa::kDense>(a.D, causal, bf16, kernel_f32, tq, tk, tv, p, nitems, variant, stream);
-  if (rc) return rc;
-
-  if (nsplit > 1) {
-    tfa::CombineParams cp;
-    cp.o_part = ws_o;
-    cp.lse_part = ws_lse;
-    cp.out = a.out;
-    cp.lse = a.lse;
-    cp.o_stride_b = a.qsb; cp.o_stride_h = a.qsh; cp.o_stride_s = a.qss;
-    cp.lse_stride_bh = lse_stride_bh;
-    cp.rows = rows;
-    cp.H = a.Hq; cp.S = a.Sq;
-    cp.nsplit = nsplit; cp.split_tiles = split_tiles;
-    cp.nkv_total = nkv_total;
-    cp.causal = causal ? 1 : 0; cp.causal_off = causal_off;
-    rc = (a.D == 64) ? launch_combine<64>(cp, bf16, f32, stream) : launch_combine<128>(cp, bf16, f32, stream);
-    if (rc) return rc;
-  }
-  return 0;
+  return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan, causal);
 }
 
 Problem from_fwd_args(const tfa_fwd_args& a) {
   Problem q;
   q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
   q.B = a.B; q.Hq = a.H; q.Hkv = a.H; q.Sq = a.S; q.Sk = a.S; q.D = a.D;
-  q.qsb = q.ksb = a.stride_b; q.qsh = q.ksh = a.stride_h; q.qss = q.kss = a.stride_s;
+  q.qsb = q.ksb = q.osb = a.stride_b; q.qsh = q.ksh = q.osh = a.stride_h; q.qss = q.kss = q.oss = a.stride_s;
+  q.lse_stride_bh = a.S;
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -435,8 +447,9 @@ Problem from_attn_args(const tfa_attn_args& a) {
   Problem q;
   q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.Sq; q.Sk = a.Sk; q.D = a.D;
-  q.qsb = a.q_stride_b; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.qsb = q.osb = a.q_stride_b; q.qsh = q.osh = a.q_stride_h; q.qss = q.oss = a.q_stride_s;
   q.ksb = a.kv_stride_b; q.ksh = a.kv_stride_h; q.kss = a.kv_stride_s;
+  q.lse_stride_bh = a.Sq;
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -450,6 +463,8 @@ Problem from_varlen_args(const tfa_attn_varlen_args& a) {
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.Sk = a.total_k; q.D = a.D;
   q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
   q.ksb = 0; q.ksh = a.kv_stride_h; q.kss = a.kv_stride_s;
+  q.osb = 0; q.osh = a.D; q.oss = static_cast<long long>(a.Hq) * a.D;   // out is (total_q, Hq, D) contiguous
+  q.lse_stride_bh = a.total_q;                                          // lse is (Hq, total_q)
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -466,32 +481,20 @@ int varlen_impl(const tfa_attn_varlen_args& va) {
   if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
 
   CUtensorMap tq, tk, tv;
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
   if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
   if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
 
-  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once
-  const long long npairs = (static_cast<long long>(va.max_seqlen_q) + 127) / 128;
-  const int variant = choose_kernel(causal, npairs, 0);
-
-  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
-  p.S = va.max_seqlen_q;
-  p.nsplit = 1;
-  p.split_tiles = 0x7fffffff;          // one split holds every KV tile of any sequence
-  p.out = f32 ? nullptr : a.out;
-  p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
-  p.lse = a.lse;
-  p.o_stride_s = static_cast<long long>(a.Hq) * a.D;     // out is (total_q, Hq, D) contiguous
-  p.o_stride_h = a.D;
-  p.lse_stride_bh = a.Sq;                                // lse is (Hq, total_q)
+  FwdParams p{};
   p.cu_q = va.cu_seqlens_q;
   p.cu_k = va.cu_seqlens_k;
   p.total_q = a.Sq;
   p.total_k = a.Sk;
-  return launch_fwd<tfa::kVarlen>(a.D, causal, bf16, f32, tq, tk, tv, p, npairs * a.B * a.Hq, variant, a.stream);
+  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once.  One
+  // split holds every KV tile of any sequence.
+  return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
 }
 
 // The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
@@ -501,8 +504,9 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.Sq; q.D = a.D;
   const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
   q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
-  q.qsb = a.q_stride_b; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.qsb = q.osb = a.q_stride_b; q.qsh = q.osh = a.q_stride_h; q.qss = q.oss = a.q_stride_s;
   q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
+  q.lse_stride_bh = a.Sq;
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -532,27 +536,18 @@ int validate_kvcache(const tfa_attn_kvcache_args& ka) {
 }
 
 int kvcache_impl(const tfa_attn_kvcache_args& ka) {
-  Problem a = from_kvcache_args(ka);
+  const Problem a = from_kvcache_args(ka);
   int rc = validate_kvcache(ka);        // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-  cudaStream_t stream = a.stream;
-  const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
   const int capacity = a.Sk;
   const int snew = ka.k_new ? ka.Snew : 0;
   const int page = ka.block_table ? ka.page_block_size : capacity;
 
-  int nsplit = resolve_splits(a, a.num_splits, num_sms());
-  if (nsplit > 1) {
-    const size_t need = splitkv_ws_bytes(a, nsplit);
-    const bool ws_ok = a.ws != nullptr && !(reinterpret_cast<uintptr_t>(a.ws) & 15u) && a.ws_bytes >= need;
-    if (!ws_ok) {
-      if (a.num_splits == 0) nsplit = 1;               // auto: no workspace, no split
-      else return TFA_EINVAL_WORKSPACE;
-    }
-  }
+  SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
+  if ((rc = plan_splits(a, plan))) return rc;
 
   CUtensorMap tq, tk, tv;
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
@@ -567,72 +562,20 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka) {
     ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
     ap.page = page; ap.capacity = capacity; ap.snew = snew; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
     ap.chunks = static_cast<long long>(a.B) * snew * a.Hkv * (a.D / 8);
-    const long long blocks = (ap.chunks + 255) / 256;
-    if (blocks > 0x7fffffffLL) return TFA_EINVAL_SHAPE;
-    if (a.D == 64) tfa::kvcache_append_kernel<64><<<static_cast<int>(blocks), 256, 0, stream>>>(ap);
-    else           tfa::kvcache_append_kernel<128><<<static_cast<int>(blocks), 256, 0, stream>>>(ap);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    if ((rc = static_cast<int>(cudaGetLastError()))) return rc;
+    rc = launch_small(a.D == 64 ? tfa::kvcache_append_kernel<64> : tfa::kvcache_append_kernel<128>, ap.chunks, 256, ap,
+                      a.stream);
+    if (rc) return rc;
   }
 
-  const long long npairs = (static_cast<long long>(a.Sq) + 127) / 128;
-  const int nkv_total = (capacity + 127) / 128;
-  const int split_tiles = (nkv_total + nsplit - 1) / nsplit;
-  const int variant = choose_kernel(causal, npairs, 0);
-  const long long rows = static_cast<long long>(a.B) * a.Hq * a.Sq;
-  float* ws_o = static_cast<float*>(a.ws);
-  float* ws_lse = ws_o ? ws_o + static_cast<size_t>(nsplit) * rows * a.D : nullptr;
-
-  FwdParams p = base_params(a.Hq, a.Hkv, npairs, a.B * a.Hq, a.scale);
-  p.S = a.Sq;
-  p.nsplit = nsplit;
-  p.split_tiles = split_tiles;
-  if (nsplit > 1) {
-    // partials: contiguous (B, Hq, Sq, D) fp32 per split, as fwd_impl's
-    p.out_f32 = ws_o;
-    p.lse = ws_lse;
-    p.o_stride_s = a.D;
-    p.o_stride_h = static_cast<long long>(a.Sq) * a.D;
-    p.o_stride_b = p.o_stride_h * a.Hq;
-    p.part_stride = rows * a.D;
-    p.lse_stride_bh = a.Sq;
-    p.lse_part_stride = rows;
-  } else {
-    p.out = f32 ? nullptr : a.out;
-    p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
-    p.lse = a.lse;
-    p.o_stride_b = a.qsb;
-    p.o_stride_h = a.qsh;
-    p.o_stride_s = a.qss;
-    p.lse_stride_bh = a.Sq;
-  }
+  FwdParams p{};
   p.cache_seqlens = ka.cache_seqlens;
   p.block_table = ka.block_table;
   p.bt_stride = ka.block_table_stride;
   p.page = page;
   p.capacity = capacity;
   p.snew = snew;
-  rc = launch_fwd<tfa::kCache>(a.D, causal, bf16, f32 || nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * nsplit,
-                               variant, stream);
-  if (rc) return rc;
-
-  if (nsplit > 1) {
-    // every split wrote its rows (LSE = -inf where it saw no key): causal = 0 makes the combine read all of them
-    tfa::CombineParams cp;
-    cp.o_part = ws_o;
-    cp.lse_part = ws_lse;
-    cp.out = a.out;
-    cp.lse = a.lse;
-    cp.o_stride_b = a.qsb; cp.o_stride_h = a.qsh; cp.o_stride_s = a.qss;
-    cp.lse_stride_bh = a.Sq;
-    cp.rows = rows;
-    cp.H = a.Hq; cp.S = a.Sq;
-    cp.nsplit = nsplit; cp.split_tiles = split_tiles;
-    cp.nkv_total = nkv_total;
-    cp.causal = 0; cp.causal_off = 0;
-    rc = (a.D == 64) ? launch_combine<64>(cp, bf16, f32, stream) : launch_combine<128>(cp, bf16, f32, stream);
-  }
-  return rc;
+  // every split writes its rows (LSE = -inf where it saw no key): the combine reads all of them
+  return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan, false);
 }
 
 // ---- host-buffer path workspace ----
@@ -797,7 +740,7 @@ int tfa_internal_last_variant(void) { return g_last_variant.load(); }
 // takes the whole problem shape, of which the rule reads the mask, the query length and the exchange
 int tfa_internal_choose_kernel(int D, int causal, int Sq, int Sk, int B, int Hq, int nsplit, int sms, int n_extra) {
   (void)D; (void)Sk; (void)B; (void)Hq; (void)nsplit; (void)sms;
-  return variant_for(causal != 0, Sq, n_extra);
+  return choose_kernel(causal != 0, (static_cast<long long>(Sq) + 127) / 128, n_extra);
 }
 // exported for the self tests living in another translation unit
 void tfa_internal_count_launch(void) { g_launches.fetch_add(1, std::memory_order_relaxed); }

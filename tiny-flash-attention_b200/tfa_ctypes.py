@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("TFA_LIB", os.path.join(HERE, "libtfa_b200.so"))   # T
 
 TFA_BF16, TFA_FP16 = 0, 1
 _LIB = None
-_WORKSPACES = {}     # (device, stream) -> last split-KV workspace, see attn_fwd()
+_WORKSPACES = {}     # (device, stream) -> last split-KV workspace, see _split_workspace()
 
 
 class TfaError(RuntimeError):
@@ -170,6 +170,22 @@ def fwd(q, k, v, is_causal, softmax_scale, out_fp32=False, layout="bhsd", stream
     return out, lse
 
 
+def _split_workspace(dense, args, device, stream):
+    """Split count of the dense problem `dense` (AttnArgs).  When it splits, allocates the workspace on `device` and
+    sets num_splits / workspace / workspace_bytes in `args` (`dense` itself, or the call's own argument struct)."""
+    import torch
+    L = lib()
+    n = int(L.tfa_attn_num_splits(ctypes.byref(dense)))
+    if n > 1:
+        need = int(L.tfa_attn_workspace_bytes(ctypes.byref(dense), n))
+        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=device)
+        args.workspace, args.workspace_bytes, args.num_splits = ws.data_ptr(), need, n
+        # the launch is asynchronous: keep the workspace alive until the next call on the same stream (which is
+        # ordered behind this one) instead of handing it back to the allocator while the kernels may still run
+        _WORKSPACES[(device.index, int(stream))] = ws
+    return n
+
+
 def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, stream=None, return_splits=False):
     """Generalised problem through tfa_attn_fwd(): q (B,Hq,Sq,D), k/v (B,Hkv,Sk,D) contiguous device tensors,
     bottom-right causal mask, optional split-KV (num_splits: 1 none, n > 1 as asked, 0 library heuristic)."""
@@ -183,16 +199,8 @@ def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, st
     a = AttnArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), B, Hq, Hkv, Sq, Sk, D,
                  Hq * Sq * D, Sq * D, D, Hkv * Sk * D, Sk * D, D, _dtype_code(q), int(bool(is_causal)),
                  float(softmax_scale), int(bool(out_fp32)), int(num_splits), None, 0, st)
-    L = lib()
-    n = int(L.tfa_attn_num_splits(ctypes.byref(a)))
-    if n > 1:
-        need = int(L.tfa_attn_workspace_bytes(ctypes.byref(a), n))
-        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=q.device)
-        a.workspace, a.workspace_bytes, a.num_splits = ws.data_ptr(), need, n
-        # the launch is asynchronous: keep the workspace alive until the next call on the same stream (which is
-        # ordered behind this one) instead of handing it back to the allocator while the kernels may still run
-        _WORKSPACES[(q.device.index, int(st))] = ws
-    check(L.tfa_attn_fwd(ctypes.byref(a)))
+    n = _split_workspace(a, a, q.device, st)
+    check(lib().tfa_attn_fwd(ctypes.byref(a)))
     if return_splits:
         return out, lse, n
     return out, lse
@@ -257,17 +265,11 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
                     q.stride(0), q.stride(1), q.stride(2), k_cache.stride(0), k_cache.stride(1), k_cache.stride(2),
                     bts, ns[0], ns[1], ns[2], _dtype_code(q), int(bool(is_causal)), float(scale),
                     int(bool(out_fp32)), int(num_splits), None, 0, st)
-    L = lib()
     # the split count and workspace of the dense problem with Sk = capacity
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
-    n = int(L.tfa_attn_num_splits(ctypes.byref(dense)))
-    if n > 1:
-        need = int(L.tfa_attn_workspace_bytes(ctypes.byref(dense), n))
-        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=q.device)
-        a.workspace, a.workspace_bytes, a.num_splits = ws.data_ptr(), need, n
-        _WORKSPACES[(q.device.index, int(st))] = ws      # alive until the next call on this stream, as attn_fwd()
-    check(L.tfa_attn_kvcache_fwd(ctypes.byref(a)))
+    n = _split_workspace(dense, a, q.device, st)
+    check(lib().tfa_attn_kvcache_fwd(ctypes.byref(a)))
     if return_splits:
         return out, lse, n
     return out, lse
