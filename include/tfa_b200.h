@@ -55,6 +55,8 @@ extern "C" {
 #define TFA_EINVAL_KVCACHE (-13)   /* KV cache: cache_seqlens / block_table null or misaligned, page size not a multiple
                                       of 128, num_blocks or max_blocks_per_seq < 1, one of k_new / v_new, Snew not in
                                       [1, capacity] */
+#define TFA_EINVAL_ROTARY (-14)    /* rotary: cos / sin / q_rot null or misaligned, rotary_dim not an even multiple of 16
+                                      in [16, D], seqlen_ro < capacity, or no k_new */
 
 /* Extended argument block (POD), the analogue of Flash_fwd_params (flash.h:29-60).
  * Strides are in ELEMENTS.  The innermost (head_dim) stride must be 1.
@@ -180,8 +182,8 @@ typedef struct tfa_attn_varlen_args {
 
 int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args);
 
-/* ---- attention against a (paged) KV cache: the decode step of a serving loop (flash-attn's flash_attn_with_kvcache,
- * without rotary) ----
+/* ---- attention against a (paged) KV cache: the decode step of a serving loop (flash-attn's flash_attn_with_kvcache;
+ * with rotary see tfa_attn_kvcache_rotary_fwd below) ----
  * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
  * tfa_attn_kvcache_fwd.
  *
@@ -236,6 +238,37 @@ typedef struct tfa_attn_kvcache_args {
 } tfa_attn_kvcache_args;
 
 int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args);
+
+/* ---- the KV-cache forward with rotary position embedding (flash-attn's flash_attn_with_kvcache with rotary_cos,
+ * rotary_sin and rotary_interleaved) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_kvcache_rotary_fwd.  tfa_attn_kvcache_fwd() with, before the attention, q and k_new rotated at their
+ * absolute positions in one launch: rot(q) goes to q_rot, which the attention reads in place of q, and rot(k_new) with
+ * the unrotated v_new goes into the cache.  The caller's q and k_new are not modified.
+ *
+ *   cos, sin   : (seqlen_ro, rotary_dim / 2) contiguous DEVICE arrays in q's dtype, 16-byte aligned.
+ *   seqlen_ro  : >= capacity (= max_blocks_per_seq * page_block_size).
+ *   rotary_dim : a multiple of 16 in [16, D].  Dimensions [rotary_dim, D) pass through unchanged.
+ *   interleaved: 0 = GPT-NeoX pairs (j, j + rotary_dim/2), != 0 = GPT-J pairs (2j, 2j+1); pair j takes cos[pos][j] and
+ *              sin[pos][j], and becomes x0' = x0 c - x1 s, x1' = x0 s + x1 c, computed in fp32 with one rounding per
+ *              operation (no FMA) and rounded once to q's dtype.
+ *   q_rot      : (B, Sq, Hq, D) contiguous DEVICE scratch in q's dtype, 16-byte aligned; it must not overlap any other
+ *              argument.  Holds rot(q) after the call.
+ *   positions  : with L_b the clamped cached length of tfa_attn_kvcache_fwd(), appended key i of sequence b is rotated
+ *              at L_b + i; query row i at L_b + i when causal, at L_b for every row otherwise (equal to the key
+ *              positions when Sq == Snew).  A query position past seqlen_ro - 1 (Sq > Snew near the capacity) is
+ *              clamped to seqlen_ro - 1.
+ * k_new / v_new are required (TFA_EINVAL_ROTARY otherwise).  out keeps q's strides.  Every argument is checked before
+ * any device work.  Launches: 2 (the rotary append, the attention), + 1 with split-KV; CUDA-graph capturable as
+ * tfa_attn_kvcache_fwd(). */
+typedef struct tfa_rotary_args {
+  const void* cos;
+  const void* sin;
+  int32_t seqlen_ro, rotary_dim, interleaved;
+  void* q_rot;
+} tfa_rotary_args;
+
+int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

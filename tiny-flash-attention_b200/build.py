@@ -33,7 +33,7 @@ CXX = os.environ.get("CXX", "g++")
 LIB_NAME = "libtfa_b200.so"
 EXT_NAME = "attention_cutlass" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so")
 
-CU_SOURCES = ["tfa_api.cu", "tfa_selftest.cu"]
+CU_SOURCES = ["tfa_api.cu", "tfa_rotary.cu", "tfa_selftest.cu"]
 CU_HEADERS = ["ptx_sm90.cuh", "fa_fwd_sm90.cuh", "fa_splitkv_combine.cuh"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [

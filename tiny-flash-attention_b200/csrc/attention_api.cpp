@@ -273,16 +273,20 @@ std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Ten
   return {out, lse};
 }
 
-// Attention against a KV cache (flash-attn's flash_attn_with_kvcache without rotary): q (B, Sq, Hq, D);
-// k_cache / v_cache (num_blocks, page_block_size, Hkv, D) with block_table int32 (B, max_blocks_per_seq), or a
-// contiguous (B, capacity, Hkv, D) cache with block_table None; cache_seqlens int32 (B); k_new / v_new None or
-// (B, Snew, Hkv, D), written into the cache in place at keys [cache_seqlens[b], + Snew) before the attention.
-// Returns out (B, Sq, Hq, D) and lse (B, Hq, Sq).  num_splits as flash_attention_v2_general.
-std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache,
-                                                      torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table,
-                                                      std::optional<torch::Tensor> k_new,
-                                                      std::optional<torch::Tensor> v_new, bool is_causal,
-                                                      float softmax_scale, int64_t num_splits) {
+namespace {
+
+// A KV-cache call's tensors after check_kvcache(): the optional ones resolved, and the shape facts the fill needs.
+struct KvcacheCall {
+  torch::Tensor q, k_cache, v_cache, cache_seqlens;
+  std::optional<torch::Tensor> block_table, k_new, v_new;
+  int64_t B, Sq, Hq, D, nblk, page, Hkv, mbps, bts, snew;
+};
+
+// Every check of a KV-cache call; throws on a bad argument, before any device work.
+KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
+                          const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
+                          const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
+                          int64_t num_splits) {
   TFA_CHECK_CUDA(q);
   TFA_CHECK_CUDA(k_cache);
   TFA_CHECK_CUDA(v_cache);
@@ -295,81 +299,152 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
   TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
                   cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == q.size(0),
               "cache_seqlens must be a contiguous int32 (B,) tensor on q's device");
-  const int64_t B = q.size(0), Sq = q.size(1), Hq = q.size(2), D = q.size(3);
-  const int64_t nblk = k_cache.size(0), page = k_cache.size(1), Hkv = k_cache.size(2);
-  int64_t mbps = 1, bts = 1;
+  KvcacheCall c{q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new};
+  c.B = q.size(0); c.Sq = q.size(1); c.Hq = q.size(2); c.D = q.size(3);
+  c.nblk = k_cache.size(0); c.page = k_cache.size(1); c.Hkv = k_cache.size(2);
+  c.mbps = 1; c.bts = 1;
   if (block_table.has_value()) {
     const torch::Tensor& bt = *block_table;
-    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == B &&
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == c.B &&
                     bt.stride(1) == 1,
                 "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
-    TORCH_CHECK(page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
-                                         static_cast<long long>(page)));
-    mbps = bt.size(1);
-    bts = bt.stride(0);
+    TORCH_CHECK(c.page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
+                                           static_cast<long long>(c.page)));
+    c.mbps = bt.size(1);
+    c.bts = bt.stride(0);
   } else {
-    TORCH_CHECK(nblk == B, "without block_table the caches must be (B, capacity, Hkv, D)");
+    TORCH_CHECK(c.nblk == c.B, "without block_table the caches must be (B, capacity, Hkv, D)");
   }
   TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
-  int64_t snew = 0;
+  c.snew = 0;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
     TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
                     vn.scalar_type() == q.scalar_type(),
                 "k_new and v_new must be on q's device with q's dtype");
-    TORCH_CHECK(kn.dim() == 4 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == B &&
-                    kn.size(2) == Hkv && kn.size(3) == D && kn.stride(3) == 1,
+    TORCH_CHECK(kn.dim() == 4 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == c.B &&
+                    kn.size(2) == c.Hkv && kn.size(3) == c.D && kn.stride(3) == 1,
                 "k_new and v_new must be (B, Snew, Hkv, D) with identical strides and a unit head_dim stride");
-    snew = kn.size(1);
-    TORCH_CHECK(snew >= 1 && snew <= mbps * page, "Snew must be in [1, capacity]");
+    c.snew = kn.size(1);
+    TORCH_CHECK(c.snew >= 1 && c.snew <= c.mbps * c.page, "Snew must be in [1, capacity]");
   }
-  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
-  TORCH_CHECK(B >= 1 && Sq >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
-  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
-                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(c.D == 64 || c.D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(c.D)));
+  TORCH_CHECK(c.B >= 1 && c.Sq >= 1 && c.Hq >= 1 && c.Hkv >= 1, "empty tensors are not supported");
+  TORCH_CHECK(c.Hq % c.Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                         static_cast<long long>(c.Hq), static_cast<long long>(c.Hkv)));
   TORCH_CHECK(num_splits >= 0 && num_splits <= 1024, "num_splits must be in [0, 1024]");
+  return c;
+}
 
+// Under q's device guard: allocates out (q's strides; a non-dense q is replaced by its contiguous copy first) and lse,
+// fills `a`, and allocates the split-KV workspace (returned; the caller keeps it until the launch is enqueued).
+torch::Tensor fill_kvcache(KvcacheCall& c, bool is_causal, float softmax_scale, int64_t num_splits,
+                           tfa_attn_kvcache_args& a, torch::Tensor& out, torch::Tensor& lse) {
+  out = torch::empty_like(c.q);
+  if (out.strides() != c.q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
+    c.q = c.q.contiguous();
+    out = torch::empty_like(c.q);
+  }
+  lse = torch::empty({c.B, c.Hq, c.Sq}, c.q.options().dtype(at::kFloat));
+  std::memset(&a, 0, sizeof(a));
+  a.q = c.q.data_ptr(); a.k_cache = c.k_cache.data_ptr(); a.v_cache = c.v_cache.data_ptr();
+  a.k_new = c.snew ? c.k_new->data_ptr() : nullptr;
+  a.v_new = c.snew ? c.v_new->data_ptr() : nullptr;
+  a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+  a.cache_seqlens = c.cache_seqlens.data_ptr<int32_t>();
+  a.block_table = c.block_table.has_value() ? c.block_table->data_ptr<int32_t>() : nullptr;
+  a.B = static_cast<int32_t>(c.B); a.Hq = static_cast<int32_t>(c.Hq); a.Hkv = static_cast<int32_t>(c.Hkv);
+  a.Sq = static_cast<int32_t>(c.Sq); a.D = static_cast<int32_t>(c.D);
+  a.num_blocks = static_cast<int32_t>(c.nblk); a.page_block_size = static_cast<int32_t>(c.page);
+  a.max_blocks_per_seq = static_cast<int32_t>(c.mbps); a.Snew = static_cast<int32_t>(c.snew);
+  a.q_stride_b = c.q.stride(0); a.q_stride_s = c.q.stride(1); a.q_stride_h = c.q.stride(2);
+  a.cache_stride_block = c.k_cache.stride(0); a.cache_stride_s = c.k_cache.stride(1);
+  a.cache_stride_h = c.k_cache.stride(2);
+  a.block_table_stride = c.bts;
+  if (c.snew) {
+    a.new_stride_b = c.k_new->stride(0); a.new_stride_s = c.k_new->stride(1); a.new_stride_h = c.k_new->stride(2);
+  }
+  a.dtype = c.q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+  a.is_causal = is_causal ? 1 : 0;
+  a.softmax_scale = softmax_scale;
+  a.num_splits = static_cast<int32_t>(num_splits);
+  a.stream = at::cuda::getCurrentCUDAStream(c.q.device().index()).stream();
+  // split count and workspace: those of the dense problem with Sk = capacity
+  tfa_attn_args d;
+  std::memset(&d, 0, sizeof(d));
+  d.B = a.B; d.Hq = a.Hq; d.Hkv = a.Hkv; d.Sq = a.Sq; d.D = a.D;
+  d.Sk = static_cast<int32_t>(std::min<int64_t>(c.mbps * c.page, 0x7fffffff));
+  d.is_causal = a.is_causal;
+  d.num_splits = a.num_splits;
+  torch::Tensor ws = split_workspace(d, c.q);
+  a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
+  return ws;
+}
+
+}  // namespace
+
+// Attention against a KV cache (flash-attn's flash_attn_with_kvcache without rotary): q (B, Sq, Hq, D);
+// k_cache / v_cache (num_blocks, page_block_size, Hkv, D) with block_table int32 (B, max_blocks_per_seq), or a
+// contiguous (B, capacity, Hkv, D) cache with block_table None; cache_seqlens int32 (B); k_new / v_new None or
+// (B, Snew, Hkv, D), written into the cache in place at keys [cache_seqlens[b], + Snew) before the attention.
+// Returns out (B, Sq, Hq, D) and lse (B, Hq, Sq).  num_splits as flash_attention_v2_general.
+std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache,
+                                                      torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table,
+                                                      std::optional<torch::Tensor> k_new,
+                                                      std::optional<torch::Tensor> v_new, bool is_causal,
+                                                      float softmax_scale, int64_t num_splits) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
   torch::Tensor out, lse, ws;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
-    out = torch::empty_like(q);
-    if (out.strides() != q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
-      q = q.contiguous();
-      out = torch::empty_like(q);
-    }
-    lse = torch::empty({B, Hq, Sq}, q.options().dtype(at::kFloat));
     tfa_attn_kvcache_args a;
-    std::memset(&a, 0, sizeof(a));
-    a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr();
-    a.k_new = snew ? k_new->data_ptr() : nullptr;
-    a.v_new = snew ? v_new->data_ptr() : nullptr;
-    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
-    a.cache_seqlens = cache_seqlens.data_ptr<int32_t>();
-    a.block_table = block_table.has_value() ? block_table->data_ptr<int32_t>() : nullptr;
-    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
-    a.Sq = static_cast<int32_t>(Sq); a.D = static_cast<int32_t>(D);
-    a.num_blocks = static_cast<int32_t>(nblk); a.page_block_size = static_cast<int32_t>(page);
-    a.max_blocks_per_seq = static_cast<int32_t>(mbps); a.Snew = static_cast<int32_t>(snew);
-    a.q_stride_b = q.stride(0); a.q_stride_s = q.stride(1); a.q_stride_h = q.stride(2);
-    a.cache_stride_block = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1); a.cache_stride_h = k_cache.stride(2);
-    a.block_table_stride = bts;
-    if (snew) { a.new_stride_b = k_new->stride(0); a.new_stride_s = k_new->stride(1); a.new_stride_h = k_new->stride(2); }
-    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
-    a.is_causal = is_causal ? 1 : 0;
-    a.softmax_scale = softmax_scale;
-    a.num_splits = static_cast<int32_t>(num_splits);
-    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    // split count and workspace: those of the dense problem with Sk = capacity
-    tfa_attn_args d;
-    std::memset(&d, 0, sizeof(d));
-    d.B = a.B; d.Hq = a.Hq; d.Hkv = a.Hkv; d.Sq = a.Sq; d.D = a.D;
-    d.Sk = static_cast<int32_t>(std::min<int64_t>(mbps * page, 0x7fffffff));
-    d.is_causal = a.is_causal;
-    d.num_splits = a.num_splits;
-    ws = split_workspace(d, q);
-    a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
+    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
     rc = tfa_attn_kvcache_fwd(&a);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
+// The same with rotary position embedding (flash-attn's rotary_cos / rotary_sin / rotary_interleaved): q and k_new
+// are rotated at their absolute positions (tfa_attn_kvcache_rotary_fwd in include/tfa_b200.h) before the attention;
+// the caller's q and k_new are not modified.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) contiguous in q's
+// dtype on q's device, seqlen_ro >= capacity, rotary_dim a multiple of 16 in [16, D]; k_new / v_new are required.
+std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
+    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
+    torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved, bool is_causal, float softmax_scale,
+    int64_t num_splits) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
+  TORCH_CHECK(c.snew > 0, "rotary needs k_new and v_new: it rotates the appended keys");
+  TORCH_CHECK(rotary_cos.device() == q.device() && rotary_sin.device() == q.device(),
+              "rotary_cos and rotary_sin must be on q's device");
+  TORCH_CHECK(rotary_cos.scalar_type() == q.scalar_type() && rotary_sin.scalar_type() == q.scalar_type(),
+              "rotary_cos and rotary_sin must have q's dtype");
+  TORCH_CHECK(rotary_cos.dim() == 2 && rotary_cos.sizes() == rotary_sin.sizes(),
+              "rotary_cos and rotary_sin must both be (seqlen_ro, rotary_dim / 2)");
+  TORCH_CHECK(rotary_cos.is_contiguous() && rotary_sin.is_contiguous(), "rotary_cos and rotary_sin must be contiguous");
+  const int64_t seqlen_ro = rotary_cos.size(0), rotary_dim = 2 * rotary_cos.size(1);
+  TORCH_CHECK(rotary_dim >= 16 && rotary_dim <= c.D && rotary_dim % 16 == 0,
+              fmt_msg("rotary_dim (2 * rotary_cos.size(1) = %lld) must be a multiple of 16 in [16, head_dim = %lld]",
+                      static_cast<long long>(rotary_dim), static_cast<long long>(c.D)));
+  TORCH_CHECK(seqlen_ro < (1LL << 31), "rotary_cos and rotary_sin are too large");
+  TORCH_CHECK(seqlen_ro >= c.mbps * c.page,
+              fmt_msg("rotary_cos / rotary_sin need a row per cache position: seqlen_ro = %lld < capacity = %lld",
+                      static_cast<long long>(seqlen_ro), static_cast<long long>(c.mbps * c.page)));
+  torch::Tensor out, lse, ws, q_rot;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    tfa_attn_kvcache_args a;
+    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
+    q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
+    tfa_rotary_args r;
+    r.cos = rotary_cos.data_ptr(); r.sin = rotary_sin.data_ptr();
+    r.seqlen_ro = static_cast<int32_t>(seqlen_ro); r.rotary_dim = static_cast<int32_t>(rotary_dim);
+    r.interleaved = rotary_interleaved ? 1 : 0;
+    r.q_rot = q_rot.data_ptr();
+    rc = tfa_attn_kvcache_rotary_fwd(&a, &r);
   }
   raise_on_error(rc);
   return {out, lse};
@@ -389,6 +464,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_kvcache", &flash_attention_v2_kvcache,
         "attention against a (paged) KV cache with an optional in-place append: (q, k_cache, v_cache, cache_seqlens, "
         "block_table, k_new, v_new, is_causal, scale, num_splits)");
+  m.def("flash_attention_v2_kvcache_rotary", &flash_attention_v2_kvcache_rotary,
+        "the KV-cache forward with q and k_new rotated (RoPE) at their cache positions: (q, k_cache, v_cache, "
+        "cache_seqlens, block_table, k_new, v_new, rotary_cos, rotary_sin, rotary_interleaved, is_causal, scale, "
+        "num_splits)");
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

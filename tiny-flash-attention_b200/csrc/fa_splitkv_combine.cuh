@@ -1,5 +1,6 @@
 // fa_splitkv_combine.cuh -- the small HBM-bound kernels either side of the attention forward when the problem
-// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below):
+// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below)
+// and its rotary variant (kvcache_rotary_append_kernel, launched from tfa_rotary.cu):
 //
 //   * splitkv_combine_kernel: merges the per-split partial results of the split-KV forward,
 //       O = sum_s exp(lse_s - LSE) * O_s ,  LSE = log sum_s exp(lse_s)
@@ -146,6 +147,145 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendParams 
   const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
   *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;
   *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + dst + sub * 8) = vx;
+}
+
+// ---- rotary position embedding (RoPE) for the KV-cache forward: flash-attn's rotary_cos / rotary_sin ----
+// The table position of query or appended key i of a sequence with clamped cached length cache_len: appended keys sit
+// at cache_len + i; query rows too when causal, every query row at cache_len otherwise.  Clamped to seqlen_ro - 1 so
+// that no cos/sin read leaves the table; only a query row can get there (Sq > Snew near the capacity), since a key
+// position is below capacity <= seqlen_ro.
+__host__ __device__ __forceinline__ int rotary_pos(int cache_len, int i, bool causal, bool is_query, int seqlen_ro) {
+  const int pos = (is_query && !causal) ? cache_len : cache_len + i;
+  return min(pos, seqlen_ro - 1);
+}
+
+// fp32 arithmetic with one IEEE rounding each, written as PTX so that nvcc can neither contract a product and a sum
+// into an FMA nor flush denormals (the build uses --use_fast_math): the rotation is then bit-identical to the same
+// formula evaluated by eager torch in fp32.
+__device__ __forceinline__ float mul_rn(float a, float b) {
+  float d;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float add_rn(float a, float b) {
+  float d;
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+__device__ __forceinline__ float sub_rn(float a, float b) {
+  float d;
+  asm("sub.rn.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+// element t (0..7) of a 16-byte chunk of 16-bit values, widened exactly to fp32
+template <bool IS_BF16>
+__device__ __forceinline__ float widen16(const uint4& v, int t) {
+  const uint32_t w = (&v.x)[t >> 1];
+  const uint32_t bits = (t & 1) ? (w >> 16) : (w & 0xffffu);
+  if constexpr (IS_BF16) return __uint_as_float(bits << 16);
+  float f;
+  asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(static_cast<unsigned short>(bits)));
+  return f;
+}
+
+// Chunk `sub` (elements [8 sub, 8 sub + 8)) of `row` rotated by the cos/sin table row `cs_row` (rotary_dim / 2
+// entries each).  Each pair (x0, x1) becomes x0' = x0 c - x1 s, x1' = x0 s + x1 c in fp32, rounded once to 16 bits.
+// Pairs are (j, j + rotary_dim/2) with angle j (GPT-NeoX), or (2j, 2j+1) with angle j when INTERLEAVED (GPT-J).
+// Elements [rotary_dim, D) pass through.  rotary_dim is a multiple of 16, so a chunk is all rotated or all passed, and
+// the NeoX partner of a chunk is another whole chunk.
+template <bool IS_BF16, bool INTERLEAVED>
+__device__ __forceinline__ uint4 rotate_chunk(const uint16_t* row, int sub, const uint16_t* cos_row,
+                                              const uint16_t* sin_row, int rotary_dim) {
+  const uint4 x = __ldg(reinterpret_cast<const uint4*>(row) + sub);
+  const int e0 = sub * 8;
+  if (e0 >= rotary_dim) return x;
+  float r[8];
+  if constexpr (INTERLEAVED) {
+    const uint2 c2 = __ldg(reinterpret_cast<const uint2*>(cos_row + e0 / 2));
+    const uint2 s2 = __ldg(reinterpret_cast<const uint2*>(sin_row + e0 / 2));
+    const uint4 c = make_uint4(c2.x, c2.y, 0u, 0u), s = make_uint4(s2.x, s2.y, 0u, 0u);
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float x0 = widen16<IS_BF16>(x, 2 * t), x1 = widen16<IS_BF16>(x, 2 * t + 1);
+      const float ct = widen16<IS_BF16>(c, t), st = widen16<IS_BF16>(s, t);
+      r[2 * t] = sub_rn(mul_rn(x0, ct), mul_rn(x1, st));
+      r[2 * t + 1] = add_rn(mul_rn(x0, st), mul_rn(x1, ct));
+    }
+  } else {
+    const int half = rotary_dim / 2;
+    const bool first = e0 < half;
+    const int j0 = first ? e0 : e0 - half;                       // angle of element 0 of this chunk
+    const uint4 y = __ldg(reinterpret_cast<const uint4*>(row + (first ? e0 + half : e0 - half)));   // the partners
+    const uint4 c = __ldg(reinterpret_cast<const uint4*>(cos_row + j0));
+    const uint4 s = __ldg(reinterpret_cast<const uint4*>(sin_row + j0));
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const float xt = widen16<IS_BF16>(x, t), yt = widen16<IS_BF16>(y, t);
+      const float ct = widen16<IS_BF16>(c, t), st = widen16<IS_BF16>(s, t);
+      r[t] = first ? sub_rn(mul_rn(xt, ct), mul_rn(yt, st))      // x0' = x0 c - x1 s  (x0 = x, x1 = y)
+                   : add_rn(mul_rn(yt, st), mul_rn(xt, ct));     // x1' = x0 s + x1 c  (x0 = y, x1 = x)
+    }
+  }
+  return make_uint4(pack_16x2<IS_BF16>(r[0], r[1]), pack_16x2<IS_BF16>(r[2], r[3]), pack_16x2<IS_BF16>(r[4], r[5]),
+                    pack_16x2<IS_BF16>(r[6], r[7]));
+}
+
+// kvcache_rotary_append_kernel: the append of kvcache_append_kernel with RoPE, plus the rotated queries, in one launch.
+// Chunks [0, q_chunks) write rot(q) into the contiguous (B, Sq, Hq, D) buffer q_rot, which the forward then reads in
+// place of q; the remaining chunks write rot(k_new) and v_new (unrotated) into the cache at keys [L_b, L_b + snew),
+// dropping a token whose block-table entry lies outside [0, num_blocks) as the plain append does.  Positions:
+// rotary_pos().  One thread per 16-byte output chunk (a NeoX chunk also reads its partner chunk and 16 bytes each of
+// cos and sin).  Algorithmic bytes: 2 * B*Sq*Hq*D * 2 (q in, q_rot out) + 2 * 2 * B*snew*Hkv*D * 2 (k/v in and out),
+// plus the cos/sin rows.
+struct RotaryAppendParams {
+  AppendParams ap;                // the append; ap.chunks = B * snew * Hkv * D / 8
+  const void* q;
+  void* q_rot;                    // (B, Sq, Hq, D) contiguous
+  long long q_sb, q_ss, q_sh;     // element strides of q
+  const void* cos;                // (seqlen_ro, rotary_dim / 2) contiguous, q's dtype
+  const void* sin;
+  int Sq, Hq, rotary_dim, seqlen_ro, causal;
+  long long q_chunks;             // B * Sq * Hq * D / 8
+};
+
+template <int D, bool IS_BF16, bool INTERLEAVED>
+__global__ void __launch_bounds__(256) kvcache_rotary_append_kernel(const RotaryAppendParams p) {
+  constexpr int CPR = D / 8;                   // 16-byte chunks per row
+  long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  const bool is_q = c < p.q_chunks;
+  if (!is_q) {
+    c -= p.q_chunks;
+    if (c >= p.ap.chunks) return;
+  }
+  const int sub = static_cast<int>(c % CPR);
+  long long r = c / CPR;                       // row index over (B, S, H), H fastest
+  const int H = is_q ? p.Hq : p.ap.Hkv;
+  const int S = is_q ? p.Sq : p.ap.snew;
+  const int h = static_cast<int>(r % H);
+  r /= H;
+  const int i = static_cast<int>(r % S);
+  const int b = static_cast<int>(r / S);
+  const int len = cache_len(__ldg(p.ap.cache_seqlens + b), p.ap.capacity, p.ap.snew);
+  const long long ro = static_cast<long long>(rotary_pos(len, i, p.causal != 0, is_q, p.seqlen_ro)) * (p.rotary_dim / 2);
+  const uint16_t* cos_row = static_cast<const uint16_t*>(p.cos) + ro;
+  const uint16_t* sin_row = static_cast<const uint16_t*>(p.sin) + ro;
+  if (is_q) {
+    const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + i * p.q_ss + h * p.q_sh;
+    const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_row, sin_row, p.rotary_dim);
+    reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + ((static_cast<long long>(b) * p.Sq + i) * p.Hq + h) * D)
+        [sub] = y;
+    return;
+  }
+  const AppendParams& a = p.ap;
+  const long long dst = append_offset(a.cache_seqlens, a.block_table, a.bt_stride, b, i, h, a.page, a.capacity, a.snew,
+                                      a.num_blocks, a.c_sb, a.c_ss, a.c_sh);
+  if (dst < 0) return;
+  const long long src = b * a.n_sb + i * a.n_ss + h * a.n_sh;
+  const uint4 kx = rotate_chunk<IS_BF16, INTERLEAVED>(static_cast<const uint16_t*>(a.k_new) + src, sub, cos_row,
+                                                      sin_row, p.rotary_dim);
+  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + src) + sub);
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.k_cache) + dst + sub * 8) = kx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.v_cache) + dst + sub * 8) = vx;
 }
 
 }  // namespace tfa

@@ -19,6 +19,10 @@
 #include <cstdlib>
 #include <cstring>
 
+// tfa_rotary.cu: the rotary append's launch, compiled apart from the forward kernels
+int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
+                                      cudaStream_t stream);
+
 namespace {
 
 using tfa::DebugRecord;
@@ -535,11 +539,26 @@ int validate_kvcache(const tfa_attn_kvcache_args& ka) {
   return 0;
 }
 
-int kvcache_impl(const tfa_attn_kvcache_args& ka) {
-  const Problem a = from_kvcache_args(ka);
+// The rotary arguments of a cache call whose cache arguments passed (capacity = a.Sk).
+int validate_rotary(const tfa_attn_kvcache_args& ka, const Problem& a, const tfa_rotary_args& ra) {
+  if (!ra.cos || !ra.sin || !ra.q_rot ||
+      ((reinterpret_cast<uintptr_t>(ra.cos) | reinterpret_cast<uintptr_t>(ra.sin) |
+        reinterpret_cast<uintptr_t>(ra.q_rot)) & 15u))
+    return TFA_EINVAL_ROTARY;
+  if (ra.rotary_dim < 16 || ra.rotary_dim > a.D || ra.rotary_dim % 16) return TFA_EINVAL_ROTARY;
+  if (ra.seqlen_ro < a.Sk) return TFA_EINVAL_ROTARY;      // every key position is below the capacity
+  if (!ka.k_new) return TFA_EINVAL_ROTARY;                // as flash-attn: rotary rotates the appended keys
+  return 0;
+}
+
+// `ra` nullptr: the plain cache forward.  Otherwise q and k_new are rotated first (kvcache_rotary_append_kernel, in
+// place of the plain append) and the forward reads its queries from ra->q_rot.
+int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
+  Problem a = from_kvcache_args(ka);
   int rc = validate_kvcache(ka);        // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
+  if (ra && (rc = validate_rotary(ka, a, *ra))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
   const int capacity = a.Sk;
@@ -549,19 +568,39 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka) {
   SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
   if ((rc = plan_splits(a, plan))) return rc;
 
+  tfa::AppendParams ap;
+  ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
+  ap.n_sb = ka.new_stride_b; ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
+  ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
+  ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
+  ap.page = page; ap.capacity = capacity; ap.snew = snew; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
+  ap.chunks = static_cast<long long>(a.B) * snew * a.Hkv * (a.D / 8);
+
+  tfa::RotaryAppendParams rp;
+  if (ra) {
+    rp.ap = ap;
+    rp.q = a.q; rp.q_rot = ra->q_rot;
+    rp.q_sb = a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
+    rp.cos = ra->cos; rp.sin = ra->sin;
+    rp.Sq = a.Sq; rp.Hq = a.Hq; rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
+    rp.causal = a.causal != 0 ? 1 : 0;
+    rp.q_chunks = static_cast<long long>(a.B) * a.Sq * a.Hq * (a.D / 8);
+    // the forward reads rot(q), contiguous (B, Sq, Hq, D); out keeps the caller's q strides (osb / osh / oss)
+    a.q = ra->q_rot;
+    a.qss = static_cast<long long>(a.Hq) * a.D;
+    a.qsh = a.D;
+    a.qsb = a.qss * a.Sq;
+  }
+
   CUtensorMap tq, tk, tv;
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
   if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
   if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
 
-  if (snew > 0) {
-    tfa::AppendParams ap;
-    ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
-    ap.n_sb = ka.new_stride_b; ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
-    ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
-    ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
-    ap.page = page; ap.capacity = capacity; ap.snew = snew; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
-    ap.chunks = static_cast<long long>(a.B) * snew * a.Hkv * (a.D / 8);
+  if (ra) {
+    rc = tfa_internal_launch_rotary_append(rp, a.D, a.dtype == TFA_BF16, ra->interleaved != 0, a.stream);
+    if (rc) return rc;
+  } else if (snew > 0) {
     rc = launch_small(a.D == 64 ? tfa::kvcache_append_kernel<64> : tfa::kvcache_append_kernel<128>, ap.chunks, 256, ap,
                       a.stream);
     if (rc) return rc;
@@ -621,7 +660,12 @@ int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
 
 int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args);
+  return kvcache_impl(*args, nullptr);
+}
+
+int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary) {
+  if (!args || !rotary) return TFA_EINVAL_PTR;
+  return kvcache_impl(*args, rotary);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -768,6 +812,10 @@ long long tfa_internal_append_offset(const int* cache_seqlens, const int* block_
   return tfa::append_offset(cache_seqlens, block_table, bt_stride, b, i, h, page, capacity, snew, num_blocks, cs_b,
                             cs_s, cs_h);
 }
+// development aid (not in the public header): the rotary position rule of fa_splitkv_combine.cuh on the host
+int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {
+  return tfa::rotary_pos(cache_len, i, causal != 0, is_query != 0, seqlen_ro);
+}
 
 int tfa_debug_record(unsigned int out[8]) {
   if (!out) return TFA_EINVAL_PTR;
@@ -798,6 +846,9 @@ const char* tfa_error_string(int code) {
     case TFA_EINVAL_KVCACHE:
       return "tfa: kv cache needs non-null 4-byte aligned cache_seqlens (block_table: aligned, page_block_size a "
              "multiple of 128), num_blocks and max_blocks_per_seq >= 1, and k_new with v_new, Snew in [1, capacity]";
+    case TFA_EINVAL_ROTARY:
+      return "tfa: rotary needs non-null 16-byte aligned cos, sin and q_rot, rotary_dim a multiple of 16 in [16, D], "
+             "seqlen_ro >= capacity, and k_new";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "tfa: unknown error";
   }
 }

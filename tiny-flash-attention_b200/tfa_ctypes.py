@@ -83,6 +83,14 @@ class KvcacheArgs(ctypes.Structure):
     ]
 
 
+class RotaryArgs(ctypes.Structure):
+    """struct tfa_rotary_args (include/tfa_b200.h)."""
+    _fields_ = [
+        ("cos", ctypes.c_void_p), ("sin", ctypes.c_void_p), ("seqlen_ro", ctypes.c_int32),
+        ("rotary_dim", ctypes.c_int32), ("interleaved", ctypes.c_int32), ("q_rot", ctypes.c_void_p),
+    ]
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -108,6 +116,8 @@ def lib():
         L.tfa_attn_varlen_fwd.restype = ci
         L.tfa_attn_kvcache_fwd.argtypes = [ctypes.POINTER(KvcacheArgs)]
         L.tfa_attn_kvcache_fwd.restype = ci
+        L.tfa_attn_kvcache_rotary_fwd.argtypes = [ctypes.POINTER(KvcacheArgs), ctypes.POINTER(RotaryArgs)]
+        L.tfa_attn_kvcache_rotary_fwd.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -232,11 +242,15 @@ def attn_varlen_fwd(q, k, v, cu_q, cu_k, max_seqlen_q, is_causal, scale, out_fp3
 
 
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
-                     scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False):
+                     scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
+                     rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None):
     """Attention against a KV cache through tfa_attn_kvcache_fwd(): q (B, Sq, Hq, D) with unit head_dim stride;
     k_cache / v_cache (num_blocks, page, Hkv, D) with a block_table (B, max_blocks_per_seq) int32, or (B, capacity,
     Hkv, D) with block_table None; cache_seqlens (B,) int32; optional k_new / v_new (B, Snew, Hkv, D) appended in
     place.  num_splits: 1 none, n > 1 as asked, 0 library heuristic (a workspace is allocated here when it splits).
+    rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and k_new first, through
+    tfa_attn_kvcache_rotary_fwd().  The rotated queries go to `q_rot`, a contiguous (B, Sq, Hq, D) tensor of q's dtype
+    that holds them after the call, or to a buffer allocated here.
     Returns out (q's shape and strides) and lse (B, Hq, Sq)."""
     import torch
     assert q.is_cuda and q.dim() == 4 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -269,7 +283,18 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
     n = _split_workspace(dense, a, q.device, st)
-    check(lib().tfa_attn_kvcache_fwd(ctypes.byref(a)))
+    if rotary_cos is None:
+        check(lib().tfa_attn_kvcache_fwd(ctypes.byref(a)))
+    else:
+        assert rotary_sin is not None and rotary_cos.dim() == 2 and rotary_cos.shape == rotary_sin.shape
+        assert rotary_cos.is_contiguous() and rotary_sin.is_contiguous()
+        if q_rot is None:
+            q_rot = torch.empty((B, Sq, Hq, D), dtype=q.dtype, device=q.device)
+            _WORKSPACES[("q_rot", q.device.index, int(st))] = q_rot      # kept alive as the split workspace is
+        assert q_rot.shape == q.shape and q_rot.dtype == q.dtype and q_rot.is_contiguous()
+        r = RotaryArgs(rotary_cos.data_ptr(), rotary_sin.data_ptr(), rotary_cos.shape[0], 2 * rotary_cos.shape[1],
+                       int(bool(rotary_interleaved)), q_rot.data_ptr())
+        check(lib().tfa_attn_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r)))
     if return_splits:
         return out, lse, n
     return out, lse
