@@ -70,6 +70,20 @@ __host__ __device__ __forceinline__ long long append_offset(const int* cache_seq
   return blk * cs_b + row * cs_s + h * cs_h;
 }
 
+// Where a call's results go: row `row` of (batch b, head h) has its O at element b*sb + h*sh + row*ss of out and its
+// LSE at element b*lse_sb + h*lse_sh + row of lse.  The host builds it once per call (tfa_api.cu); the combine and the
+// empty-rows fill address out / lse through it, and set_output derives the forward's strides below from it.
+struct OutLayout {
+  long long sb, sh, ss;
+  long long lse_sb, lse_sh;
+  __host__ __device__ __forceinline__ long long o(long long b, long long h, long long row) const {
+    return b * sb + h * sh + row * ss;
+  }
+  __host__ __device__ __forceinline__ long long lse(long long b, long long h, long long row) const {
+    return b * lse_sb + h * lse_sh + row;
+  }
+};
+
 struct FwdParams {
   void* out;          // 16-bit output, element strides below
   // Fused exchange (multi-GPU): when n_extra_dst > 0 every 16-byte chunk of O is ALSO stored to these buffers

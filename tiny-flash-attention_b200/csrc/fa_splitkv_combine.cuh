@@ -23,10 +23,9 @@ namespace tfa {
 struct CombineParams {
   const float* o_part;        // [nsplit][B*H*S][D] fp32, normalised partial outputs
   const float* lse_part;      // [nsplit][B*H*S]
-  void* out;                  // 16-bit (or fp32 when OUT_F32) output, strided
-  float* lse;                 // (B*H, lse_stride_bh) or nullptr
-  long long o_stride_b, o_stride_h, o_stride_s;   // elements
-  long long lse_stride_bh;
+  void* out;                  // 16-bit (or fp32 when OUT_F32) output at `ol`
+  float* lse;                 // or nullptr
+  OutLayout ol;
   long long rows;             // B*H*S
   int H, S;
   int nsplit, split_tiles;    // as launched
@@ -71,7 +70,7 @@ __global__ void __launch_bounds__(256) splitkv_combine_kernel(const CombineParam
   const float inv = wsum > 0.f ? 1.0f / wsum : 0.f;
   acc.x *= inv; acc.y *= inv; acc.z *= inv; acc.w *= inv;
   const long long b = bh / p.H, h = bh % p.H;
-  const long long off = b * p.o_stride_b + h * p.o_stride_h + static_cast<long long>(i) * p.o_stride_s + sub * 4;
+  const long long off = p.ol.o(b, h, i) + sub * 4;
   if constexpr (OUT_F32) {
     *reinterpret_cast<float4*>(static_cast<float*>(p.out) + off) = acc;
   } else {
@@ -81,14 +80,13 @@ __global__ void __launch_bounds__(256) splitkv_combine_kernel(const CombineParam
     *reinterpret_cast<uint2*>(static_cast<uint16_t*>(p.out) + off) = v;
   }
   if (p.lse != nullptr && sub == 0)
-    p.lse[bh * p.lse_stride_bh + i] = wsum > 0.f ? m + logf(wsum) : INFINITY;
+    p.lse[p.ol.lse(b, h, i)] = wsum > 0.f ? m + logf(wsum) : INFINITY;
 }
 
 struct FillParams {
   void* out;
   float* lse;
-  long long o_stride_b, o_stride_h, o_stride_s;
-  long long lse_stride_bh;
+  OutLayout ol;
   long long rows;             // B*H*n_empty
   int H, n_empty;
 };
@@ -103,10 +101,10 @@ __global__ void __launch_bounds__(256) empty_rows_fill_kernel(const FillParams p
   const int i = static_cast<int>(row % p.n_empty);
   const long long bh = row / p.n_empty;
   const long long b = bh / p.H, h = bh % p.H;
-  const long long off = b * p.o_stride_b + h * p.o_stride_h + static_cast<long long>(i) * p.o_stride_s + sub * 4;
+  const long long off = p.ol.o(b, h, i) + sub * 4;
   if constexpr (OUT_F32) *reinterpret_cast<float4*>(static_cast<float*>(p.out) + off) = make_float4(0.f, 0.f, 0.f, 0.f);
   else *reinterpret_cast<uint2*>(static_cast<uint16_t*>(p.out) + off) = make_uint2(0u, 0u);
-  if (p.lse != nullptr && sub == 0) p.lse[bh * p.lse_stride_bh + i] = INFINITY;
+  if (p.lse != nullptr && sub == 0) p.lse[p.ol.lse(b, h, i)] = INFINITY;
 }
 
 // kvcache_append_kernel: writes k_new / v_new (B, snew, Hkv, D) into the (paged) KV cache at keys

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 #include <cudaTypedefs.h>
 #include <atomic>
+#include <cassert>
 #include <mutex>
 #include <vector>
 #include <cstdlib>
@@ -220,7 +221,7 @@ struct Problem {
   float* lse;
   int B, Hq, Hkv, Sq, Sk, D;
   long long qsb, qsh, qss, ksb, ksh, kss;   // element strides of q and of k/v
-  long long osb, osh, oss, lse_stride_bh;   // where results go: element strides of out, lse elements per (b, h)
+  tfa::OutLayout ol;                        // where results go
   int dtype, causal;
   float scale;
   int out_fp32;
@@ -301,7 +302,7 @@ int plan_splits(const Problem& a, SplitPlan& plan) {
 
 // Where the forward over S query rows per (batch, head) writes: the caller's out / lse in one pass; with split-KV,
 // contiguous (B, Hq, S, D) fp32 partials per split with their LSEs, which the combine merges into out / lse.
-void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
+void set_output(FwdParams& p, const Problem& a, int S, int nsplit, bool varlen) {
   if (nsplit > 1) {
     const long long rows = static_cast<long long>(a.B) * a.Hq * S;
     float* ws_o = static_cast<float*>(a.ws);
@@ -319,11 +320,14 @@ void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
     p.out = f32 ? nullptr : a.out;
     p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
     p.lse = a.lse;
-    p.o_stride_b = a.osb;
-    p.o_stride_h = a.osh;
-    p.o_stride_s = a.oss;
+    p.o_stride_b = a.ol.sb;
+    p.o_stride_h = a.ol.sh;
+    p.o_stride_s = a.ol.ss;
     p.part_stride = 0;
-    p.lse_stride_bh = a.lse_stride_bh;
+    // The forward steps through lse in (batch*head) rows of lse_sh, or, for varlen, in head rows plus the sequence's
+    // first packed row; the combine and the fill read a.ol itself.  Both agree only for these layouts.
+    assert(a.ol.lse_sb == (varlen ? 0 : static_cast<long long>(a.Hq) * a.ol.lse_sh));
+    p.lse_stride_bh = a.ol.lse_sh;
     p.lse_part_stride = 0;
   }
 }
@@ -364,7 +368,7 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   p.S = S;
   p.nsplit = plan.nsplit;
   p.split_tiles = plan.split_tiles;
-  set_output(p, a, S, plan.nsplit);
+  set_output(p, a, S, plan.nsplit, MODE == tfa::kVarlen);
 
   const int variant = choose_kernel(causal, npairs, p.n_extra_dst);
   int rc = launch_fwd<MODE>(a.D, causal, bf16, f32 || plan.nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * plan.nsplit,
@@ -376,8 +380,7 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   cp.lse_part = p.lse;
   cp.out = a.out;
   cp.lse = a.lse;
-  cp.o_stride_b = a.osb; cp.o_stride_h = a.osh; cp.o_stride_s = a.oss;
-  cp.lse_stride_bh = a.lse_stride_bh;
+  cp.ol = a.ol;
   cp.rows = static_cast<long long>(a.B) * a.Hq * S;
   cp.H = a.Hq; cp.S = S;
   cp.nsplit = plan.nsplit; cp.split_tiles = plan.split_tiles;
@@ -409,15 +412,13 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   if (causal && a.Sk < a.Sq) {
     const int n_empty = a.Sq - a.Sk;
     tfa::FillParams fp;
-    fp.out = a.out; fp.lse = a.lse;
-    fp.o_stride_b = a.osb; fp.o_stride_h = a.osh; fp.o_stride_s = a.oss;
-    fp.lse_stride_bh = a.lse_stride_bh;
+    fp.out = a.out; fp.lse = a.lse; fp.ol = a.ol;
     fp.rows = static_cast<long long>(a.B) * a.Hq * n_empty;
     fp.H = a.Hq; fp.n_empty = n_empty;
     rc = (a.D == 64) ? launch_fill<64>(fp, f32, a.stream) : launch_fill<128>(fp, f32, a.stream);
     if (rc) return rc;
     a.q = static_cast<const char*>(a.q) + static_cast<size_t>(n_empty) * a.qss * 2;
-    a.out = static_cast<char*>(a.out) + static_cast<size_t>(n_empty) * a.oss * (f32 ? 4 : 2);
+    a.out = static_cast<char*>(a.out) + static_cast<size_t>(n_empty) * a.ol.ss * (f32 ? 4 : 2);
     if (a.lse) a.lse += n_empty;
     a.Sq = a.Sk;
   }
@@ -439,8 +440,8 @@ Problem from_fwd_args(const tfa_fwd_args& a) {
   Problem q;
   q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
   q.B = a.B; q.Hq = a.H; q.Hkv = a.H; q.Sq = a.S; q.Sk = a.S; q.D = a.D;
-  q.qsb = q.ksb = q.osb = a.stride_b; q.qsh = q.ksh = q.osh = a.stride_h; q.qss = q.kss = q.oss = a.stride_s;
-  q.lse_stride_bh = a.S;
+  q.qsb = q.ksb = a.stride_b; q.qsh = q.ksh = a.stride_h; q.qss = q.kss = a.stride_s;
+  q.ol = {a.stride_b, a.stride_h, a.stride_s, static_cast<long long>(a.H) * a.S, a.S};   // lse is (B, H, S)
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -451,9 +452,9 @@ Problem from_attn_args(const tfa_attn_args& a) {
   Problem q;
   q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.Sq; q.Sk = a.Sk; q.D = a.D;
-  q.qsb = q.osb = a.q_stride_b; q.qsh = q.osh = a.q_stride_h; q.qss = q.oss = a.q_stride_s;
+  q.qsb = a.q_stride_b; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
   q.ksb = a.kv_stride_b; q.ksh = a.kv_stride_h; q.kss = a.kv_stride_s;
-  q.lse_stride_bh = a.Sq;
+  q.ol = {q.qsb, q.qsh, q.qss, static_cast<long long>(a.Hq) * a.Sq, a.Sq};   // out as q, lse (B, Hq, Sq)
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -467,8 +468,7 @@ Problem from_varlen_args(const tfa_attn_varlen_args& a) {
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.Sk = a.total_k; q.D = a.D;
   q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
   q.ksb = 0; q.ksh = a.kv_stride_h; q.kss = a.kv_stride_s;
-  q.osb = 0; q.osh = a.D; q.oss = static_cast<long long>(a.Hq) * a.D;   // out is (total_q, Hq, D) contiguous
-  q.lse_stride_bh = a.total_q;                                          // lse is (Hq, total_q)
+  q.ol = {0, a.D, static_cast<long long>(a.Hq) * a.D, 0, a.total_q};   // out (total_q, Hq, D), lse (Hq, total_q)
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -508,9 +508,9 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.Sq; q.D = a.D;
   const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
   q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
-  q.qsb = q.osb = a.q_stride_b; q.qsh = q.osh = a.q_stride_h; q.qss = q.oss = a.q_stride_s;
+  q.qsb = a.q_stride_b; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
   q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
-  q.lse_stride_bh = a.Sq;
+  q.ol = {q.qsb, q.qsh, q.qss, static_cast<long long>(a.Hq) * a.Sq, a.Sq};   // out as q, lse (B, Hq, Sq)
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
@@ -585,7 +585,7 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
     rp.Sq = a.Sq; rp.Hq = a.Hq; rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
     rp.causal = a.causal != 0 ? 1 : 0;
     rp.q_chunks = static_cast<long long>(a.B) * a.Sq * a.Hq * (a.D / 8);
-    // the forward reads rot(q), contiguous (B, Sq, Hq, D); out keeps the caller's q strides (osb / osh / oss)
+    // the forward reads rot(q), contiguous (B, Sq, Hq, D); out keeps the caller's q strides (ol)
     a.q = ra->q_rot;
     a.qss = static_cast<long long>(a.Hq) * a.D;
     a.qsh = a.D;
