@@ -270,6 +270,64 @@ typedef struct tfa_rotary_args {
 
 int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary);
 
+/* ---- a variable-length batch of queries against a (paged) KV cache: the mixed prefill / decode step of a
+ * continuous-batching loop (flash-attn's flash_attn_varlen_func with block_table and seqused_k) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_varlen_kvcache_fwd.  Queries as tfa_attn_varlen_fwd(), keys and values as tfa_attn_kvcache_fwd().
+ *
+ *   q        : (total_q, Hq, D) through q_stride_s / q_stride_h (elements, unit head_dim stride)
+ *   out      : (total_q, Hq, D) contiguous, dtype of q, or fp32 when out_fp32 != 0
+ *   lse      : (Hq, total_q) contiguous fp32, natural log; may be NULL
+ *   cu_seqlens_q : int32 DEVICE array of B + 1 offsets: sequence b is rows [cu[b], cu[b+1]) of q / out.  Its query
+ *              count Sq_b is taken with the offsets clamped to [0, total_q]; n_b = min(Sq_b, max_seqlen_q).
+ *   max_seqlen_q : in [1, total_q], >= every Sq_b.  Rows of a sequence beyond its first max_seqlen_q are neither
+ *              computed nor appended and keep what out / lse held; the sequence is then its first n_b rows.
+ *   k_cache, v_cache, block_table, num_blocks, page_block_size, max_blocks_per_seq, cache_stride_*,
+ *   block_table_stride, cache_seqlens : as tfa_attn_kvcache_args (page_block_size % 128 == 0 with a table; NULL
+ *              table: a contiguous (B, capacity, Hkv, D) cache).  capacity = max_blocks_per_seq * page_block_size.
+ *   k_new, v_new : optional (both or neither), packed (total_q, Hkv, D) through new_stride_s / new_stride_h, sharing
+ *              cu_seqlens_q with q: row cu[b] + i is key L_b + i of sequence b.  Written into the cache in place
+ *              before the attention; cache_seqlens is not incremented.
+ *   lengths  : with k_new, L_b = clamp(cache_seqlens[b], 0, max(capacity - n_b, 0)) and K_b = min(L_b + n_b,
+ *              capacity); an appended token past the capacity or whose block-table entry lies outside
+ *              [0, num_blocks) is dropped.  Without k_new (the caller wrote the step's keys: seqused_k),
+ *              K_b = clamp(cache_seqlens[b], 0, capacity).
+ *   attention: sequence b's n_b rows attend to its first K_b keys.  Query head h reads K/V head h / (Hq/Hkv); causal
+ *              is bottom-right aligned, row i sees keys j <= i + K_b - n_b; rows that see no key get out = 0 and
+ *              lse = +inf; a sequence with Sq_b == 0 writes nothing.  Cache slots past K_b may hold anything (NaN
+ *              included) and do not change the result.
+ * The host never reads cu_seqlens_q, cache_seqlens or block_table: the call (append included) can be captured in a
+ * CUDA graph and replayed with new contents of the same total_q.  The kernels clamp every length and offset, so
+ * malformed contents cannot make a store leave out, lse or a sequence's appended cache slots.  No split-KV (a
+ * decode-only batch keeps tfa_attn_kvcache_fwd(), which has it).  Every argument is checked before any device work.
+ * Launches: 1, + 1 with k_new. */
+typedef struct tfa_attn_varlen_kvcache_args {
+  const void* q;
+  void* k_cache;
+  void* v_cache;
+  const void* k_new;        /* may be NULL (then v_new must be NULL too) */
+  const void* v_new;
+  void* out;
+  float* lse;
+  const int32_t* cu_seqlens_q;
+  const int32_t* cache_seqlens;
+  const int32_t* block_table;  /* may be NULL: contiguous cache */
+  int32_t B, Hq, Hkv, D;
+  int32_t total_q, max_seqlen_q;
+  int32_t num_blocks, page_block_size, max_blocks_per_seq;
+  int64_t q_stride_s, q_stride_h;
+  int64_t cache_stride_block, cache_stride_s, cache_stride_h;
+  int64_t block_table_stride;
+  int64_t new_stride_s, new_stride_h;
+  int32_t dtype;
+  int32_t is_causal;
+  float softmax_scale;
+  int32_t out_fp32;
+  void* stream;
+} tfa_attn_varlen_kvcache_args;
+
+int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args);
+
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on
  * `n_streams` internal streams so H2D, compute and D2H overlap, copies out, and

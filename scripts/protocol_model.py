@@ -264,6 +264,26 @@ def random_cache_items(rng):
     return items, empty, vtail
 
 
+def random_varlen_cache_items(rng):
+    """Items of a variable-length batch against a KV cache (kVarlenCache): items past a sequence's end, skipped by
+    every role (0, not empty); items inside it whose rows see no key (cached length 0 without appended keys, or causal
+    rows above the first key), written without a barrier (0, empty); items with tiles, most of which end on a page
+    with slots past the sequence's keys, whose V rows the consumers zero (vtail)."""
+    items, empty, vtail = [], [], []
+    for i in range(rng.randint(1, 12)):
+        kind = rng.random()
+        if kind < 0.25:
+            items.append(0)
+        elif kind < 0.45:
+            items.append(0)
+            empty.append(i)
+        else:
+            items.append(rng.randint(1, 6))
+            if rng.random() < 0.7:
+                vtail.append(i)
+    return items, empty, vtail
+
+
 def main():
     trials = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     for trial in range(trials):
@@ -272,6 +292,8 @@ def main():
         items, empty = random_varlen_items(rng)
         Sim(items, rng.choice([4, 8]), rng, empty).run()
         items, empty, vtail = random_cache_items(rng)
+        Sim(items, rng.choice([4, 8]), rng, empty, vtail).run()
+        items, empty, vtail = random_varlen_cache_items(rng)
         Sim(items, rng.choice([4, 8]), rng, empty, vtail).run()
     print(f"{trials} trials: no violation")
 

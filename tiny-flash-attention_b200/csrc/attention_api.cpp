@@ -450,6 +450,105 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
   return {out, lse};
 }
 
+// A packed variable-length batch of queries against a (paged) KV cache (flash-attn's flash_attn_varlen_func with
+// block_table and seqused_k): q (total_q, Hq, D) with cu_seqlens_q int32 (B + 1) offsets as flash_attention_v2_varlen;
+// k_cache / v_cache / block_table / cache_seqlens as flash_attention_v2_kvcache; k_new / v_new None or packed
+// (total_q, Hkv, D) sharing cu_seqlens_q, written into the cache in place at keys [cache_seqlens[b], + the sequence's
+// query rows) before the attention.  Returns out (total_q, Hq, D) and lse (Hq, total_q).  No split-KV.
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale) {
+  TFA_CHECK_CUDA(q);
+  TFA_CHECK_CUDA(k_cache);
+  TFA_CHECK_CUDA(v_cache);
+  TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "k_cache, v_cache must have 4 dimensions");
+  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
+  TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
+              "k_cache and v_cache must have identical shapes and strides");
+  TORCH_CHECK(q.stride(2) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
+  TORCH_CHECK(k_cache.size(3) == q.size(2), "the caches must share head_dim with q");
+  TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
+  TORCH_CHECK(cu_seqlens_q.device() == q.device(), "cu_seqlens_q must be on q's device");
+  TORCH_CHECK(cu_seqlens_q.dim() == 1 && cu_seqlens_q.is_contiguous(), "cu_seqlens_q must be a contiguous 1-D tensor");
+  TORCH_CHECK(cu_seqlens_q.numel() >= 2, fmt_msg("cu_seqlens_q must hold B + 1 >= 2 offsets, got %lld",
+                                                 static_cast<long long>(cu_seqlens_q.numel())));
+  const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2);
+  const int64_t B = cu_seqlens_q.numel() - 1;
+  const int64_t nblk = k_cache.size(0), page = k_cache.size(1), Hkv = k_cache.size(2);
+  TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
+                  cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == B,
+              "cache_seqlens must be a contiguous int32 (B,) tensor on q's device, B = cu_seqlens_q.numel() - 1");
+  int64_t mbps = 1, bts = 1;
+  if (block_table.has_value()) {
+    const torch::Tensor& bt = *block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == B &&
+                    bt.stride(1) == 1,
+                "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
+    TORCH_CHECK(page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
+                                         static_cast<long long>(page)));
+    mbps = bt.size(1);
+    bts = bt.stride(0);
+  } else {
+    TORCH_CHECK(nblk == B, "without block_table the caches must be (B, capacity, Hkv, D)");
+  }
+  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
+  if (k_new.has_value()) {
+    const torch::Tensor &kn = *k_new, &vn = *v_new;
+    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
+                    vn.scalar_type() == q.scalar_type(),
+                "k_new and v_new must be on q's device with q's dtype");
+    TORCH_CHECK(kn.dim() == 3 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == total_q &&
+                    kn.size(1) == Hkv && kn.size(2) == D && kn.stride(2) == 1,
+                "k_new and v_new must be (total_q, Hkv, D) with identical strides and a unit head_dim stride");
+  }
+  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
+  TORCH_CHECK(total_q >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
+  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(max_seqlen_q >= 1 && max_seqlen_q <= total_q,
+              fmt_msg("max_seqlen_q must be in [1, total_q = %lld], got %lld", static_cast<long long>(total_q),
+                      static_cast<long long>(max_seqlen_q)));
+  TORCH_CHECK(total_q < (1LL << 31) && B < (1LL << 31) && nblk < (1LL << 31) && page < (1LL << 31) &&
+                  mbps < (1LL << 31),
+              "tensors too large");
+
+  torch::Tensor out, lse;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    out = torch::empty({total_q, Hq, D}, q.options());
+    lse = torch::empty({Hq, total_q}, q.options().dtype(at::kFloat));
+    tfa_attn_varlen_kvcache_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.q = q.data_ptr(); a.k_cache = k_cache.data_ptr(); a.v_cache = v_cache.data_ptr();
+    a.k_new = k_new.has_value() ? k_new->data_ptr() : nullptr;
+    a.v_new = v_new.has_value() ? v_new->data_ptr() : nullptr;
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.cu_seqlens_q = cu_seqlens_q.data_ptr<int32_t>();
+    a.cache_seqlens = cache_seqlens.data_ptr<int32_t>();
+    a.block_table = block_table.has_value() ? block_table->data_ptr<int32_t>() : nullptr;
+    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
+    a.D = static_cast<int32_t>(D);
+    a.total_q = static_cast<int32_t>(total_q); a.max_seqlen_q = static_cast<int32_t>(max_seqlen_q);
+    a.num_blocks = static_cast<int32_t>(nblk); a.page_block_size = static_cast<int32_t>(page);
+    a.max_blocks_per_seq = static_cast<int32_t>(mbps);
+    a.q_stride_s = q.stride(0); a.q_stride_h = q.stride(1);
+    a.cache_stride_block = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1); a.cache_stride_h = k_cache.stride(2);
+    a.block_table_stride = bts;
+    if (k_new.has_value()) { a.new_stride_s = k_new->stride(0); a.new_stride_h = k_new->stride(1); }
+    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.out_fp32 = 0;
+    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    rc = tfa_attn_varlen_kvcache_fwd(&a);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_cutlass", &flash_attention_v2_cutlass,
         "Flash attention v2 forward, H100-native (sm_90a wgmma/TMA)");
@@ -468,6 +567,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "the KV-cache forward with q and k_new rotated (RoPE) at their cache positions: (q, k_cache, v_cache, "
         "cache_seqlens, block_table, k_new, v_new, rotary_cos, rotary_sin, rotary_interleaved, is_causal, scale, "
         "num_splits)");
+  m.def("flash_attention_v2_varlen_kvcache", &flash_attention_v2_varlen_kvcache,
+        "a packed variable-length batch of queries against a (paged) KV cache with an optional in-place append: (q, "
+        "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, is_causal, scale)");
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

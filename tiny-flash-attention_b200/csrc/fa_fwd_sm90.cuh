@@ -33,13 +33,14 @@
 // and its producer runs ahead into the next item's Q and K/V while the softmax warpgroups finish the current one.
 // MODE (the problem the grid solves): kDense = (B, H, S, D) tensors; kVarlen = a packed variable-length batch, each
 // item reads its sequence's offsets and lengths from cu_seqlens; kCache = decode against a (paged) KV cache, each item
-// reads its sequence's cached length from cache_seqlens and its K/V boxes' pages from a block table.
+// reads its sequence's cached length from cache_seqlens and its K/V boxes' pages from a block table; kVarlenCache =
+// both at once, a packed variable-length batch of queries (cu_seqlens) against a (paged) KV cache.
 #pragma once
 #include "ptx_sm90.cuh"
 
 namespace tfa {
 
-enum : int { kDense = 0, kVarlen = 1, kCache = 2 };
+enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3 };
 
 // ---- KV-cache address math, host-callable so that a CPU test can check it exhaustively (tests/test_kvcache.py) ----
 // Keys attended by sequence b: its cached length clamped to [0, capacity - snew], plus the snew appended keys.  The
@@ -64,6 +65,31 @@ __host__ __device__ __forceinline__ long long append_offset(const int* cache_seq
                                                             int capacity, int snew, int num_blocks, long long cs_b,
                                                             long long cs_s, long long cs_h) {
   const int key = cache_len(cache_seqlens[b], capacity, snew) + i;
+  int blk, row;
+  page_lookup(block_table, bt_stride, b, key, page, blk, row);
+  if (!block_ok(blk, num_blocks)) return -1;
+  return blk * cs_b + row * cs_s + h * cs_h;
+}
+
+// ---- the variable-length batch against a KV cache (kVarlenCache) ----
+// Sequence b has n = min(Sq_b, max_seqlen_q) query rows, and as many appended keys when the call appends (n = 0
+// otherwise).  Its cached length L is clamped to [0, max(capacity - n, 0)] and it attends to K = min(L + n, capacity)
+// keys: appended keys that do not fit the capacity (n > capacity) are dropped.  Unlike cache_len, n may exceed the
+// capacity, since the host does not know it.
+__host__ __device__ __forceinline__ void varlen_cache_lens(int raw, int capacity, int n, int& L, int& K) {
+  L = min(max(raw, 0), max(capacity - n, 0));
+  K = min(L + n, capacity);
+}
+// Element offset of appended token i (0 <= i < n) of sequence b at head h, as append_offset, or -1 when the token
+// does not fit the capacity or its block-table entry lies outside [0, num_blocks) (the token is then dropped).
+__host__ __device__ __forceinline__ long long varlen_append_offset(int raw, const int* block_table, long long bt_stride,
+                                                                   int b, int i, int h, int page, int capacity, int n,
+                                                                   int num_blocks, long long cs_b, long long cs_s,
+                                                                   long long cs_h) {
+  int L, K;
+  varlen_cache_lens(raw, capacity, n, L, K);
+  const int key = L + i;
+  if (key >= K) return -1;
   int blk, row;
   page_lookup(block_table, bt_stride, b, key, page, blk, row);
   if (!block_ok(blk, num_blocks)) return -1;
@@ -124,6 +150,8 @@ struct FwdParams {
   // KV cache (MODE == kCache): q / out / lse are the dense (B, H, S) problem; sequence b attends to the first
   // cache_len(cache_seqlens[b]) + snew keys of its cache, whose key r lives at page_lookup(block_table, b, r).  The
   // K/V tensor maps are (D, page, Hkv, num_blocks).  Sk / causal_off are unused.
+  // kVarlenCache: q / out / lse as varlen (cu_q, total_q; cu_k unused), K/V as kCache; sequence b attends to the
+  // varlen_cache_lens() keys of its n_b = min(Sq_b, S) rows, with n_b appended keys when snew != 0 (a flag here).
   const int* cache_seqlens;
   const int* block_table;     // nullptr: contiguous cache, page = capacity
   long long bt_stride;
@@ -189,6 +217,7 @@ struct Item {
 template <bool CAUSAL, int MODE>
 __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   constexpr bool VARLEN = MODE == kVarlen;
+  constexpr bool QPACK = MODE == kVarlen || MODE == kVarlenCache;    // packed queries: items past a sequence skipped
   Item w;
   int pr;
   decode_work(item, p.npairs, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
@@ -214,6 +243,17 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.Sq = p.S;
     w.Sk = cache_len(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew) + p.snew;
     w.coff = w.Sk - w.Sq;           // may be negative, as for varlen
+  } else if constexpr (MODE == kVarlenCache) {
+    // queries as varlen, but only the first S = max_seqlen_q rows: the grid covers no more, and the keys appended
+    // for the sequence are those rows' own
+    const int q0 = min(max(__ldg(p.cu_q + w.bidx), 0), p.total_q);
+    const int q1 = min(max(__ldg(p.cu_q + w.bidx + 1), 0), p.total_q);
+    w.q0 = q0;
+    w.k0 = 0;
+    w.Sq = min(max(q1 - q0, 0), p.S);
+    int L;
+    varlen_cache_lens(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew ? w.Sq : 0, L, w.Sk);
+    w.coff = w.Sk - w.Sq;
   } else {
     w.q0 = 0;
     w.k0 = 0;
@@ -229,8 +269,8 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   // dense: an item without tiles writes nothing (its rows belong to other splits); varlen: an item inside its sequence
   // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0); cache: every item writes its rows,
   // a split without tiles too (LSE = -inf), so the combine can read every split's partial
-  w.live = VARLEN ? w.row0 < w.Sq : (MODE == kCache || w.n > 0);
-  if (VARLEN && !w.live) w.n = 0;    // past the sequence's end: the producer must skip it as the consumers do
+  w.live = QPACK ? w.row0 < w.Sq : (MODE == kCache || w.n > 0);
+  if (QPACK && !w.live) w.n = 0;     // past the sequence's end: the producer must skip it as the consumers do
   return w;
 }
 
@@ -238,8 +278,8 @@ template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST, int MODE
 __global__ void __launch_bounds__(384, 1)
 fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
-  constexpr bool VARLEN = MODE == kVarlen;
-  constexpr bool CACHE = MODE == kCache;
+  constexpr bool QPACK = MODE == kVarlen || MODE == kVarlenCache;   // q / out / lse packed as varlen
+  constexpr bool PAGED = MODE == kCache || MODE == kVarlenCache;    // K/V from a (paged) cache
   using C = FwdCfg<D>;
   constexpr int TILE = C::TILE_BYTES;
   constexpr int NSTAGE = C::NSTAGE;
@@ -290,14 +330,14 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         mbar_arrive_expect_tx(q_full, TILE);
         // varlen: the packed tensors are one batch entry; rows of the next sequence a box takes in are never stored
         // (queries) or masked (keys)
-        const int wz = VARLEN ? 0 : w.bidx;
+        const int wz = QPACK ? 0 : w.bidx;
 #pragma unroll
         for (int sl = 0; sl < C::SLABS; ++sl)
           tma_load_4d(sQ + sl * C::SLAB_BYTES, &tmQ, q_full, sl * 64, w.q0 + w.row0, w.hidx, wz);
         for (int j = 0; j < w.n; ++j) {
           // cache: the tile's 128 keys lie in one page (page % 128 == 0, or one page per sequence)
           int ky = w.k0 + (w.jb + j) * C::BN, kw = wz;
-          if constexpr (CACHE) page_lookup(p.block_table, p.bt_stride, w.bidx, ky, p.page, kw, ky);
+          if constexpr (PAGED) page_lookup(p.block_table, p.bt_stride, w.bidx, ky, p.page, kw, ky);
 #pragma unroll
           for (int kv = 0; kv < 2; ++kv, ++ent) {
             const uint32_t slot = ent % NSTAGE;
@@ -363,7 +403,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     // warpgroups write the same zeros; the slot is released only after both have read it.  Between the kv_full wait
     // and the release, so the producer cannot refill the slot under the stores (scripts/protocol_model.py).
     auto zero_v_tail = [&](uint32_t vslot, int jt) {
-      if constexpr (CACHE) {
+      if constexpr (PAGED) {
         const int valid = Sk - (w.jb + jt) * C::BN;          // warpgroup-uniform
         if (valid < C::BN) {
           uint8_t* vt = sKV + vslot * TILE;
@@ -525,16 +565,16 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const float inv_lo = (l_lo > 0.f) ? 1.0f / l_lo : 0.f;
     const float inv_hi = (l_hi > 0.f) ? 1.0f / l_hi : 0.f;
     const long long tile_off =
-        (VARLEN ? static_cast<long long>(w.q0) * p.o_stride_s : static_cast<long long>(w.bidx) * p.o_stride_b) +
+        (QPACK ? static_cast<long long>(w.q0) * p.o_stride_s : static_cast<long long>(w.bidx) * p.o_stride_b) +
         static_cast<long long>(w.hidx) * p.o_stride_h;
     if (p.lse != nullptr && tq == 0) {
-      if constexpr (VARLEN) {
+      if constexpr (QPACK) {
         // (H, total_q); a row that saw no key (l == 0) gets +inf.  Not for split-KV partials, whose -inf tells the
         // combine that the split holds nothing.
         float* lrow = p.lse + static_cast<long long>(w.hidx) * p.lse_stride_bh + w.q0;
         if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : INFINITY;
         if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : INFINITY;
-      } else if constexpr (CACHE) {
+      } else if constexpr (MODE == kCache) {
         // (B, H, S) as dense; a row that saw no key gets +inf, or -inf in a split-KV partial (as above)
         const float none = p.nsplit > 1 ? -INFINITY : INFINITY;
         float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;

@@ -1,6 +1,7 @@
 // fa_splitkv_combine.cuh -- the small HBM-bound kernels either side of the attention forward when the problem
-// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below)
-// and its rotary variant (kvcache_rotary_append_kernel, launched from tfa_rotary.cu):
+// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below),
+// its variable-length variant (kvcache_varlen_append_kernel, launched from tfa_varlen_kvcache.cu) and its rotary
+// variant (kvcache_rotary_append_kernel, launched from tfa_rotary.cu):
 //
 //   * splitkv_combine_kernel: merges the per-split partial results of the split-KV forward,
 //       O = sum_s exp(lse_s - LSE) * O_s ,  LSE = log sum_s exp(lse_s)
@@ -141,6 +142,45 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendParams 
                                       p.snew, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
   if (dst < 0) return;
   const long long src = b * p.n_sb + i * p.n_ss + h * p.n_sh + sub * 8;
+  const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
+  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + dst + sub * 8) = vx;
+}
+
+// kvcache_varlen_append_kernel: the append of a variable-length batch (the kVarlenCache forward, launched from
+// tfa_varlen_kvcache.cu).  k_new / v_new are packed (total_q, Hkv, D) as q is: row cu_q[b] + i is key L_b + i of
+// sequence b, for i < n_b = min(Sq_b, max_seqlen_q), at varlen_append_offset().  The grid is B * max_seqlen_q * Hkv *
+// D/8 chunks, one 16-byte chunk of K and of V per thread, as the forward's grid covers max_seqlen_q rows of every
+// sequence: a chunk with i >= n_b returns, so no search over cu_seqlens is needed.  A token past the capacity or with a
+// block-table entry outside [0, num_blocks) is dropped.  Here ap.snew is max_seqlen_q and ap.n_sb is unused.
+struct VarlenAppendParams {
+  AppendParams ap;
+  const int* cu_q;
+  int total_q;
+};
+
+template <int D>
+__global__ void __launch_bounds__(256) kvcache_varlen_append_kernel(const VarlenAppendParams vp) {
+  constexpr int CPR = D / 8;                   // 16-byte chunks per row
+  const AppendParams& p = vp.ap;
+  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (c >= p.chunks) return;
+  const int sub = static_cast<int>(c % CPR);
+  long long r = c / CPR;
+  const int h = static_cast<int>(r % p.Hkv);
+  r /= p.Hkv;
+  const int i = static_cast<int>(r % p.snew);
+  const int b = static_cast<int>(r / p.snew);
+  // the forward's clamps (decode_item): whatever cu_seqlens holds, no row outside [0, total_q) is read
+  const int q0 = min(max(__ldg(vp.cu_q + b), 0), vp.total_q);
+  const int q1 = min(max(__ldg(vp.cu_q + b + 1), 0), vp.total_q);
+  const int n = min(max(q1 - q0, 0), p.snew);
+  if (i >= n) return;
+  const long long dst = varlen_append_offset(__ldg(p.cache_seqlens + b), p.block_table, p.bt_stride, b, i, h, p.page,
+                                             p.capacity, n, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
+  if (dst < 0) return;
+  const long long src = (q0 + i) * p.n_ss + h * p.n_sh + sub * 8;
   const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
   const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
   *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;

@@ -23,6 +23,11 @@
 // tfa_rotary.cu: the rotary append's launch, compiled apart from the forward kernels
 int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
                                       cudaStream_t stream);
+// tfa_varlen_kvcache.cu: the variable-length cache forward and its append, compiled apart from the other forward kernels
+int tfa_internal_launch_varlen_kvcache_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq,
+                                           const CUtensorMap& tk, const CUtensorMap& tv, const tfa::FwdParams& p,
+                                           int nblocks, bool persist, cudaStream_t stream);
+int tfa_internal_launch_varlen_append(const tfa::VarlenAppendParams& vp, int D, cudaStream_t stream);
 
 namespace {
 
@@ -156,17 +161,22 @@ int launch_small(void (*kern)(P), long long n, int per_block, const P& prm, cuda
   return count_launch();
 }
 
+// CTAs of a forward launch over `nitems` work items: one per item, or for the persistent schedule one per SM (0 when
+// the SM count is unknown).  Records the schedule for tfa_internal_last_variant.
+long long fwd_grid(long long nitems, int variant) {
+  g_last_variant.store(variant, std::memory_order_relaxed);
+  if (variant != KV_PERSIST) return nitems;
+  const int sms = num_sms();
+  if (sms <= 0) return 0;
+  return nitems > sms ? sms : nitems;                                   // one CTA per SM
+}
+
 template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, int MODE>
 int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
                 int variant, cudaStream_t stream) {
-  g_last_variant.store(variant, std::memory_order_relaxed);
   const bool persist = variant == KV_PERSIST;
-  long long nblocks = nitems;
-  if (persist) {
-    const int sms = num_sms();
-    if (sms <= 0) return TFA_EARCH;
-    if (nblocks > sms) nblocks = sms;                                   // one CTA per SM
-  }
+  const long long nblocks = fwd_grid(nitems, variant);
+  if (nblocks <= 0) return TFA_EARCH;
   auto kern = persist ? tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, MODE>
                       : tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
   const cudaError_t cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES);
@@ -189,14 +199,26 @@ int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUte
 #undef TFA_GO
 }
 
-// One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache).
+// One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache /
+// kVarlenCache).
 template <int MODE>
 int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
   if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
   p.total_items = static_cast<int>(nitems);
-  if (D == 64) return dispatch<64, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
-  return dispatch<128, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+  // kVarlenCache is instantiated only in tfa_varlen_kvcache.cu.  The dispatch must stay in the `else` branch: a
+  // statement after a returning `if constexpr` is still instantiated, and would compile this mode's 32 kernels into
+  // this translation unit as well (a second, unused copy under the same names).
+  if constexpr (MODE == tfa::kVarlenCache) {
+    const long long nblocks = fwd_grid(nitems, variant);
+    if (nblocks <= 0) return TFA_EARCH;
+    const int rc = tfa_internal_launch_varlen_kvcache_fwd(D, causal, bf16, f32, tq, tk, tv, p, static_cast<int>(nblocks),
+                                                          variant == KV_PERSIST, stream);
+    return rc ? rc : count_launch();
+  } else {
+    if (D == 64) return dispatch<64, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+    return dispatch<128, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
+  }
 }
 
 bool arch_ok() {
@@ -368,7 +390,7 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   p.S = S;
   p.nsplit = plan.nsplit;
   p.split_tiles = plan.split_tiles;
-  set_output(p, a, S, plan.nsplit, MODE == tfa::kVarlen);
+  set_output(p, a, S, plan.nsplit, MODE == tfa::kVarlen || MODE == tfa::kVarlenCache);
 
   const int variant = choose_kernel(causal, npairs, p.n_extra_dst);
   int rc = launch_fwd<MODE>(a.D, causal, bf16, f32 || plan.nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * plan.nsplit,
@@ -517,7 +539,9 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   return q;
 }
 
-int validate_kvcache(const tfa_attn_kvcache_args& ka) {
+// The cache arguments the cache calls share: the lengths, the block table or the contiguous cache, k_new with v_new.
+template <typename Args>
+int validate_cache(const Args& ka) {
   if (!ka.cache_seqlens || (reinterpret_cast<uintptr_t>(ka.cache_seqlens) & 3u) ||
       (reinterpret_cast<uintptr_t>(ka.block_table) & 3u))
     return TFA_EINVAL_KVCACHE;
@@ -528,6 +552,11 @@ int validate_kvcache(const tfa_attn_kvcache_args& ka) {
     return TFA_EINVAL_KVCACHE;           // contiguous: one page (block b) per sequence
   }
   if ((ka.k_new == nullptr) != (ka.v_new == nullptr)) return TFA_EINVAL_KVCACHE;
+  return 0;
+}
+
+int validate_kvcache(const tfa_attn_kvcache_args& ka) {
+  if (int rc = validate_cache(ka)) return rc;
   if (ka.k_new) {
     const long long cap = static_cast<long long>(ka.max_blocks_per_seq) * ka.page_block_size;
     if (ka.Snew < 1 || ka.Snew > cap) return TFA_EINVAL_KVCACHE;
@@ -617,6 +646,72 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
   return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan, false);
 }
 
+// The variable-length cache problem as the varlen one of total_q query rows (what validate() checks of q and out)
+// against the cache of Sk = capacity keys.
+Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
+  Problem q;
+  q.q = a.q; q.k = a.k_cache; q.v = a.v_cache; q.out = a.out; q.lse = a.lse;
+  q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.D = a.D;
+  const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
+  q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
+  q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
+  q.ol = {0, a.D, static_cast<long long>(a.Hq) * a.D, 0, a.total_q};   // out (total_q, Hq, D), lse (Hq, total_q)
+  q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
+  q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
+  q.stream = static_cast<cudaStream_t>(a.stream);
+  return q;
+}
+
+int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va) {
+  const Problem a = from_varlen_kvcache_args(va);
+  int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
+  if (rc) return rc;
+  if (va.k_new) {
+    if ((reinterpret_cast<uintptr_t>(va.k_new) | reinterpret_cast<uintptr_t>(va.v_new)) & 15u) return TFA_EINVAL_PTR;
+    if ((va.new_stride_s % 8) || (va.new_stride_h % 8) || va.new_stride_s < 0 || va.new_stride_h < 0)
+      return TFA_EINVAL_STRIDE;
+  }
+  if ((rc = validate(a))) return rc;
+  if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
+  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
+  if (!arch_ok()) return TFA_EARCH;
+  init_dbg();
+  const int capacity = a.Sk;
+  const int page = va.block_table ? va.page_block_size : capacity;
+
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
+  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, page, va.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, page, va.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+
+  if (va.k_new) {
+    tfa::VarlenAppendParams vp;
+    tfa::AppendParams& ap = vp.ap;
+    ap.k_new = va.k_new; ap.v_new = va.v_new; ap.k_cache = va.k_cache; ap.v_cache = va.v_cache;
+    ap.n_sb = 0; ap.n_ss = va.new_stride_s; ap.n_sh = va.new_stride_h;
+    ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
+    ap.cache_seqlens = va.cache_seqlens; ap.block_table = va.block_table; ap.bt_stride = va.block_table_stride;
+    ap.page = page; ap.capacity = capacity; ap.snew = va.max_seqlen_q; ap.num_blocks = va.num_blocks; ap.Hkv = a.Hkv;
+    ap.chunks = static_cast<long long>(a.B) * va.max_seqlen_q * a.Hkv * (a.D / 8);
+    vp.cu_q = va.cu_seqlens_q;
+    vp.total_q = a.Sq;
+    if ((rc = tfa_internal_launch_varlen_append(vp, a.D, a.stream))) return rc;
+  }
+
+  FwdParams p{};
+  p.cu_q = va.cu_seqlens_q;
+  p.total_q = a.Sq;
+  p.cache_seqlens = va.cache_seqlens;
+  p.block_table = va.block_table;
+  p.bt_stride = va.block_table_stride;
+  p.page = page;
+  p.capacity = capacity;
+  p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
+  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
+  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
+}
+
 // ---- host-buffer path workspace ----
 struct HostWs {
   void* d[4] = {nullptr, nullptr, nullptr, nullptr};   // q k v o
@@ -666,6 +761,11 @@ int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
 int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary) {
   if (!args || !rotary) return TFA_EINVAL_PTR;
   return kvcache_impl(*args, rotary);
+}
+
+int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args) {
+  if (!args) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {

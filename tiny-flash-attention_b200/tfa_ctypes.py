@@ -83,6 +83,23 @@ class KvcacheArgs(ctypes.Structure):
     ]
 
 
+class VarlenKvcacheArgs(ctypes.Structure):
+    """struct tfa_attn_varlen_kvcache_args (include/tfa_b200.h)."""
+    _fields_ = [
+        ("q", ctypes.c_void_p), ("k_cache", ctypes.c_void_p), ("v_cache", ctypes.c_void_p),
+        ("k_new", ctypes.c_void_p), ("v_new", ctypes.c_void_p), ("out", ctypes.c_void_p), ("lse", ctypes.c_void_p),
+        ("cu_seqlens_q", ctypes.c_void_p), ("cache_seqlens", ctypes.c_void_p), ("block_table", ctypes.c_void_p),
+        ("B", ctypes.c_int32), ("Hq", ctypes.c_int32), ("Hkv", ctypes.c_int32), ("D", ctypes.c_int32),
+        ("total_q", ctypes.c_int32), ("max_seqlen_q", ctypes.c_int32),
+        ("num_blocks", ctypes.c_int32), ("page_block_size", ctypes.c_int32), ("max_blocks_per_seq", ctypes.c_int32),
+        ("q_stride_s", ctypes.c_int64), ("q_stride_h", ctypes.c_int64),
+        ("cache_stride_block", ctypes.c_int64), ("cache_stride_s", ctypes.c_int64), ("cache_stride_h", ctypes.c_int64),
+        ("block_table_stride", ctypes.c_int64), ("new_stride_s", ctypes.c_int64), ("new_stride_h", ctypes.c_int64),
+        ("dtype", ctypes.c_int32), ("is_causal", ctypes.c_int32), ("softmax_scale", ctypes.c_float),
+        ("out_fp32", ctypes.c_int32), ("stream", ctypes.c_void_p),
+    ]
+
+
 class RotaryArgs(ctypes.Structure):
     """struct tfa_rotary_args (include/tfa_b200.h)."""
     _fields_ = [
@@ -118,6 +135,8 @@ def lib():
         L.tfa_attn_kvcache_fwd.restype = ci
         L.tfa_attn_kvcache_rotary_fwd.argtypes = [ctypes.POINTER(KvcacheArgs), ctypes.POINTER(RotaryArgs)]
         L.tfa_attn_kvcache_rotary_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs)]
+        L.tfa_attn_varlen_kvcache_fwd.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -297,6 +316,44 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
         check(lib().tfa_attn_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r)))
     if return_splits:
         return out, lse, n
+    return out, lse
+
+
+def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
+                            v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None):
+    """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
+    (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
+    and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
+    sharing cu_q, appended in place.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given
+    to write into caller-owned buffers."""
+    import torch
+    assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
+    assert k_cache.stride() == v_cache.stride() and q.stride(2) == 1 and k_cache.stride(3) == 1
+    assert cu_q.dtype == torch.int32 and cu_q.numel() >= 2 and cache_seqlens.dtype == torch.int32
+    total_q, Hq, D = q.shape
+    nblk, page, Hkv, _ = k_cache.shape
+    if block_table is not None:
+        assert block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
+        mbps, bts, bt_ptr = block_table.shape[1], block_table.stride(0), block_table.data_ptr()
+    else:
+        mbps, bts, bt_ptr = 1, 1, None
+    nptr, vptr, ns = None, None, (0, 0)
+    if k_new is not None:
+        assert k_new.shape == v_new.shape and k_new.stride() == v_new.stride() and k_new.stride(2) == 1
+        nptr, vptr, ns = k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:2]
+    if scale is None:
+        scale = D ** -0.5
+    if out is None:
+        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+    if lse is None:
+        lse = torch.empty((Hq, total_q), dtype=torch.float32, device=q.device)
+    st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
+    a = VarlenKvcacheArgs(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), nptr, vptr, out.data_ptr(),
+                          lse.data_ptr(), cu_q.data_ptr(), cache_seqlens.data_ptr(), bt_ptr, cu_q.numel() - 1, Hq, Hkv,
+                          D, total_q, int(max_seqlen_q), nblk, page, mbps, q.stride(0), q.stride(1),
+                          k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1], _dtype_code(q),
+                          int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
+    check(lib().tfa_attn_varlen_kvcache_fwd(ctypes.byref(a)))
     return out, lse
 
 
