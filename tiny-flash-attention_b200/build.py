@@ -33,8 +33,8 @@ CXX = os.environ.get("CXX", "g++")
 LIB_NAME = "libtfa_b200.so"
 EXT_NAME = "attention_cutlass" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so")
 
-CU_SOURCES = ["tfa_api.cu", "tfa_rotary.cu", "tfa_varlen_kvcache.cu", "tfa_selftest.cu"]
-CU_HEADERS = ["ptx_sm90.cuh", "fa_fwd_sm90.cuh", "fa_splitkv_combine.cuh"]
+CU_SOURCES = ["tfa_api.cu", "tfa_append.cu", "tfa_varlen_kvcache.cu", "tfa_selftest.cu"]
+CU_HEADERS = ["ptx_sm90.cuh", "fa_fwd_sm90.cuh", "fa_fwd_launch.cuh", "fa_splitkv_combine.cuh"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [
     "-O3", "-std=c++17", "-lineinfo",

@@ -275,6 +275,51 @@ std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Ten
 
 namespace {
 
+// The cache's shape as the cache entry points pass it to the library.
+struct CacheShape {
+  int64_t nblk, page, Hkv, mbps, bts;
+};
+
+// The arguments both cache entry points share, for a q of B sequences: the caches, cache_seqlens, block_table and the
+// pairing, device and dtype of k_new / v_new.  Each entry point checks the shapes of its q and k_new itself.  Throws
+// on a bad argument, before any device work.
+CacheShape check_cache(const torch::Tensor& q, int64_t B, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
+                       const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
+                       const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new) {
+  TFA_CHECK_CUDA(k_cache);
+  TFA_CHECK_CUDA(v_cache);
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "k_cache, v_cache must have 4 dimensions");
+  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
+  TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
+              "k_cache and v_cache must have identical shapes and strides");
+  TORCH_CHECK(q.stride(-1) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
+  TORCH_CHECK(k_cache.size(3) == q.size(-1), "the caches must share head_dim with q");
+  TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
+                  cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == B,
+              "cache_seqlens must be a contiguous int32 (B,) tensor on q's device");
+  CacheShape c{k_cache.size(0), k_cache.size(1), k_cache.size(2), 1, 1};
+  if (block_table.has_value()) {
+    const torch::Tensor& bt = *block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == B &&
+                    bt.stride(1) == 1,
+                "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
+    TORCH_CHECK(c.page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
+                                           static_cast<long long>(c.page)));
+    c.mbps = bt.size(1);
+    c.bts = bt.stride(0);
+  } else {
+    TORCH_CHECK(c.nblk == B, "without block_table the caches must be (B, capacity, Hkv, D)");
+  }
+  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
+  if (k_new.has_value()) {
+    const torch::Tensor &kn = *k_new, &vn = *v_new;
+    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
+                    vn.scalar_type() == q.scalar_type(),
+                "k_new and v_new must be on q's device with q's dtype");
+  }
+  return c;
+}
+
 // A KV-cache call's tensors after check_kvcache(): the optional ones resolved, and the shape facts the fill needs.
 struct KvcacheCall {
   torch::Tensor q, k_cache, v_cache, cache_seqlens;
@@ -288,40 +333,14 @@ KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, 
                           const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
                           int64_t num_splits) {
   TFA_CHECK_CUDA(q);
-  TFA_CHECK_CUDA(k_cache);
-  TFA_CHECK_CUDA(v_cache);
-  TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "q, k_cache, v_cache must have 4 dimensions");
-  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
-  TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
-              "k_cache and v_cache must have identical shapes and strides");
-  TORCH_CHECK(q.stride(3) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
-  TORCH_CHECK(k_cache.size(3) == q.size(3), "the caches must share head_dim with q");
-  TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
-                  cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == q.size(0),
-              "cache_seqlens must be a contiguous int32 (B,) tensor on q's device");
+  TORCH_CHECK(q.dim() == 4, "q must have 4 dimensions (B, Sq, Hq, D)");
+  const CacheShape cs = check_cache(q, q.size(0), k_cache, v_cache, cache_seqlens, block_table, k_new, v_new);
   KvcacheCall c{q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new};
   c.B = q.size(0); c.Sq = q.size(1); c.Hq = q.size(2); c.D = q.size(3);
-  c.nblk = k_cache.size(0); c.page = k_cache.size(1); c.Hkv = k_cache.size(2);
-  c.mbps = 1; c.bts = 1;
-  if (block_table.has_value()) {
-    const torch::Tensor& bt = *block_table;
-    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == c.B &&
-                    bt.stride(1) == 1,
-                "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
-    TORCH_CHECK(c.page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
-                                           static_cast<long long>(c.page)));
-    c.mbps = bt.size(1);
-    c.bts = bt.stride(0);
-  } else {
-    TORCH_CHECK(c.nblk == c.B, "without block_table the caches must be (B, capacity, Hkv, D)");
-  }
-  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
+  c.nblk = cs.nblk; c.page = cs.page; c.Hkv = cs.Hkv; c.mbps = cs.mbps; c.bts = cs.bts;
   c.snew = 0;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
-    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
-                    vn.scalar_type() == q.scalar_type(),
-                "k_new and v_new must be on q's device with q's dtype");
     TORCH_CHECK(kn.dim() == 4 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == c.B &&
                     kn.size(2) == c.Hkv && kn.size(3) == c.D && kn.stride(3) == 1,
                 "k_new and v_new must be (B, Snew, Hkv, D) with identical strides and a unit head_dim stride");
@@ -460,15 +479,7 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
     std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale) {
   TFA_CHECK_CUDA(q);
-  TFA_CHECK_CUDA(k_cache);
-  TFA_CHECK_CUDA(v_cache);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
-  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "k_cache, v_cache must have 4 dimensions");
-  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
-  TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
-              "k_cache and v_cache must have identical shapes and strides");
-  TORCH_CHECK(q.stride(2) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
-  TORCH_CHECK(k_cache.size(3) == q.size(2), "the caches must share head_dim with q");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
   TORCH_CHECK(cu_seqlens_q.device() == q.device(), "cu_seqlens_q must be on q's device");
   TORCH_CHECK(cu_seqlens_q.dim() == 1 && cu_seqlens_q.is_contiguous(), "cu_seqlens_q must be a contiguous 1-D tensor");
@@ -476,29 +487,10 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
                                                  static_cast<long long>(cu_seqlens_q.numel())));
   const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2);
   const int64_t B = cu_seqlens_q.numel() - 1;
-  const int64_t nblk = k_cache.size(0), page = k_cache.size(1), Hkv = k_cache.size(2);
-  TORCH_CHECK(cache_seqlens.scalar_type() == at::kInt && cache_seqlens.device() == q.device() &&
-                  cache_seqlens.dim() == 1 && cache_seqlens.is_contiguous() && cache_seqlens.numel() == B,
-              "cache_seqlens must be a contiguous int32 (B,) tensor on q's device, B = cu_seqlens_q.numel() - 1");
-  int64_t mbps = 1, bts = 1;
-  if (block_table.has_value()) {
-    const torch::Tensor& bt = *block_table;
-    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.device() == q.device() && bt.dim() == 2 && bt.size(0) == B &&
-                    bt.stride(1) == 1,
-                "block_table must be an int32 (B, max_blocks_per_seq) tensor on q's device with unit column stride");
-    TORCH_CHECK(page % 128 == 0, fmt_msg("a paged cache needs page_block_size % 128 == 0, got %lld",
-                                         static_cast<long long>(page)));
-    mbps = bt.size(1);
-    bts = bt.stride(0);
-  } else {
-    TORCH_CHECK(nblk == B, "without block_table the caches must be (B, capacity, Hkv, D)");
-  }
-  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
+  const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new);
+  const int64_t nblk = cs.nblk, page = cs.page, Hkv = cs.Hkv, mbps = cs.mbps, bts = cs.bts;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
-    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
-                    vn.scalar_type() == q.scalar_type(),
-                "k_new and v_new must be on q's device with q's dtype");
     TORCH_CHECK(kn.dim() == 3 && kn.sizes() == vn.sizes() && kn.strides() == vn.strides() && kn.size(0) == total_q &&
                     kn.size(1) == Hkv && kn.size(2) == D && kn.stride(2) == 1,
                 "k_new and v_new must be (total_q, Hkv, D) with identical strides and a unit head_dim stride");

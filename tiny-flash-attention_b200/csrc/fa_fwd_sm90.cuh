@@ -58,36 +58,22 @@ __host__ __device__ __forceinline__ void page_lookup(const int* block_table, lon
   row = key - pg * page;
 }
 __host__ __device__ __forceinline__ bool block_ok(int blk, int num_blocks) { return blk >= 0 && blk < num_blocks; }
-// Element offset, in a cache with (block, row, head) element strides cs_b / cs_s / cs_h, of appended token i of
-// sequence b at head h, or -1 when its block-table entry lies outside [0, num_blocks) (the token is then dropped).
-__host__ __device__ __forceinline__ long long append_offset(const int* cache_seqlens, const int* block_table,
-                                                            long long bt_stride, int b, int i, int h, int page,
-                                                            int capacity, int snew, int num_blocks, long long cs_b,
-                                                            long long cs_s, long long cs_h) {
-  const int key = cache_len(cache_seqlens[b], capacity, snew) + i;
-  int blk, row;
-  page_lookup(block_table, bt_stride, b, key, page, blk, row);
-  if (!block_ok(blk, num_blocks)) return -1;
-  return blk * cs_b + row * cs_s + h * cs_h;
+// Sequence b appends n keys (n = 0: no append) and keeps the first min(n, capacity) of them: the rest do not fit and
+// are dropped.  n exceeds the capacity only in the variable-length call, whose n_b = min(Sq_b, max_seqlen_q) the host
+// does not know.  L = its clamped cached length (cache_len of the kept count), K = the keys it attends.
+__host__ __device__ __forceinline__ void cache_lens(int raw, int capacity, int n, int& L, int& K) {
+  const int kept = min(n, capacity);
+  L = cache_len(raw, capacity, kept);
+  K = L + kept;
 }
-
-// ---- the variable-length batch against a KV cache (kVarlenCache) ----
-// Sequence b has n = min(Sq_b, max_seqlen_q) query rows, and as many appended keys when the call appends (n = 0
-// otherwise).  Its cached length L is clamped to [0, max(capacity - n, 0)] and it attends to K = min(L + n, capacity)
-// keys: appended keys that do not fit the capacity (n > capacity) are dropped.  Unlike cache_len, n may exceed the
-// capacity, since the host does not know it.
-__host__ __device__ __forceinline__ void varlen_cache_lens(int raw, int capacity, int n, int& L, int& K) {
-  L = min(max(raw, 0), max(capacity - n, 0));
-  K = min(L + n, capacity);
-}
-// Element offset of appended token i (0 <= i < n) of sequence b at head h, as append_offset, or -1 when the token
-// does not fit the capacity or its block-table entry lies outside [0, num_blocks) (the token is then dropped).
-__host__ __device__ __forceinline__ long long varlen_append_offset(int raw, const int* block_table, long long bt_stride,
-                                                                   int b, int i, int h, int page, int capacity, int n,
-                                                                   int num_blocks, long long cs_b, long long cs_s,
-                                                                   long long cs_h) {
+// Element offset, in a cache with (block, row, head) element strides cs_b / cs_s / cs_h, of appended token i
+// (0 <= i < n) of sequence b at head h (raw = cache_seqlens[b]), or -1 when the token is dropped: it does not fit the
+// capacity (i >= min(n, capacity)) or its block-table entry lies outside [0, num_blocks).
+__host__ __device__ __forceinline__ long long append_offset(int raw, const int* block_table, long long bt_stride, int b,
+                                                            int i, int h, int page, int capacity, int n, int num_blocks,
+                                                            long long cs_b, long long cs_s, long long cs_h) {
   int L, K;
-  varlen_cache_lens(raw, capacity, n, L, K);
+  cache_lens(raw, capacity, n, L, K);
   const int key = L + i;
   if (key >= K) return -1;
   int blk, row;
@@ -151,7 +137,7 @@ struct FwdParams {
   // cache_len(cache_seqlens[b]) + snew keys of its cache, whose key r lives at page_lookup(block_table, b, r).  The
   // K/V tensor maps are (D, page, Hkv, num_blocks).  Sk / causal_off are unused.
   // kVarlenCache: q / out / lse as varlen (cu_q, total_q; cu_k unused), K/V as kCache; sequence b attends to the
-  // varlen_cache_lens() keys of its n_b = min(Sq_b, S) rows, with n_b appended keys when snew != 0 (a flag here).
+  // cache_lens() keys of its n_b = min(Sq_b, S) rows, with n_b appended keys when snew != 0 (a flag here).
   const int* cache_seqlens;
   const int* block_table;     // nullptr: contiguous cache, page = capacity
   long long bt_stride;
@@ -252,7 +238,7 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.k0 = 0;
     w.Sq = min(max(q1 - q0, 0), p.S);
     int L;
-    varlen_cache_lens(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew ? w.Sq : 0, L, w.Sk);
+    cache_lens(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew ? w.Sq : 0, L, w.Sk);
     w.coff = w.Sk - w.Sq;
   } else {
     w.q0 = 0;

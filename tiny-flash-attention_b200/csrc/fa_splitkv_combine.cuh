@@ -1,7 +1,7 @@
 // fa_splitkv_combine.cuh -- the small HBM-bound kernels either side of the attention forward when the problem
-// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append (kvcache_append_kernel, below),
-// its variable-length variant (kvcache_varlen_append_kernel, launched from tfa_varlen_kvcache.cu) and its rotary
-// variant (kvcache_rotary_append_kernel, launched from tfa_rotary.cu):
+// is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append of both cache calls
+// (kvcache_append_kernel, below) and its rotary variant (kvcache_rotary_append_kernel), both launched from
+// tfa_append.cu:
 //
 //   * splitkv_combine_kernel: merges the per-split partial results of the split-KV forward,
 //       O = sum_s exp(lse_s - LSE) * O_s ,  LSE = log sum_s exp(lse_s)
@@ -108,83 +108,70 @@ __global__ void __launch_bounds__(256) empty_rows_fill_kernel(const FillParams p
   if (p.lse != nullptr && sub == 0) p.lse[p.ol.lse(b, h, i)] = INFINITY;
 }
 
-// kvcache_append_kernel: writes k_new / v_new (B, snew, Hkv, D) into the (paged) KV cache at keys
-// [L_b, L_b + snew) of each sequence, L_b = cache_len(cache_seqlens[b]), before the forward reads the cache.  One thread
-// copies one 16-byte chunk of K and the same chunk of V.  cache_seqlens is not incremented.  A token whose block-table
-// entry lies outside [0, num_blocks) is dropped: no store leaves the cache.  Algorithmic bytes: 2 * 2 * B*snew*Hkv*D
-// read and written.
+// kvcache_append_kernel: writes k_new / v_new into the (paged) KV cache at keys [L_b, L_b + n_b) of each sequence,
+// before the forward reads the cache (L_b from cache_lens).  The dense-query call appends n_b = snew rows of
+// (B, snew, Hkv, D) k_new / v_new.  The variable-length call (cu_q set) appends rows cu_q[b] + i, i < n_b =
+// min(Sq_b, snew), of packed (total_q, Hkv, D) ones, with snew = max_seqlen_q as its forward's grid covers max_seqlen_q
+// rows of every sequence: a chunk with i >= n_b returns, so no search over cu_seqlens is needed.  The grid is
+// B * snew * Hkv * D/8 chunks; one thread copies one 16-byte chunk of K and the same chunk of V.  cache_seqlens is not
+// incremented.  A token past the capacity or behind a block-table entry outside [0, num_blocks) is dropped: no store
+// leaves the cache.  Algorithmic bytes: 2 * 2 * (appended tokens) * Hkv * D read and written.
 struct AppendParams {
   const void* k_new;
   const void* v_new;
   void* k_cache;
   void* v_cache;
-  long long n_sb, n_ss, n_sh;     // element strides of k_new / v_new
+  long long n_sb, n_ss, n_sh;     // element strides of k_new / v_new (n_sb = 0 when packed)
   long long c_sb, c_ss, c_sh;     // element strides of the caches: block, row, head
   const int* cache_seqlens;
   const int* block_table;         // nullptr: contiguous cache
   long long bt_stride;
+  const int* cu_q;                // nullptr: k_new / v_new are (B, snew, Hkv, D); else packed as q, total_q rows
+  int total_q;
   int page, capacity, snew, num_blocks, Hkv;
   long long chunks;               // B * snew * Hkv * D / 8
 };
 
+// Chunk c < p.chunks of the append: 16-byte chunk `sub` of appended token i of sequence b at head h, read at element
+// src of k_new / v_new and written at element dst of the caches, or dropped (dst < 0).
+struct AppendChunk {
+  int b, i, h, sub;
+  long long src, dst;
+};
 template <int D>
-__global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendParams p) {
+__device__ __forceinline__ AppendChunk append_chunk(const AppendParams& p, long long c) {
   constexpr int CPR = D / 8;                   // 16-byte chunks per row
-  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
-  if (c >= p.chunks) return;
-  const int sub = static_cast<int>(c % CPR);
+  AppendChunk a;
+  a.sub = static_cast<int>(c % CPR);
   long long r = c / CPR;
-  const int h = static_cast<int>(r % p.Hkv);
+  a.h = static_cast<int>(r % p.Hkv);
   r /= p.Hkv;
-  const int i = static_cast<int>(r % p.snew);
-  const int b = static_cast<int>(r / p.snew);
-  const long long dst = append_offset(p.cache_seqlens, p.block_table, p.bt_stride, b, i, h, p.page, p.capacity,
-                                      p.snew, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
-  if (dst < 0) return;
-  const long long src = b * p.n_sb + i * p.n_ss + h * p.n_sh + sub * 8;
-  const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
-  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + dst + sub * 8) = vx;
+  a.i = static_cast<int>(r % p.snew);
+  a.b = static_cast<int>(r / p.snew);
+  int q0 = 0, n = p.snew;
+  if (p.cu_q) {
+    // the forward's clamps (decode_item): whatever cu_seqlens holds, no row outside [0, total_q) is read
+    q0 = min(max(__ldg(p.cu_q + a.b), 0), p.total_q);
+    const int q1 = min(max(__ldg(p.cu_q + a.b + 1), 0), p.total_q);
+    n = min(max(q1 - q0, 0), p.snew);
+  }
+  a.dst = append_offset(__ldg(p.cache_seqlens + a.b), p.block_table, p.bt_stride, a.b, a.i, a.h, p.page, p.capacity, n,
+                        p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
+  a.src = a.b * p.n_sb + (q0 + a.i) * p.n_ss + a.h * p.n_sh;
+  return a;
 }
 
-// kvcache_varlen_append_kernel: the append of a variable-length batch (the kVarlenCache forward, launched from
-// tfa_varlen_kvcache.cu).  k_new / v_new are packed (total_q, Hkv, D) as q is: row cu_q[b] + i is key L_b + i of
-// sequence b, for i < n_b = min(Sq_b, max_seqlen_q), at varlen_append_offset().  The grid is B * max_seqlen_q * Hkv *
-// D/8 chunks, one 16-byte chunk of K and of V per thread, as the forward's grid covers max_seqlen_q rows of every
-// sequence: a chunk with i >= n_b returns, so no search over cu_seqlens is needed.  A token past the capacity or with a
-// block-table entry outside [0, num_blocks) is dropped.  Here ap.snew is max_seqlen_q and ap.n_sb is unused.
-struct VarlenAppendParams {
-  AppendParams ap;
-  const int* cu_q;
-  int total_q;
-};
-
 template <int D>
-__global__ void __launch_bounds__(256) kvcache_varlen_append_kernel(const VarlenAppendParams vp) {
-  constexpr int CPR = D / 8;                   // 16-byte chunks per row
-  const AppendParams& p = vp.ap;
+__global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendParams p) {
   const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   if (c >= p.chunks) return;
-  const int sub = static_cast<int>(c % CPR);
-  long long r = c / CPR;
-  const int h = static_cast<int>(r % p.Hkv);
-  r /= p.Hkv;
-  const int i = static_cast<int>(r % p.snew);
-  const int b = static_cast<int>(r / p.snew);
-  // the forward's clamps (decode_item): whatever cu_seqlens holds, no row outside [0, total_q) is read
-  const int q0 = min(max(__ldg(vp.cu_q + b), 0), vp.total_q);
-  const int q1 = min(max(__ldg(vp.cu_q + b + 1), 0), vp.total_q);
-  const int n = min(max(q1 - q0, 0), p.snew);
-  if (i >= n) return;
-  const long long dst = varlen_append_offset(__ldg(p.cache_seqlens + b), p.block_table, p.bt_stride, b, i, h, p.page,
-                                             p.capacity, n, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
-  if (dst < 0) return;
-  const long long src = (q0 + i) * p.n_ss + h * p.n_sh + sub * 8;
+  const AppendChunk a = append_chunk<D>(p, c);
+  if (a.dst < 0) return;
+  const long long src = a.src + a.sub * 8;
   const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
   const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + dst + sub * 8) = kx;
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + dst + sub * 8) = vx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.k_cache) + a.dst + a.sub * 8) = kx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.v_cache) + a.dst + a.sub * 8) = vx;
 }
 
 // ---- rotary position embedding (RoPE) for the KV-cache forward: flash-attn's rotary_cos / rotary_sin ----
@@ -268,10 +255,10 @@ __device__ __forceinline__ uint4 rotate_chunk(const uint16_t* row, int sub, cons
                     pack_16x2<IS_BF16>(r[6], r[7]));
 }
 
-// kvcache_rotary_append_kernel: the append of kvcache_append_kernel with RoPE, plus the rotated queries, in one launch.
-// Chunks [0, q_chunks) write rot(q) into the contiguous (B, Sq, Hq, D) buffer q_rot, which the forward then reads in
-// place of q; the remaining chunks write rot(k_new) and v_new (unrotated) into the cache at keys [L_b, L_b + snew),
-// dropping a token whose block-table entry lies outside [0, num_blocks) as the plain append does.  Positions:
+// kvcache_rotary_append_kernel: the append of kvcache_append_kernel with RoPE, plus the rotated queries, in one launch
+// (the dense-query call only: cu_q is nullptr).  Chunks [0, q_chunks) write rot(q) into the contiguous (B, Sq, Hq, D)
+// buffer q_rot, which the forward then reads in place of q; the remaining chunks write rot(k_new) and v_new
+// (unrotated) into the cache at keys [L_b, L_b + snew), through the plain append's append_chunk().  Positions:
 // rotary_pos().  One thread per 16-byte output chunk (a NeoX chunk also reads its partner chunk and 16 bytes each of
 // cos and sin).  Algorithmic bytes: 2 * B*Sq*Hq*D * 2 (q in, q_rot out) + 2 * 2 * B*snew*Hkv*D * 2 (k/v in and out),
 // plus the cos/sin rows.
@@ -289,41 +276,37 @@ struct RotaryAppendParams {
 template <int D, bool IS_BF16, bool INTERLEAVED>
 __global__ void __launch_bounds__(256) kvcache_rotary_append_kernel(const RotaryAppendParams p) {
   constexpr int CPR = D / 8;                   // 16-byte chunks per row
-  long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
-  const bool is_q = c < p.q_chunks;
-  if (!is_q) {
-    c -= p.q_chunks;
-    if (c >= p.ap.chunks) return;
-  }
-  const int sub = static_cast<int>(c % CPR);
-  long long r = c / CPR;                       // row index over (B, S, H), H fastest
-  const int H = is_q ? p.Hq : p.ap.Hkv;
-  const int S = is_q ? p.Sq : p.ap.snew;
-  const int h = static_cast<int>(r % H);
-  r /= H;
-  const int i = static_cast<int>(r % S);
-  const int b = static_cast<int>(r / S);
-  const int len = cache_len(__ldg(p.ap.cache_seqlens + b), p.ap.capacity, p.ap.snew);
-  const long long ro = static_cast<long long>(rotary_pos(len, i, p.causal != 0, is_q, p.seqlen_ro)) * (p.rotary_dim / 2);
-  const uint16_t* cos_row = static_cast<const uint16_t*>(p.cos) + ro;
-  const uint16_t* sin_row = static_cast<const uint16_t*>(p.sin) + ro;
-  if (is_q) {
+  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  const AppendParams& a = p.ap;
+  const uint16_t* cos_tab = static_cast<const uint16_t*>(p.cos);
+  const uint16_t* sin_tab = static_cast<const uint16_t*>(p.sin);
+  if (c < p.q_chunks) {
+    const int sub = static_cast<int>(c % CPR);
+    long long r = c / CPR;                     // row index over (B, Sq, Hq), Hq fastest
+    const int h = static_cast<int>(r % p.Hq);
+    r /= p.Hq;
+    const int i = static_cast<int>(r % p.Sq);
+    const int b = static_cast<int>(r / p.Sq);
+    const int len = cache_len(__ldg(a.cache_seqlens + b), a.capacity, a.snew);
+    const long long ro =
+        static_cast<long long>(rotary_pos(len, i, p.causal != 0, true, p.seqlen_ro)) * (p.rotary_dim / 2);
     const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + i * p.q_ss + h * p.q_sh;
-    const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_row, sin_row, p.rotary_dim);
+    const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_tab + ro, sin_tab + ro, p.rotary_dim);
     reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + ((static_cast<long long>(b) * p.Sq + i) * p.Hq + h) * D)
         [sub] = y;
     return;
   }
-  const AppendParams& a = p.ap;
-  const long long dst = append_offset(a.cache_seqlens, a.block_table, a.bt_stride, b, i, h, a.page, a.capacity, a.snew,
-                                      a.num_blocks, a.c_sb, a.c_ss, a.c_sh);
-  if (dst < 0) return;
-  const long long src = b * a.n_sb + i * a.n_ss + h * a.n_sh;
-  const uint4 kx = rotate_chunk<IS_BF16, INTERLEAVED>(static_cast<const uint16_t*>(a.k_new) + src, sub, cos_row,
-                                                      sin_row, p.rotary_dim);
-  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + src) + sub);
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.k_cache) + dst + sub * 8) = kx;
-  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.v_cache) + dst + sub * 8) = vx;
+  if (c - p.q_chunks >= a.chunks) return;
+  const AppendChunk k = append_chunk<D>(a, c - p.q_chunks);
+  if (k.dst < 0) return;
+  const int len = cache_len(__ldg(a.cache_seqlens + k.b), a.capacity, a.snew);
+  const long long ro =
+      static_cast<long long>(rotary_pos(len, k.i, p.causal != 0, false, p.seqlen_ro)) * (p.rotary_dim / 2);
+  const uint4 kx = rotate_chunk<IS_BF16, INTERLEAVED>(static_cast<const uint16_t*>(a.k_new) + k.src, k.sub,
+                                                      cos_tab + ro, sin_tab + ro, p.rotary_dim);
+  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + k.src) + k.sub);
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.k_cache) + k.dst + k.sub * 8) = kx;
+  *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.v_cache) + k.dst + k.sub * 8) = vx;
 }
 
 }  // namespace tfa

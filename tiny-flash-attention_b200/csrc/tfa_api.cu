@@ -8,7 +8,7 @@
 // Differences on purpose (SURVEY.md A.2): arguments are validated and rejected loudly, the
 // caller's stream is honoured, nothing synchronises the device, nothing calls exit().
 #include "../../include/tfa_b200.h"
-#include "fa_fwd_sm90.cuh"
+#include "fa_fwd_launch.cuh"
 #include "fa_splitkv_combine.cuh"
 
 #include <cuda_runtime.h>
@@ -16,18 +16,20 @@
 #include <atomic>
 #include <cassert>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 #include <cstdlib>
 #include <cstring>
 
-// tfa_rotary.cu: the rotary append's launch, compiled apart from the forward kernels
+// tfa_append.cu: the appends' launches, compiled apart from the forward kernels
+int tfa_internal_launch_append(const tfa::AppendParams& p, int D, cudaStream_t stream);
 int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
                                       cudaStream_t stream);
-// tfa_varlen_kvcache.cu: the variable-length cache forward and its append, compiled apart from the other forward kernels
-int tfa_internal_launch_varlen_kvcache_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq,
-                                           const CUtensorMap& tk, const CUtensorMap& tv, const tfa::FwdParams& p,
-                                           int nblocks, bool persist, cudaStream_t stream);
-int tfa_internal_launch_varlen_append(const tfa::VarlenAppendParams& vp, int D, cudaStream_t stream);
+// tfa_varlen_kvcache.cu: the variable-length cache forward, compiled apart from the other forward kernels
+extern template cudaError_t tfa::launch_forward<tfa::kVarlenCache>(int D, bool causal, bool bf16, bool f32,
+                                                                   const CUtensorMap& tq, const CUtensorMap& tk,
+                                                                   const CUtensorMap& tv, const tfa::FwdParams& p,
+                                                                   int nblocks, bool persist, cudaStream_t stream);
 
 namespace {
 
@@ -139,13 +141,6 @@ int choose_kernel(bool causal, long long npairs, int n_extra) {
   return npairs <= 8 ? KV_PERSIST : KV_CLASSIC;
 }
 
-// cudaFuncSetAttribute is per device (context) and costs well under a microsecond: set it on every launch instead of
-// caching "done once" per process, which breaks the first launch on a second GPU of the same process.
-template <typename K>
-cudaError_t opt_in_smem(K kernel, int bytes) {
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-
 // Every launch ends here: count it (tfa_launch_count) and report a launch error.
 int count_launch() {
   g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -171,34 +166,6 @@ long long fwd_grid(long long nitems, int variant) {
   return nitems > sms ? sms : nitems;                                   // one CTA per SM
 }
 
-template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, int MODE>
-int launch_inst(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, FwdParams p, long long nitems,
-                int variant, cudaStream_t stream) {
-  const bool persist = variant == KV_PERSIST;
-  const long long nblocks = fwd_grid(nitems, variant);
-  if (nblocks <= 0) return TFA_EARCH;
-  auto kern = persist ? tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, true, MODE>
-                      : tfa::fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
-  const cudaError_t cerr = opt_in_smem(kern, FwdCfg<D>::SMEM_BYTES);
-  if (cerr != cudaSuccess) return static_cast<int>(cerr);
-  kern<<<static_cast<int>(nblocks), FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
-  return count_launch();
-}
-
-template <int D, int MODE>
-int dispatch(bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
-             const FwdParams& p, long long nblocks, int variant, cudaStream_t s) {
-#define TFA_GO(C_, B_, F_) return launch_inst<D, C_, B_, F_, MODE>(tq, tk, tv, p, nblocks, variant, s)
-  if (causal) {
-    if (bf16) { if (f32) TFA_GO(true, true, true); else TFA_GO(true, true, false); }
-    else      { if (f32) TFA_GO(true, false, true); else TFA_GO(true, false, false); }
-  } else {
-    if (bf16) { if (f32) TFA_GO(false, true, true); else TFA_GO(false, true, false); }
-    else      { if (f32) TFA_GO(false, false, true); else TFA_GO(false, false, false); }
-  }
-#undef TFA_GO
-}
-
 // One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache /
 // kVarlenCache).
 template <int MODE>
@@ -206,19 +173,11 @@ int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, c
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
   if (nitems > 0x3fffffffLL) return TFA_EINVAL_SHAPE;
   p.total_items = static_cast<int>(nitems);
-  // kVarlenCache is instantiated only in tfa_varlen_kvcache.cu.  The dispatch must stay in the `else` branch: a
-  // statement after a returning `if constexpr` is still instantiated, and would compile this mode's 32 kernels into
-  // this translation unit as well (a second, unused copy under the same names).
-  if constexpr (MODE == tfa::kVarlenCache) {
-    const long long nblocks = fwd_grid(nitems, variant);
-    if (nblocks <= 0) return TFA_EARCH;
-    const int rc = tfa_internal_launch_varlen_kvcache_fwd(D, causal, bf16, f32, tq, tk, tv, p, static_cast<int>(nblocks),
-                                                          variant == KV_PERSIST, stream);
-    return rc ? rc : count_launch();
-  } else {
-    if (D == 64) return dispatch<64, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
-    return dispatch<128, MODE>(causal, bf16, f32, tq, tk, tv, p, nitems, variant, stream);
-  }
+  const long long nblocks = fwd_grid(nitems, variant);
+  if (nblocks <= 0) return TFA_EARCH;
+  const cudaError_t e = tfa::launch_forward<MODE>(D, causal, bf16, f32, tq, tk, tv, p, static_cast<int>(nblocks),
+                                                  variant == KV_PERSIST, stream);
+  return e != cudaSuccess ? static_cast<int>(e) : count_launch();
 }
 
 bool arch_ok() {
@@ -539,9 +498,11 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   return q;
 }
 
-// The cache arguments the cache calls share: the lengths, the block table or the contiguous cache, k_new with v_new.
+// The cache arguments of both cache calls: the lengths, the block table or the contiguous cache, k_new with v_new and
+// their strides.  Only the dense-query call has Snew and a batch stride of k_new.
 template <typename Args>
 int validate_cache(const Args& ka) {
+  constexpr bool dense_q = std::is_same_v<Args, tfa_attn_kvcache_args>;
   if (!ka.cache_seqlens || (reinterpret_cast<uintptr_t>(ka.cache_seqlens) & 3u) ||
       (reinterpret_cast<uintptr_t>(ka.block_table) & 3u))
     return TFA_EINVAL_KVCACHE;
@@ -552,19 +513,42 @@ int validate_cache(const Args& ka) {
     return TFA_EINVAL_KVCACHE;           // contiguous: one page (block b) per sequence
   }
   if ((ka.k_new == nullptr) != (ka.v_new == nullptr)) return TFA_EINVAL_KVCACHE;
+  if (ka.k_new) {
+    if constexpr (dense_q) {
+      const long long cap = static_cast<long long>(ka.max_blocks_per_seq) * ka.page_block_size;
+      if (ka.Snew < 1 || ka.Snew > cap) return TFA_EINVAL_KVCACHE;
+    }
+    if ((reinterpret_cast<uintptr_t>(ka.k_new) | reinterpret_cast<uintptr_t>(ka.v_new)) & 15u) return TFA_EINVAL_PTR;
+    if ((ka.new_stride_s % 8) || (ka.new_stride_h % 8) || ka.new_stride_s < 0 || ka.new_stride_h < 0)
+      return TFA_EINVAL_STRIDE;
+    if constexpr (dense_q) {
+      if ((ka.new_stride_b % 8) || ka.new_stride_b < 0) return TFA_EINVAL_STRIDE;
+    }
+  }
   return 0;
 }
 
-int validate_kvcache(const tfa_attn_kvcache_args& ka) {
-  if (int rc = validate_cache(ka)) return rc;
-  if (ka.k_new) {
-    const long long cap = static_cast<long long>(ka.max_blocks_per_seq) * ka.page_block_size;
-    if (ka.Snew < 1 || ka.Snew > cap) return TFA_EINVAL_KVCACHE;
-    if ((reinterpret_cast<uintptr_t>(ka.k_new) | reinterpret_cast<uintptr_t>(ka.v_new)) & 15u) return TFA_EINVAL_PTR;
-    if ((ka.new_stride_s % 8) || (ka.new_stride_h % 8) || (ka.new_stride_b % 8) || ka.new_stride_s < 0 ||
-        ka.new_stride_h < 0 || ka.new_stride_b < 0)
-      return TFA_EINVAL_STRIDE;
-  }
+// The cache side of a cache call whose arguments passed (a = its Problem, capacity = a.Sk): the K/V tensor maps over
+// the pages, the append of `n` rows per sequence (ap.chunks = 0 without k_new; the caller sets its k_new layout fields
+// n_sb / cu_q / total_q) and the cache fields of the forward but snew.
+template <typename Args>
+int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtensorMap& tv, tfa::AppendParams& ap,
+                FwdParams& p) {
+  const int page = ka.block_table ? ka.page_block_size : a.Sk;
+  if (int rc = make_tmap(&tk, a.k, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
+  if (int rc = make_tmap(&tv, a.v, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
+  ap = tfa::AppendParams{};
+  ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
+  ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
+  ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
+  ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
+  ap.page = page; ap.capacity = a.Sk; ap.snew = n; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
+  ap.chunks = ka.k_new ? static_cast<long long>(a.B) * n * a.Hkv * (a.D / 8) : 0;
+  p.cache_seqlens = ka.cache_seqlens;
+  p.block_table = ka.block_table;
+  p.bt_stride = ka.block_table_stride;
+  p.page = page;
+  p.capacity = a.Sk;
   return 0;
 }
 
@@ -584,30 +568,19 @@ int validate_rotary(const tfa_attn_kvcache_args& ka, const Problem& a, const tfa
 // place of the plain append) and the forward reads its queries from ra->q_rot.
 int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
   Problem a = from_kvcache_args(ka);
-  int rc = validate_kvcache(ka);        // first: a table of 0 pages is a cache error, not a 0-key shape error
+  int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if (ra && (rc = validate_rotary(ka, a, *ra))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-  const int capacity = a.Sk;
   const int snew = ka.k_new ? ka.Snew : 0;
-  const int page = ka.block_table ? ka.page_block_size : capacity;
 
   SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
   if ((rc = plan_splits(a, plan))) return rc;
 
-  tfa::AppendParams ap;
-  ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
-  ap.n_sb = ka.new_stride_b; ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
-  ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
-  ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
-  ap.page = page; ap.capacity = capacity; ap.snew = snew; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
-  ap.chunks = static_cast<long long>(a.B) * snew * a.Hkv * (a.D / 8);
-
   tfa::RotaryAppendParams rp;
   if (ra) {
-    rp.ap = ap;
     rp.q = a.q; rp.q_rot = ra->q_rot;
     rp.q_sb = a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
     rp.cos = ra->cos; rp.sin = ra->sin;
@@ -622,25 +595,20 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
   }
 
   CUtensorMap tq, tk, tv;
+  tfa::AppendParams ap;
+  FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
-  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+  if ((rc = setup_cache(ka, a, snew, tk, tv, ap, p))) return rc;
+  ap.n_sb = ka.new_stride_b;
 
   if (ra) {
+    rp.ap = ap;
     rc = tfa_internal_launch_rotary_append(rp, a.D, a.dtype == TFA_BF16, ra->interleaved != 0, a.stream);
     if (rc) return rc;
   } else if (snew > 0) {
-    rc = launch_small(a.D == 64 ? tfa::kvcache_append_kernel<64> : tfa::kvcache_append_kernel<128>, ap.chunks, 256, ap,
-                      a.stream);
-    if (rc) return rc;
+    if ((rc = tfa_internal_launch_append(ap, a.D, a.stream))) return rc;
   }
 
-  FwdParams p{};
-  p.cache_seqlens = ka.cache_seqlens;
-  p.block_table = ka.block_table;
-  p.bt_stride = ka.block_table_stride;
-  p.page = page;
-  p.capacity = capacity;
   p.snew = snew;
   // every split writes its rows (LSE = -inf where it saw no key): the combine reads all of them
   return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan, false);
@@ -667,46 +635,25 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va) {
   const Problem a = from_varlen_kvcache_args(va);
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
-  if (va.k_new) {
-    if ((reinterpret_cast<uintptr_t>(va.k_new) | reinterpret_cast<uintptr_t>(va.v_new)) & 15u) return TFA_EINVAL_PTR;
-    if ((va.new_stride_s % 8) || (va.new_stride_h % 8) || va.new_stride_s < 0 || va.new_stride_h < 0)
-      return TFA_EINVAL_STRIDE;
-  }
   if ((rc = validate(a))) return rc;
   if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
   if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-  const int capacity = a.Sk;
-  const int page = va.block_table ? va.page_block_size : capacity;
 
   CUtensorMap tq, tk, tv;
+  tfa::AppendParams ap;
+  FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
-  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, page, va.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, page, va.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-
+  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, ap, p))) return rc;
   if (va.k_new) {
-    tfa::VarlenAppendParams vp;
-    tfa::AppendParams& ap = vp.ap;
-    ap.k_new = va.k_new; ap.v_new = va.v_new; ap.k_cache = va.k_cache; ap.v_cache = va.v_cache;
-    ap.n_sb = 0; ap.n_ss = va.new_stride_s; ap.n_sh = va.new_stride_h;
-    ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
-    ap.cache_seqlens = va.cache_seqlens; ap.block_table = va.block_table; ap.bt_stride = va.block_table_stride;
-    ap.page = page; ap.capacity = capacity; ap.snew = va.max_seqlen_q; ap.num_blocks = va.num_blocks; ap.Hkv = a.Hkv;
-    ap.chunks = static_cast<long long>(a.B) * va.max_seqlen_q * a.Hkv * (a.D / 8);
-    vp.cu_q = va.cu_seqlens_q;
-    vp.total_q = a.Sq;
-    if ((rc = tfa_internal_launch_varlen_append(vp, a.D, a.stream))) return rc;
+    ap.cu_q = va.cu_seqlens_q;
+    ap.total_q = a.Sq;
+    if ((rc = tfa_internal_launch_append(ap, a.D, a.stream))) return rc;
   }
 
-  FwdParams p{};
   p.cu_q = va.cu_seqlens_q;
   p.total_q = a.Sq;
-  p.cache_seqlens = va.cache_seqlens;
-  p.block_table = va.block_table;
-  p.bt_stride = va.block_table_stride;
-  p.page = page;
-  p.capacity = capacity;
   p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
   // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
   return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
@@ -905,12 +852,26 @@ int tfa_internal_page_lookup(const int* block_table, long long bt_stride, int b,
   tfa::page_lookup(block_table, bt_stride, b, key, page, out2[0], out2[1]);
   return 0;
 }
+// The length rule and the append destination (cache_lens, append_offset), in the forms each cache call uses them; the
+// exhaustive tests call both forms.  The dense-query call: the clamped cached length for snew <= capacity appended
+// keys, and the destination of token i of sequence b read from cache_seqlens.
 int tfa_internal_cache_len(int raw, int capacity, int snew) { return tfa::cache_len(raw, capacity, snew); }
-long long tfa_internal_append_offset(const int* cache_seqlens, const int* block_table, long long bt_stride, int b, int i,
-                                     int h, int page, int capacity, int snew, int num_blocks, long long cs_b,
+long long tfa_internal_append_offset(const int* cache_seqlens, const int* block_table, long long bt_stride, int b,
+                                     int i, int h, int page, int capacity, int snew, int num_blocks, long long cs_b,
                                      long long cs_s, long long cs_h) {
-  return tfa::append_offset(cache_seqlens, block_table, bt_stride, b, i, h, page, capacity, snew, num_blocks, cs_b,
+  return tfa::append_offset(cache_seqlens[b], block_table, bt_stride, b, i, h, page, capacity, snew, num_blocks, cs_b,
                             cs_s, cs_h);
+}
+// The variable-length call: out2 = {L, K} for n query rows (n appended keys when `append`, which may exceed the
+// capacity), and the destination of token i (raw = cache_seqlens[b]), or -1 when the token is dropped.
+int tfa_internal_varlen_cache_lens(int raw, int capacity, int n, int append, int* out2) {
+  tfa::cache_lens(raw, capacity, append ? n : 0, out2[0], out2[1]);
+  return 0;
+}
+long long tfa_internal_varlen_append_offset(int raw, const int* block_table, long long bt_stride, int b, int i, int h,
+                                            int page, int capacity, int n, int num_blocks, long long cs_b,
+                                            long long cs_s, long long cs_h) {
+  return tfa::append_offset(raw, block_table, bt_stride, b, i, h, page, capacity, n, num_blocks, cs_b, cs_s, cs_h);
 }
 // development aid (not in the public header): the rotary position rule of fa_splitkv_combine.cuh on the host
 int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {

@@ -260,6 +260,22 @@ def attn_varlen_fwd(q, k, v, cu_q, cu_k, max_seqlen_q, is_causal, scale, out_fp3
     return out, lse
 
 
+def _cache_args(block_table, k_new, v_new, new_dims):
+    """What the two cache calls take of block_table, k_new and v_new: (max_blocks_per_seq, the table's row stride, its
+    pointer), or (1, 1, None) for a contiguous cache; then the k_new / v_new pointers and k_new's first `new_dims`
+    strides, or None, None and zeros without an append."""
+    import torch
+    if block_table is not None:
+        assert block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
+        bt = (block_table.shape[1], block_table.stride(0), block_table.data_ptr())
+    else:
+        bt = (1, 1, None)
+    if k_new is None:
+        return bt, None, None, (0,) * new_dims
+    assert k_new.shape == v_new.shape and k_new.stride() == v_new.stride() and k_new.stride(-1) == 1
+    return bt, k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:new_dims]
+
+
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
                      scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
                      rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None):
@@ -277,15 +293,8 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     assert cache_seqlens.dtype == torch.int32
     B, Sq, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    if block_table is not None:
-        assert block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
-        mbps, bts, bt_ptr = block_table.shape[1], block_table.stride(0), block_table.data_ptr()
-    else:
-        mbps, bts, bt_ptr = 1, 1, None
-    snew, nptr, vptr, ns = 0, None, None, (0, 0, 0)
-    if k_new is not None:
-        assert k_new.shape == v_new.shape and k_new.stride() == v_new.stride() and k_new.stride(3) == 1
-        snew, nptr, vptr, ns = k_new.shape[1], k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:3]
+    (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 3)
+    snew = k_new.shape[1] if k_new is not None else 0
     if scale is None:
         scale = D ** -0.5
     if out is None:
@@ -332,15 +341,7 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
     assert cu_q.dtype == torch.int32 and cu_q.numel() >= 2 and cache_seqlens.dtype == torch.int32
     total_q, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    if block_table is not None:
-        assert block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
-        mbps, bts, bt_ptr = block_table.shape[1], block_table.stride(0), block_table.data_ptr()
-    else:
-        mbps, bts, bt_ptr = 1, 1, None
-    nptr, vptr, ns = None, None, (0, 0)
-    if k_new is not None:
-        assert k_new.shape == v_new.shape and k_new.stride() == v_new.stride() and k_new.stride(2) == 1
-        nptr, vptr, ns = k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:2]
+    (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 2)
     if scale is None:
         scale = D ** -0.5
     if out is None:
