@@ -38,6 +38,7 @@ extern "C" {
 /* dtype codes (reference: Qkv_params::is_bf16, flash.h:27) */
 #define TFA_BF16 0
 #define TFA_FP16 1
+#define TFA_FP8_E4M3 2  /* cache element type of the quantized cache calls only (tfa_kv_quant_args) */
 
 /* argument errors */
 #define TFA_EINVAL_PTR    (-1)  /* null or not 16-byte aligned pointer           */
@@ -57,6 +58,8 @@ extern "C" {
                                       [1, capacity] */
 #define TFA_EINVAL_ROTARY (-14)    /* rotary: cos / sin / q_rot null or misaligned, rotary_dim not an even multiple of 16
                                       in [16, D], seqlen_ro < capacity, or no k_new */
+#define TFA_EINVAL_KVQUANT (-15)   /* FP8 cache: cache_dtype not TFA_FP8_E4M3, k_scale / v_scale not finite and > 0, or
+                                      cache strides not multiples of 16 elements */
 
 /* Extended argument block (POD), the analogue of Flash_fwd_params (flash.h:29-60).
  * Strides are in ELEMENTS.  The innermost (head_dim) stride must be 1.
@@ -327,6 +330,38 @@ typedef struct tfa_attn_varlen_kvcache_args {
 } tfa_attn_varlen_kvcache_args;
 
 int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args);
+
+/* ---- the KV-cache calls against an FP8 (e4m3) cache with per-tensor scales (vLLM's kv_cache_dtype="fp8") ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect them by the exported symbols
+ * tfa_attn_kvcache_fp8_fwd and tfa_attn_varlen_kvcache_fp8_fwd.  tfa_attn_kvcache_fwd() (with `rotary`:
+ * tfa_attn_kvcache_rotary_fwd()) and tfa_attn_varlen_kvcache_fwd() with k_cache / v_cache holding one byte per element.
+ * args->dtype stays q's dtype; q, k_new, v_new, out and lse keep their types.  Cache strides are in elements (bytes)
+ * and must be multiples of 16.
+ *
+ *   cache values : an element x8 (e4m3 codes, torch.float8_e4m3fn) stands for k_scale * x8 in K, v_scale * x8 in V.
+ *   append       : key K8 = e4m3_rn_satfinite(k_new / k_scale), value V8 = e4m3_rn_satfinite(v_new / v_scale): IEEE
+ *                  fp32 division, round to nearest-even, saturated to +-448 -- bit-identical to torch's
+ *                  (x.float() / scale).clamp(-448, 448).to(torch.float8_e4m3fn).  With rotary the rotated key is rounded
+ *                  to q's dtype as tfa_attn_kvcache_rotary_fwd() stores it, then quantized.  Lengths, the table,
+ *                  dropped tokens and the capacity clamp are those of the 16-bit calls.
+ *   attention    : every finite e4m3 code widens exactly to bf16 / fp16; the kernel runs the 16-bit call's arithmetic
+ *                  on the widened cache with softmax scale s' = fp32(softmax_scale * k_scale) and the output scaled by
+ *                  v_scale.  So for v_scale a power of two, out and lse are bit-identical to the 16-bit call on
+ *                  k8.to(q dtype) / v8.to(q dtype) with softmax_scale = s', its out multiplied by v_scale; for other
+ *                  v_scale they differ by the rounding of that product.  Slots past K_b may hold any byte, NaN codes
+ *                  0x7f / 0xff included, and do not change the result.
+ * s' must stay a normal fp32 number: when it overflows, or when softmax_scale > 0 and it underflows below FLT_MIN (which
+ * would make the attention uniform), the call returns TFA_EINVAL_SCALE.
+ * Every check runs before any device work, those of the 16-bit call first (TFA_EINVAL_KVQUANT after them).  Launches
+ * and CUDA-graph capture as the 16-bit calls; split-KV as tfa_attn_kvcache_fwd() (the varlen call has none). */
+typedef struct tfa_kv_quant_args {
+  int32_t cache_dtype;      /* TFA_FP8_E4M3 */
+  float k_scale, v_scale;   /* finite, > 0 */
+} tfa_kv_quant_args;
+
+int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary /* NULL: none */,
+                             const tfa_kv_quant_args* quant);
+int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

@@ -19,6 +19,13 @@ catches what a deadlock-only test would miss:
   * a wgmma that reads a buffer holding the wrong (item, tile) -- a release that came too early or a parity slip,
   * every warpgroup consumes every item's K/V tiles exactly once and in order, and finishes every item.
 
+With `fp8` (the FP8-cache modes) a fourth role joins: the converter (producer warps 1-3).  The TMA lane then loads
+each K/V tile into a ring of raw e4m3 tiles (raw_full / raw_empty); the converter waits on the entry's raw_full and
+on its K/V slot's kv_empty, widens the raw tile into the slot (stores spanning a scheduling point), arrives on
+kv_full and releases the raw tile.  The softmax warpgroups are unchanged, but do not zero V tails (the converter
+writes those rows as zeros).  Shadow state adds: a raw tile overwritten by TMA while the converter reads it, and the
+converter storing into a slot a wgmma still reads.
+
 Run:  python scripts/protocol_model.py [trials]      (exit code 0 = no violation found)
 """
 import random
@@ -41,10 +48,16 @@ class Bar:
 
 
 class Sim:
-    def __init__(self, items, nstage, rng, empty=(), vtail=()):
+    def __init__(self, items, nstage, rng, empty=(), vtail=(), fp8=False, nraw=2):
         self.items, self.N, self.rng = items, nstage, rng     # items: KV tiles per work item (0 = skipped)
         self.empty = set(empty)                               # items with 0 tiles whose rows are still written
-        self.vtail = set(vtail)                               # items whose last V tile the consumers zero in place
+        self.fp8, self.R = fp8, nraw                          # FP8 cache: raw ring of nraw tiles + the converter
+        # items whose last V tile the consumers zero in place (FP8: the converter zeroes it, not the consumers)
+        self.vtail = set() if fp8 else set(vtail)
+        self.raw_full = [Bar(f"raw_full{i}", 1) for i in range(nraw)]
+        self.raw_empty = [Bar(f"raw_empty{i}", 1) for i in range(nraw)]   # one arrival per converter warp
+        self.raw_buf = [None] * nraw
+        self.raw_readers = [0] * nraw
         self.q_full = Bar("q_full", 1)
         self.q_empty = Bar("q_empty", 2)                      # one arrival per warpgroup (per warp in the kernel)
         self.kv_full = [Bar(f"kv_full{i}", 1) for i in range(nstage)]
@@ -98,6 +111,19 @@ class Sim:
             self.tma(q_landed)
             for j in range(n):
                 for kv in "KV":
+                    if self.fp8:                              # the raw tile; the converter fills the slot
+                        rs = ent % self.R
+                        yield lambda s=rs, p=((ent // self.R) & 1) ^ 1: self.raw_empty[s].done(p)
+                        assert self.raw_readers[rs] == 0, f"raw tile {rs} overwritten while the converter reads it"
+                        self.raw_buf[rs] = "busy"
+
+                        def raw_landed(rs=rs, tag=(item, j, kv)):
+                            assert self.raw_readers[rs] == 0, "raw tile written under the converter"
+                            self.raw_buf[rs] = tag
+                            self.raw_full[rs].arrive()
+                        self.tma(raw_landed)
+                        ent += 1
+                        continue
                     slot = ent % N
                     yield lambda s=slot, p=((ent // N) & 1) ^ 1: self.kv_empty[s].done(p)
                     assert self.kv_readers[slot] == 0, f"slot {slot} overwritten while a wgmma reads it"
@@ -110,6 +136,32 @@ class Sim:
                         self.kv_buf[slot] = tag
                         self.kv_full[slot].arrive()
                     self.tma(kv_landed)
+                    ent += 1
+
+    def converter(self):
+        """Producer warps 1-3 of the FP8-cache modes: raw ring entry -> K/V ring slot, over the TMA lane's entries."""
+        N, R, ent = self.N, self.R, 0
+        for item, n in enumerate(self.items):
+            if n == 0:
+                continue
+            for j in range(n):
+                for kv in "KV":
+                    slot, rs, tag = ent % N, ent % R, (item, j, kv)
+                    yield lambda s=rs, p=(ent // R) & 1: self.raw_full[s].done(p)
+                    yield lambda s=slot, p=((ent // N) & 1) ^ 1: self.kv_empty[s].done(p)
+                    # widen: read the raw tile, store into the slot; the stores span a scheduling point
+                    assert self.raw_buf[rs] == tag, f"converter: raw tile {rs} holds {self.raw_buf[rs]}, not {tag}"
+                    assert self.kv_readers[slot] == 0, f"converter stores into slot {slot} while a wgmma reads it"
+                    self.raw_readers[rs] += 1
+                    self.kv_writers[slot] += 1
+                    self.kv_buf[slot] = "converting"
+                    yield lambda: True
+                    assert self.kv_readers[slot] == 0, f"slot {slot} read by a wgmma under the converter's stores"
+                    self.kv_buf[slot] = tag
+                    self.kv_writers[slot] -= 1
+                    self.raw_readers[rs] -= 1
+                    self.kv_full[slot].arrive()               # after the last store (and its proxy fence)
+                    self.raw_empty[rs].arrive()
                     ent += 1
 
     def consumer(self, t):
@@ -190,16 +242,17 @@ class Sim:
             self.finished[t].append(item)
 
     def run(self, max_steps=200000):
-        roles = [self.producer(), self.consumer(0), self.consumer(1)]
-        waits = [None, None, None]
-        alive = [True, True, True]
+        roles = [self.producer(), self.consumer(0), self.consumer(1)] + ([self.converter()] if self.fp8 else [])
+        nr = len(roles)
+        waits = [None] * nr
+        alive = [True] * nr
         for _ in range(max_steps):
-            ready = [i for i in range(3) if alive[i] and (waits[i] is None or waits[i]())]
+            ready = [i for i in range(nr) if alive[i] and (waits[i] is None or waits[i]())]
             busy = bool(self.tma_q) or any(self.mma_q)
             if not ready and not busy:
                 if not any(alive):
                     break
-                raise AssertionError("deadlock: " + ", ".join(f"role{i}" for i in range(3) if alive[i]))
+                raise AssertionError("deadlock: " + ", ".join(f"role{i}" for i in range(nr) if alive[i]))
             if ready and (not busy or self.rng.random() < 0.6):
                 i = self.rng.choice(ready)
                 try:
@@ -284,6 +337,14 @@ def random_varlen_cache_items(rng):
     return items, empty, vtail
 
 
+def random_fp8_cache_items(rng, varlen):
+    """Items of an FP8-cache problem (kCacheFp8, or kVarlenCacheFp8 when `varlen`): those of its 16-bit mode -- items
+    skipped by every role, items without tiles whose rows are still written, items whose last tile has rows past the
+    sequence's keys (which the converter writes as zeros) -- and a raw-ring depth."""
+    items, empty, vtail = random_varlen_cache_items(rng) if varlen else random_cache_items(rng)
+    return items, empty, vtail, rng.choice([2, 4])
+
+
 def main():
     trials = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     for trial in range(trials):
@@ -295,6 +356,9 @@ def main():
         Sim(items, rng.choice([4, 8]), rng, empty, vtail).run()
         items, empty, vtail = random_varlen_cache_items(rng)
         Sim(items, rng.choice([4, 8]), rng, empty, vtail).run()
+        for varlen in (False, True):
+            items, empty, vtail, nraw = random_fp8_cache_items(rng, varlen)
+            Sim(items, rng.choice([4, 8]), rng, empty, vtail, fp8=True, nraw=nraw).run()
     print(f"{trials} trials: no violation")
 
 

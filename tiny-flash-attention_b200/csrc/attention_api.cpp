@@ -19,6 +19,7 @@
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -282,14 +283,24 @@ struct CacheShape {
 
 // The arguments both cache entry points share, for a q of B sequences: the caches, cache_seqlens, block_table and the
 // pairing, device and dtype of k_new / v_new.  Each entry point checks the shapes of its q and k_new itself.  Throws
-// on a bad argument, before any device work.
+// on a bad argument, before any device work.  `fp8`: the caches are float8_e4m3fn (the FP8 entry points), else q's
+// dtype.
 CacheShape check_cache(const torch::Tensor& q, int64_t B, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
                        const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
-                       const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new) {
+                       const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
+                       bool fp8 = false) {
   TFA_CHECK_CUDA(k_cache);
   TFA_CHECK_CUDA(v_cache);
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "k_cache, v_cache must have 4 dimensions");
-  check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
+  if (fp8) {
+    TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
+    TORCH_CHECK(k_cache.scalar_type() == at::kFloat8_e4m3fn && v_cache.scalar_type() == at::kFloat8_e4m3fn,
+                "k_cache and v_cache must be float8_e4m3fn for the FP8 cache calls");
+    TORCH_CHECK(k_cache.device() == q.device() && v_cache.device() == q.device(),
+                "q, k_cache, v_cache must be on the same device");
+  } else {
+    check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache");
+  }
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes() && k_cache.strides() == v_cache.strides(),
               "k_cache and v_cache must have identical shapes and strides");
   TORCH_CHECK(q.stride(-1) == 1 && k_cache.stride(3) == 1, "q and the caches must have a unit head_dim stride");
@@ -331,10 +342,10 @@ struct KvcacheCall {
 KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
                           const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
                           const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
-                          int64_t num_splits) {
+                          int64_t num_splits, bool fp8 = false) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 4, "q must have 4 dimensions (B, Sq, Hq, D)");
-  const CacheShape cs = check_cache(q, q.size(0), k_cache, v_cache, cache_seqlens, block_table, k_new, v_new);
+  const CacheShape cs = check_cache(q, q.size(0), k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, fp8);
   KvcacheCall c{q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new};
   c.B = q.size(0); c.Sq = q.size(1); c.Hq = q.size(2); c.D = q.size(3);
   c.nblk = cs.nblk; c.page = cs.page; c.Hkv = cs.Hkv; c.mbps = cs.mbps; c.bts = cs.bts;
@@ -425,16 +436,12 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
   return {out, lse};
 }
 
-// The same with rotary position embedding (flash-attn's rotary_cos / rotary_sin / rotary_interleaved): q and k_new
-// are rotated at their absolute positions (tfa_attn_kvcache_rotary_fwd in include/tfa_b200.h) before the attention;
-// the caller's q and k_new are not modified.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) contiguous in q's
-// dtype on q's device, seqlen_ro >= capacity, rotary_dim a multiple of 16 in [16, D]; k_new / v_new are required.
-std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
-    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
-    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
-    torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved, bool is_causal, float softmax_scale,
-    int64_t num_splits) {
-  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
+namespace {
+
+// The rotary arguments of a cache call (c checked): the tfa_rotary_args but q_rot.  Throws before any device work.
+tfa_rotary_args check_rotary(const KvcacheCall& c, const torch::Tensor& rotary_cos, const torch::Tensor& rotary_sin,
+                             bool rotary_interleaved) {
+  const torch::Tensor& q = c.q;
   TORCH_CHECK(c.snew > 0, "rotary needs k_new and v_new: it rotates the appended keys");
   TORCH_CHECK(rotary_cos.device() == q.device() && rotary_sin.device() == q.device(),
               "rotary_cos and rotary_sin must be on q's device");
@@ -451,19 +458,76 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
   TORCH_CHECK(seqlen_ro >= c.mbps * c.page,
               fmt_msg("rotary_cos / rotary_sin need a row per cache position: seqlen_ro = %lld < capacity = %lld",
                       static_cast<long long>(seqlen_ro), static_cast<long long>(c.mbps * c.page)));
+  tfa_rotary_args r;
+  r.cos = rotary_cos.data_ptr(); r.sin = rotary_sin.data_ptr();
+  r.seqlen_ro = static_cast<int32_t>(seqlen_ro); r.rotary_dim = static_cast<int32_t>(rotary_dim);
+  r.interleaved = rotary_interleaved ? 1 : 0;
+  r.q_rot = nullptr;
+  return r;
+}
+
+// The per-tensor scales of an FP8 cache call; throws before any device work.
+tfa_kv_quant_args check_quant(double k_scale, double v_scale) {
+  TORCH_CHECK(std::isfinite(k_scale) && k_scale > 0 && std::isfinite(v_scale) && v_scale > 0,
+              "k_scale and v_scale must be finite and > 0");
+  tfa_kv_quant_args qa;
+  qa.cache_dtype = TFA_FP8_E4M3;
+  qa.k_scale = static_cast<float>(k_scale);
+  qa.v_scale = static_cast<float>(v_scale);
+  return qa;
+}
+
+}  // namespace
+
+// The same with rotary position embedding (flash-attn's rotary_cos / rotary_sin / rotary_interleaved): q and k_new
+// are rotated at their absolute positions (tfa_attn_kvcache_rotary_fwd in include/tfa_b200.h) before the attention;
+// the caller's q and k_new are not modified.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) contiguous in q's
+// dtype on q's device, seqlen_ro >= capacity, rotary_dim a multiple of 16 in [16, D]; k_new / v_new are required.
+std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
+    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
+    torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved, bool is_causal, float softmax_scale,
+    int64_t num_splits) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
   torch::Tensor out, lse, ws, q_rot;
+  tfa_rotary_args r = check_rotary(c, rotary_cos, rotary_sin, rotary_interleaved);
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
     tfa_attn_kvcache_args a;
     ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
     q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
-    tfa_rotary_args r;
-    r.cos = rotary_cos.data_ptr(); r.sin = rotary_sin.data_ptr();
-    r.seqlen_ro = static_cast<int32_t>(seqlen_ro); r.rotary_dim = static_cast<int32_t>(rotary_dim);
-    r.interleaved = rotary_interleaved ? 1 : 0;
     r.q_rot = q_rot.data_ptr();
     rc = tfa_attn_kvcache_rotary_fwd(&a, &r);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
+// flash_attention_v2_kvcache (and, with rotary_cos / rotary_sin, flash_attention_v2_kvcache_rotary) against an FP8
+// cache: k_cache / v_cache are float8_e4m3fn, an element x8 standing for k_scale * x8 in K and v_scale * x8 in V;
+// k_new / v_new (q's dtype) are quantized into them (tfa_attn_kvcache_fp8_fwd in include/tfa_b200.h).
+std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
+    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
+    double k_scale, double v_scale, bool is_causal, float softmax_scale, int64_t num_splits,
+    std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin, bool rotary_interleaved) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits, true);
+  const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
+  TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
+  tfa_rotary_args r;
+  if (rotary_cos.has_value()) r = check_rotary(c, *rotary_cos, *rotary_sin, rotary_interleaved);
+  torch::Tensor out, lse, ws, q_rot;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    tfa_attn_kvcache_args a;
+    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
+    if (rotary_cos.has_value()) {
+      q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
+      r.q_rot = q_rot.data_ptr();
+    }
+    rc = tfa_attn_kvcache_fp8_fwd(&a, rotary_cos.has_value() ? &r : nullptr, &qa);
   }
   raise_on_error(rc);
   return {out, lse};
@@ -474,10 +538,14 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
 // k_cache / v_cache / block_table / cache_seqlens as flash_attention_v2_kvcache; k_new / v_new None or packed
 // (total_q, Hkv, D) sharing cu_seqlens_q, written into the cache in place at keys [cache_seqlens[b], + the sequence's
 // query rows) before the attention.  Returns out (total_q, Hq, D) and lse (Hq, total_q).  No split-KV.
-std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
-    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
-    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
-    std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale) {
+namespace {
+
+// flash_attention_v2_varlen_kvcache, or with `quant` its FP8-cache form.
+std::vector<torch::Tensor> varlen_kvcache(
+    const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
+    const torch::Tensor& cu_seqlens_q, int64_t max_seqlen_q, const torch::Tensor& cache_seqlens,
+    const std::optional<torch::Tensor>& block_table, const std::optional<torch::Tensor>& k_new,
+    const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
@@ -487,7 +555,7 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
                                                  static_cast<long long>(cu_seqlens_q.numel())));
   const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2);
   const int64_t B = cu_seqlens_q.numel() - 1;
-  const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new);
+  const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, quant != nullptr);
   const int64_t nblk = cs.nblk, page = cs.page, Hkv = cs.Hkv, mbps = cs.mbps, bts = cs.bts;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
@@ -535,10 +603,31 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    rc = tfa_attn_varlen_kvcache_fwd(&a);
+    rc = quant ? tfa_attn_varlen_kvcache_fp8_fwd(&a, quant) : tfa_attn_varlen_kvcache_fwd(&a);
   }
   raise_on_error(rc);
   return {out, lse};
+}
+
+}  // namespace
+
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale) {
+  return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
+                        is_causal, softmax_scale, nullptr);
+}
+
+// The same against an FP8 cache (float8_e4m3fn k_cache / v_cache with per-tensor k_scale / v_scale), as
+// flash_attention_v2_kvcache_fp8.
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_fp8(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, double k_scale, double v_scale, bool is_causal, float softmax_scale) {
+  const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
+  return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
+                        is_causal, softmax_scale, &qa);
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -562,6 +651,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_varlen_kvcache", &flash_attention_v2_varlen_kvcache,
         "a packed variable-length batch of queries against a (paged) KV cache with an optional in-place append: (q, "
         "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, is_causal, scale)");
+  m.def("flash_attention_v2_kvcache_fp8", &flash_attention_v2_kvcache_fp8,
+        "the KV-cache forward against an FP8 (float8_e4m3fn) cache with per-tensor scales, k_new / v_new quantized on "
+        "append, optional rotary",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("block_table"),
+        py::arg("k_new"), py::arg("v_new"), py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"),
+        py::arg("softmax_scale"), py::arg("num_splits"), py::arg("rotary_cos") = py::none(),
+        py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
+  m.def("flash_attention_v2_varlen_kvcache_fp8", &flash_attention_v2_varlen_kvcache_fp8,
+        "a packed variable-length batch of queries against an FP8 (float8_e4m3fn) cache with per-tensor scales: (q, "
+        "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, k_scale, v_scale, "
+        "is_causal, scale)");
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

@@ -2,9 +2,9 @@
 // units: the kernel of the chosen schedule, its shared-memory opt-in, the launch, and the causal x dtype x fp32
 // dispatch.  The caller sizes the grid and counts the launch.
 //
-// tfa_varlen_kvcache.cu explicitly instantiates launch_forward<kVarlenCache>, and tfa_api.cu declares that
-// instantiation `extern template`, so that the mode's 32 kernels are compiled in that unit only (the comment there says
-// why).
+// tfa_varlen_kvcache.cu explicitly instantiates launch_forward<kVarlenCache>, tfa_kvcache_fp8.cu launch_forward<
+// kCacheFp8> and launch_forward<kVarlenCacheFp8>, and tfa_api.cu declares those instantiations `extern template`, so
+// that each mode's 32 kernels are compiled in that unit only (the comment there says why).
 #pragma once
 #include "fa_fwd_sm90.cuh"
 
@@ -20,9 +20,10 @@ cudaError_t launch_forward_inst(const CUtensorMap& tq, const CUtensorMap& tk, co
                       : fa_fwd_sm90_kernel<D, CAUSAL, IS_BF16, OUT_F32, false, MODE>;
   // cudaFuncSetAttribute is per device (context) and costs well under a microsecond: set it on every launch instead of
   // caching "done once" per process, which breaks the first launch on a second GPU of the same process.
-  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdCfg<D>::SMEM_BYTES);
+  constexpr int smem = fwd_smem_bytes<D, MODE>();
+  const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  kern<<<nblocks, FwdCfg<D>::THREADS, FwdCfg<D>::SMEM_BYTES, stream>>>(tq, tk, tv, p);
+  kern<<<nblocks, FwdCfg<D>::THREADS, smem, stream>>>(tq, tk, tv, p);
   return cudaSuccess;
 }
 

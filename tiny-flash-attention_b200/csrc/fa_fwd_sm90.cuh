@@ -34,13 +34,21 @@
 // MODE (the problem the grid solves): kDense = (B, H, S, D) tensors; kVarlen = a packed variable-length batch, each
 // item reads its sequence's offsets and lengths from cu_seqlens; kCache = decode against a (paged) KV cache, each item
 // reads its sequence's cached length from cache_seqlens and its K/V boxes' pages from a block table; kVarlenCache =
-// both at once, a packed variable-length batch of queries (cu_seqlens) against a (paged) KV cache.
+// both at once, a packed variable-length batch of queries (cu_seqlens) against a (paged) KV cache.  kCacheFp8 and
+// kVarlenCacheFp8 are kCache and kVarlenCache against an FP8 (e4m3) cache: the TMA lane loads raw e4m3 tiles into a
+// ring of their own, and producer warps 1-3 (the converter) widen each into the 16-bit K/V ring slot the softmax
+// warpgroups read, exactly, in the layout TMA gives a 16-bit tile; their code does not change.
 #pragma once
 #include "ptx_sm90.cuh"
 
 namespace tfa {
 
-enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3 };
+enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5 };
+// The problem an FP8-cache mode solves is that of its 16-bit mode: they differ only in how K/V reach the ring.
+__host__ __device__ constexpr bool fp8_mode(int mode) { return mode == kCacheFp8 || mode == kVarlenCacheFp8; }
+__host__ __device__ constexpr int base_mode(int mode) {
+  return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode;
+}
 
 // ---- KV-cache address math, host-callable so that a CPU test can check it exhaustively (tests/test_kvcache.py) ----
 // Keys attended by sequence b: its cached length clamped to [0, capacity - snew], plus the snew appended keys.  The
@@ -142,6 +150,9 @@ struct FwdParams {
   const int* block_table;     // nullptr: contiguous cache, page = capacity
   long long bt_stride;
   int page, capacity, snew;
+  // FP8 cache (kCacheFp8 / kVarlenCacheFp8): V element x8 stands for v_scale * x8; the epilogue folds it into 1/l.
+  // (k_scale is folded into scale / scale_log2 by the host.)
+  float v_scale;
 };
 
 template <int D>
@@ -160,8 +171,60 @@ struct FwdCfg {
   static constexpr int THREADS = 384;
 };
 
+// Shared-memory plan of the FP8-cache modes: the same Q and staging tiles, a 16-bit K/V ring of NSTAGE tiles, then a
+// ring of NRAW raw e4m3 tiles (128 keys x D bytes, unswizzled, as TMA loads them), then the barriers: q_full, q_empty,
+// kv_full / kv_empty[NSTAGE], raw_full / raw_empty[NRAW].  The D = 128 depths (4 + 2) come from an A/B of 4 + 2, 3 + 4
+// and 2 + 6 on K1 / K3 of scripts/kvcache_fp8_bench.py (profiles/h100_kvcache_fp8.json; TFA_FP8_RING128 /
+// TFA_FP8_RAW128 build the other pairs).  D = 64 keeps FwdCfg's 8-deep ring plus 4 raw tiles (197,840 B; 8 + 8 would
+// fit too): no D = 64 workload was measured.
+#ifndef TFA_FP8_RING128
+#define TFA_FP8_RING128 4
+#endif
+#ifndef TFA_FP8_RAW128
+#define TFA_FP8_RAW128 2
+#endif
+template <int D>
+struct Fp8Cfg {
+  using C = FwdCfg<D>;
+  static constexpr int NSTAGE = (D == 128) ? TFA_FP8_RING128 : C::NSTAGE;
+  static constexpr int RAW_BYTES = 128 * D;
+  static constexpr int NRAW = (D == 128) ? TFA_FP8_RAW128 : 4;
+  static constexpr int NUM_BARS = 2 + 2 * NSTAGE + 2 * NRAW;
+  static constexpr int SMEM_BYTES =
+      1024 + 2 * C::TILE_BYTES + NSTAGE * C::TILE_BYTES + NRAW * RAW_BYTES + NUM_BARS * 8;
+  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a block may use");
+  static constexpr int CONVERTER_WARPS = 3;   // producer warps 1..3
+};
+template <int D, int MODE>
+__host__ __device__ constexpr int fwd_smem_bytes() { return fp8_mode(MODE) ? Fp8Cfg<D>::SMEM_BYTES : FwdCfg<D>::SMEM_BYTES; }
+
+// 8 e4m3 codes (bytes of r, element 0 in the low byte of r.x) -> 8 16-bit values, exactly: the code's sign and its
+// 7 exponent-mantissa bits placed at the top of the 16-bit type's exponent-mantissa field give x8 * 2^-(bias gap), and
+// one exact multiply by 2^(bias gap) undoes it (subnormal codes included: they land on the 16-bit type's subnormals,
+// which this multiply keeps).  The NaN codes 0x7f / 0xff give a NaN.
+template <bool IS_BF16>
+__device__ __forceinline__ uint4 widen_e4m3x8(uint2 r) {
+  constexpr int SHIFT = IS_BF16 ? 4 : 7;                // 8 exponent bits (bf16) or 5 (fp16) above the mantissa
+  constexpr uint32_t SCALE = IS_BF16 ? 0x7b807b80u : 0x5c005c00u;   // 2^120 (bf16), 2^8 (fp16), two lanes
+  constexpr uint32_t NAN_MUL = IS_BF16 ? 0xffu : 0xf8u;              // 0x80 -> 0x7f80 / 0x7c00: exponent all ones
+  uint32_t out[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t w = i < 2 ? r.x : r.y;
+    // bytes 2(i&1), 2(i&1)+1 of w -> the low bytes of the two 16-bit lanes
+    const uint32_t y = __byte_perm(w, 0u, (i & 1) ? 0x4342u : 0x4140u);
+    const uint32_t em = y & 0x007f007fu, sgn = y & 0x00800080u;
+    uint32_t h = (sgn << 8) | (em << SHIFT), d;
+    if constexpr (IS_BF16) asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(h), "r"(SCALE));
+    else asm("mul.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(h), "r"(SCALE));
+    const uint32_t nan = ((em + 0x00010001u) & 0x00800080u) * NAN_MUL;   // lanes whose code is 0x7f / 0xff
+    out[i] = d | nan;
+  }
+  return make_uint4(out[0], out[1], out[2], out[3]);
+}
+
 // watchdog call sites
-enum : uint32_t { SITE_LOAD_EMPTY = 1, SITE_LOAD_Q = 2, SITE_MMA_Q = 3, SITE_MMA_K = 4, SITE_MMA_V = 5 };
+enum : uint32_t { SITE_LOAD_EMPTY = 1, SITE_LOAD_Q = 2, SITE_MMA_Q = 3, SITE_MMA_K = 4, SITE_MMA_V = 5, SITE_CONV_RAW = 6 };
 
 constexpr float kRescaleThresholdLog2 = 8.0f;  // lazy rescale: tolerate P up to 2^8
 // Register re-allocation after the prologue.  setmaxnreg moves registers inside the CTA's OWN pool, which is
@@ -170,6 +233,11 @@ constexpr float kRescaleThresholdLog2 = 8.0f;  // lazy rescale: tolerate P up to
 constexpr uint32_t kRegsSoftmax = 240;
 constexpr uint32_t kRegsProducer = 24;
 static_assert((2 * kRegsSoftmax + kRegsProducer) * 128 <= 384 * 168, "setmaxnreg budget exceeds the CTA register pool");
+// The FP8-cache modes: the producer warpgroup widens every K/V tile, so it keeps more (2 x 232 + 40 = 504).
+constexpr uint32_t kRegsSoftmaxFp8 = 232;
+constexpr uint32_t kRegsProducerFp8 = 40;
+static_assert((2 * kRegsSoftmaxFp8 + kRegsProducerFp8) * 128 <= 384 * 168,
+              "setmaxnreg budget exceeds the CTA register pool");
 
 // work item -> (batch*head, split, Q-tile pair).  CTAs are handed to SMs in blockIdx order (and the persistent kernel
 // walks the same order), so this order IS the schedule.  Heads are taken in chunks of `head_chunk` (8) and INSIDE a
@@ -202,8 +270,9 @@ struct Item {
 };
 template <bool CAUSAL, int MODE>
 __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
-  constexpr bool VARLEN = MODE == kVarlen;
-  constexpr bool QPACK = MODE == kVarlen || MODE == kVarlenCache;    // packed queries: items past a sequence skipped
+  constexpr int M = base_mode(MODE);
+  constexpr bool VARLEN = M == kVarlen;
+  constexpr bool QPACK = M == kVarlen || M == kVarlenCache;          // packed queries: items past a sequence skipped
   Item w;
   int pr;
   decode_work(item, p.npairs, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
@@ -223,13 +292,13 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.Sq = max(q1 - q0, 0);
     w.Sk = max(k1 - k0, 0);
     w.coff = w.Sk - w.Sq;           // may be negative: the sequence's first rows see no key
-  } else if constexpr (MODE == kCache) {
+  } else if constexpr (M == kCache) {
     w.q0 = 0;
     w.k0 = 0;
     w.Sq = p.S;
     w.Sk = cache_len(__ldg(p.cache_seqlens + w.bidx), p.capacity, p.snew) + p.snew;
     w.coff = w.Sk - w.Sq;           // may be negative, as for varlen
-  } else if constexpr (MODE == kVarlenCache) {
+  } else if constexpr (M == kVarlenCache) {
     // queries as varlen, but only the first S = max_seqlen_q rows: the grid covers no more, and the keys appended
     // for the sequence are those rows' own
     const int q0 = min(max(__ldg(p.cu_q + w.bidx), 0), p.total_q);
@@ -250,12 +319,12 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   const int nkv_total = (w.Sk + 127) >> 7;
   // causal: the item's last row sees keys <= last (none when last < 0, which only varlen and cache sequences can have)
   const int last = w.row0 + 127 + w.coff;
-  const int nfull = CAUSAL ? ((MODE != kDense && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
+  const int nfull = CAUSAL ? ((M != kDense && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
   w.n = max(0, min(nfull - w.jb, p.split_tiles));   // 0: a split-KV item wholly above the causal diagonal
   // dense: an item without tiles writes nothing (its rows belong to other splits); varlen: an item inside its sequence
   // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0); cache: every item writes its rows,
   // a split without tiles too (LSE = -inf), so the combine can read every split's partial
-  w.live = QPACK ? w.row0 < w.Sq : (MODE == kCache || w.n > 0);
+  w.live = QPACK ? w.row0 < w.Sq : (M == kCache || w.n > 0);
   if (QPACK && !w.live) w.n = 0;     // past the sequence's end: the producer must skip it as the consumers do
   return w;
 }
@@ -264,11 +333,14 @@ template <int D, bool CAUSAL, bool IS_BF16, bool OUT_F32, bool PERSIST, int MODE
 __global__ void __launch_bounds__(384, 1)
 fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const FwdParams p) {
-  constexpr bool QPACK = MODE == kVarlen || MODE == kVarlenCache;   // q / out / lse packed as varlen
-  constexpr bool PAGED = MODE == kCache || MODE == kVarlenCache;    // K/V from a (paged) cache
+  constexpr int M = base_mode(MODE);
+  constexpr bool FP8 = fp8_mode(MODE);                          // K/V from an e4m3 cache, widened by the converter
+  constexpr bool QPACK = M == kVarlen || M == kVarlenCache;     // q / out / lse packed as varlen
+  constexpr bool PAGED = M == kCache || M == kVarlenCache;      // K/V from a (paged) cache
   using C = FwdCfg<D>;
+  using F = Fp8Cfg<D>;
   constexpr int TILE = C::TILE_BYTES;
-  constexpr int NSTAGE = C::NSTAGE;
+  constexpr int NSTAGE = FP8 ? F::NSTAGE : C::NSTAGE;          // 16-bit K/V ring depth
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operands need 1024-byte alignment (the swizzle is a function of address bits 7..9)
@@ -276,11 +348,15 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint8_t* sQ = smem;                       // the item's two Q tiles: rows [0,64) tile 0, [64,128) tile 1
   uint8_t* sStg = smem + TILE;              // epilogue staging, 128 rows x D 16-bit
   uint8_t* sKV = smem + 2 * TILE;           // NSTAGE tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + NSTAGE * TILE);
+  // FP8: the raw e4m3 ring sits between the K/V ring and the barriers, its barriers after the others
+  uint8_t* sRaw = sKV + NSTAGE * TILE;      // [NRAW] tiles of 128 keys x D bytes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + NSTAGE * TILE + (FP8 ? F::NRAW * F::RAW_BYTES : 0));
   uint64_t* q_full = bars;
   uint64_t* q_empty = bars + 1;
   uint64_t* kv_full = bars + 2;             // [NSTAGE]
   uint64_t* kv_empty = kv_full + NSTAGE;    // [NSTAGE]
+  uint64_t* raw_full = kv_empty + NSTAGE;   // [NRAW] (FP8 only)
+  uint64_t* raw_empty = raw_full + F::NRAW; // [NRAW]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -295,8 +371,14 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     mbar_init(q_full, 1);
     mbar_init(q_empty, 8);             // one arrival per softmax warp
     for (int i = 0; i < NSTAGE; ++i) {
-      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_full[i], FP8 ? F::CONVERTER_WARPS : 1);   // FP8: one arrival per converter warp
       mbar_init(&kv_empty[i], 8);
+    }
+    if constexpr (FP8) {
+      for (int i = 0; i < F::NRAW; ++i) {
+        mbar_init(&raw_full[i], 1);
+        mbar_init(&raw_empty[i], F::CONVERTER_WARPS);
+      }
     }
     fence_mbar_init();
   }
@@ -304,7 +386,54 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   if (warp < 4) {
     // =========================== TMA producer ===========================
-    setmaxnreg_dec<kRegsProducer>();
+    setmaxnreg_dec<FP8 ? kRegsProducerFp8 : kRegsProducer>();
+    if constexpr (FP8) {
+      if (warp > 0) {
+        // ---- the converter (warps 1..3): raw ring entry -> 16-bit K/V ring slot, walking the TMA lane's entries ----
+        uint32_t ent = 0;
+        const int ct = threadIdx.x - 32;                          // 0 .. 95
+        for (int item = first; item < p.total_items; item += stride) {
+          const Item w = decode_item<CAUSAL, MODE>(item, p);
+          if (w.n == 0) continue;
+          for (int j = 0; j < w.n; ++j) {
+            // rows at or past the sequence's keys become zeros: a slot past K_b may hold any byte, NaN codes included,
+            // and P = 0 does not cancel 0 * NaN in the PV product (the 16-bit modes' zero_v_tail)
+            const int valid = w.Sk - (w.jb + j) * C::BN;
+#pragma unroll 1
+            for (int kv = 0; kv < 2; ++kv, ++ent) {
+              const uint32_t slot = ent % NSTAGE, rslot = ent % F::NRAW;
+              mbar_wait(&raw_full[rslot], (ent / F::NRAW) & 1, p.dbg, SITE_CONV_RAW, ent);
+              mbar_wait(&kv_empty[slot], ((ent / NSTAGE) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, ent);
+              // 32-bit shared-memory addresses: this warpgroup runs on kRegsProducerFp8 registers
+              const uint32_t raw = smem_u32(sRaw) + rslot * F::RAW_BYTES;
+              const uint32_t dst = smem_u32(sKV) + slot * TILE;
+              constexpr int CPR = D / 8;                          // 16-byte output chunks per key row
+#pragma unroll 2
+              for (int idx = ct; idx < C::BN * CPR; idx += 32 * F::CONVERTER_WARPS) {
+                const int r = idx / CPR, c = idx % CPR;           // key row, chunk of 8 elements
+                uint4 v = make_uint4(0u, 0u, 0u, 0u);
+                if (r < valid) {
+                  uint2 x;
+                  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(x.x), "=r"(x.y) : "r"(raw + idx * 8));
+                  v = widen_e4m3x8<IS_BF16>(x);
+                }
+                // SWIZZLE_128B, as TMA lays out a 16-bit tile: 64-column slabs, chunk c of row r at (c ^ r) & 7
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};"
+                             ::"r"(dst + (c / 8) * C::SLAB_BYTES + r * 128 + (((c & 7) ^ (r & 7)) * 16)),
+                               "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+              }
+              fence_proxy_async_smem();                           // generic-proxy stores -> the wgmma's operand reads
+              __syncwarp();
+              if (lane == 0) {
+                mbar_arrive(&kv_full[slot]);
+                mbar_arrive(&raw_empty[rslot]);
+              }
+            }
+          }
+        }
+        return;
+      }
+    }
     if (warp == 0 && lane == 0) {
       uint32_t ent = 0;      // running K/V ring entry (K_j and V_j of every item in turn; never reset between items)
       uint32_t qcnt = 0;     // items loaded
@@ -326,13 +455,21 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           if constexpr (PAGED) page_lookup(p.block_table, p.bt_stride, w.bidx, ky, p.page, kw, ky);
 #pragma unroll
           for (int kv = 0; kv < 2; ++kv, ++ent) {
-            const uint32_t slot = ent % NSTAGE;
-            mbar_wait(&kv_empty[slot], ((ent / NSTAGE) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, ent);
-            mbar_arrive_expect_tx(&kv_full[slot], TILE);
             const CUtensorMap* tm = kv ? &tmV : &tmK;
+            if constexpr (FP8) {
+              // one unswizzled box of 128 keys x D bytes into the raw ring; the converter fills the K/V slot
+              const uint32_t rslot = ent % F::NRAW;
+              mbar_wait(&raw_empty[rslot], ((ent / F::NRAW) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, ent);
+              mbar_arrive_expect_tx(&raw_full[rslot], F::RAW_BYTES);
+              tma_load_4d(sRaw + rslot * F::RAW_BYTES, tm, &raw_full[rslot], 0, ky, w.hkv, kw);
+            } else {
+              const uint32_t slot = ent % NSTAGE;
+              mbar_wait(&kv_empty[slot], ((ent / NSTAGE) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, ent);
+              mbar_arrive_expect_tx(&kv_full[slot], TILE);
 #pragma unroll
-            for (int sl = 0; sl < C::SLABS; ++sl)
-              tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64, ky, w.hkv, kw);
+              for (int sl = 0; sl < C::SLABS; ++sl)
+                tma_load_4d(sKV + slot * TILE + sl * C::SLAB_BYTES, tm, &kv_full[slot], sl * 64, ky, w.hkv, kw);
+            }
           }
         }
       }
@@ -341,7 +478,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
 
   // ================= softmax / wgmma / epilogue warpgroup t =================
-  setmaxnreg_inc<kRegsSoftmax>();
+  setmaxnreg_inc<FP8 ? kRegsSoftmaxFp8 : kRegsSoftmax>();
   using MmaS = Wgmma<128, IS_BF16>;
   using MmaO = Wgmma<D, IS_BF16>;
   const int t = (warp >> 2) - 1;                 // Q tile
@@ -388,8 +525,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     // [Sk, tile end) in shared memory (whole 128-byte swizzle rows of each slab, so the swizzle does not matter).  Both
     // warpgroups write the same zeros; the slot is released only after both have read it.  Between the kv_full wait
     // and the release, so the producer cannot refill the slot under the stores (scripts/protocol_model.py).
+    // FP8: the converter wrote those rows as zeros already.
     auto zero_v_tail = [&](uint32_t vslot, int jt) {
-      if constexpr (PAGED) {
+      if constexpr (PAGED && !FP8) {
         const int valid = Sk - (w.jb + jt) * C::BN;          // warpgroup-uniform
         if (valid < C::BN) {
           uint8_t* vt = sKV + vslot * TILE;
@@ -482,7 +620,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
     // A varlen or cache item whose rows all see no key has no tiles: it waits on no barrier, its rows get O = 0 and
     // LSE = +inf (-inf for a split-KV partial).
-    if (MODE == kDense || n > 0) {
+    if (M == kDense || n > 0) {
       mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
       ++qcnt;
       // ---- KV tile 0 ----
@@ -548,8 +686,12 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       l_lo += __shfl_xor_sync(0xffffffffu, l_lo, d);
       l_hi += __shfl_xor_sync(0xffffffffu, l_hi, d);
     }
-    const float inv_lo = (l_lo > 0.f) ? 1.0f / l_lo : 0.f;
-    const float inv_hi = (l_hi > 0.f) ? 1.0f / l_hi : 0.f;
+    float inv_lo = (l_lo > 0.f) ? 1.0f / l_lo : 0.f;
+    float inv_hi = (l_hi > 0.f) ? 1.0f / l_hi : 0.f;
+    if constexpr (FP8) {          // V = v_scale * V8: O = (P V8 / l) * v_scale; a split's partial too (the combine is linear)
+      inv_lo *= p.v_scale;
+      inv_hi *= p.v_scale;
+    }
     const long long tile_off =
         (QPACK ? static_cast<long long>(w.q0) * p.o_stride_s : static_cast<long long>(w.bidx) * p.o_stride_b) +
         static_cast<long long>(w.hidx) * p.o_stride_h;
@@ -560,7 +702,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         float* lrow = p.lse + static_cast<long long>(w.hidx) * p.lse_stride_bh + w.q0;
         if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : INFINITY;
         if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : INFINITY;
-      } else if constexpr (MODE == kCache) {
+      } else if constexpr (M == kCache) {
         // (B, H, S) as dense; a row that saw no key gets +inf, or -inf in a split-KV partial (as above)
         const float none = p.nsplit > 1 ? -INFINITY : INFINITY;
         float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;

@@ -1,7 +1,7 @@
 // fa_splitkv_combine.cuh -- the small HBM-bound kernels either side of the attention forward when the problem
 // is not the reference's square one (SURVEY.md 8f rows 2-3), plus the KV-cache append of both cache calls
-// (kvcache_append_kernel, below) and its rotary variant (kvcache_rotary_append_kernel), both launched from
-// tfa_append.cu:
+// (kvcache_append_kernel, below), its rotary variant (kvcache_rotary_append_kernel) and their quantizing variants for
+// an FP8 cache (kvcache_append_fp8_kernel, kvcache_rotary_append_fp8_kernel), all launched from tfa_append.cu:
 //
 //   * splitkv_combine_kernel: merges the per-split partial results of the split-KV forward,
 //       O = sum_s exp(lse_s - LSE) * O_s ,  LSE = log sum_s exp(lse_s)
@@ -273,6 +273,44 @@ struct RotaryAppendParams {
   long long q_chunks;             // B * Sq * Hq * D / 8
 };
 
+// The two halves of kvcache_rotary_append_kernel (below) as functions, for its FP8 variant.  The 16-bit kernel keeps
+// its own copy of the body: built from these functions, its interleaved instantiations compile to different SASS (8
+// more instructions at D = 128), and its generated code is kept as it was.
+// Chunk c < q_chunks of the rotary append: rot(q) into q_rot.
+template <int D, bool IS_BF16, bool INTERLEAVED>
+__device__ __forceinline__ void rotary_q_chunk(const RotaryAppendParams& p, long long c) {
+  constexpr int CPR = D / 8;                   // 16-byte chunks per row
+  const AppendParams& a = p.ap;
+  const uint16_t* cos_tab = static_cast<const uint16_t*>(p.cos);
+  const uint16_t* sin_tab = static_cast<const uint16_t*>(p.sin);
+  const int sub = static_cast<int>(c % CPR);
+  long long r = c / CPR;                       // row index over (B, Sq, Hq), Hq fastest
+  const int h = static_cast<int>(r % p.Hq);
+  r /= p.Hq;
+  const int i = static_cast<int>(r % p.Sq);
+  const int b = static_cast<int>(r / p.Sq);
+  const int len = cache_len(__ldg(a.cache_seqlens + b), a.capacity, a.snew);
+  const long long ro =
+      static_cast<long long>(rotary_pos(len, i, p.causal != 0, true, p.seqlen_ro)) * (p.rotary_dim / 2);
+  const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + i * p.q_ss + h * p.q_sh;
+  const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_tab + ro, sin_tab + ro, p.rotary_dim);
+  reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + ((static_cast<long long>(b) * p.Sq + i) * p.Hq + h) * D)
+      [sub] = y;
+}
+// The key half: rot(k_new) and v_new of appended chunk k (k.dst >= 0), as 16-bit chunks.
+template <bool IS_BF16, bool INTERLEAVED>
+__device__ __forceinline__ void rotary_kv_chunk(const RotaryAppendParams& p, const AppendChunk& k, uint4& kx,
+                                                uint4& vx) {
+  const AppendParams& a = p.ap;
+  const int len = cache_len(__ldg(a.cache_seqlens + k.b), a.capacity, a.snew);
+  const long long ro =
+      static_cast<long long>(rotary_pos(len, k.i, p.causal != 0, false, p.seqlen_ro)) * (p.rotary_dim / 2);
+  kx = rotate_chunk<IS_BF16, INTERLEAVED>(static_cast<const uint16_t*>(a.k_new) + k.src, k.sub,
+                                          static_cast<const uint16_t*>(p.cos) + ro,
+                                          static_cast<const uint16_t*>(p.sin) + ro, p.rotary_dim);
+  vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + k.src) + k.sub);
+}
+
 template <int D, bool IS_BF16, bool INTERLEAVED>
 __global__ void __launch_bounds__(256) kvcache_rotary_append_kernel(const RotaryAppendParams p) {
   constexpr int CPR = D / 8;                   // 16-byte chunks per row
@@ -307,6 +345,69 @@ __global__ void __launch_bounds__(256) kvcache_rotary_append_kernel(const Rotary
   const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + k.src) + k.sub);
   *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.k_cache) + k.dst + k.sub * 8) = kx;
   *reinterpret_cast<uint4*>(static_cast<uint16_t*>(a.v_cache) + k.dst + k.sub * 8) = vx;
+}
+
+// ---- FP8 (e4m3) cache: the appends quantize what they would have stored ----
+// A stored key is K8 = e4m3_rn_satfinite(k / k_scale), a value V8 = e4m3_rn_satfinite(v / v_scale): an IEEE fp32
+// division (div.rn, not the fast-math approximation the build would otherwise emit), rounded to nearest-even and
+// saturated to +-448 -- bit-identical to torch's (x.float() / scale).clamp(-448, 448).to(torch.float8_e4m3fn).  With
+// rotary the key is rotated and rounded to q's dtype first, as the 16-bit rotary append stores it.
+struct KvQuant {
+  float k_scale, v_scale;
+};
+__device__ __forceinline__ float div_rn(float a, float b) {
+  float d;
+  asm("div.rn.f32 %0, %1, %2;" : "=f"(d) : "f"(a), "f"(b));
+  return d;
+}
+// 8 16-bit values -> 8 e4m3 codes, element 0 in the low byte
+template <bool IS_BF16>
+__device__ __forceinline__ uint2 quantize_chunk(const uint4& x, float scale) {
+  uint32_t w[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    unsigned short lo, hi;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;"
+        : "=h"(lo)
+        : "f"(div_rn(widen16<IS_BF16>(x, 4 * i + 1), scale)), "f"(div_rn(widen16<IS_BF16>(x, 4 * i), scale)));
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;"
+        : "=h"(hi)
+        : "f"(div_rn(widen16<IS_BF16>(x, 4 * i + 3), scale)), "f"(div_rn(widen16<IS_BF16>(x, 4 * i + 2), scale)));
+    w[i] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+  }
+  return make_uint2(w[0], w[1]);
+}
+
+// kvcache_append_kernel into an e4m3 cache: 16 bytes of k_new / v_new in, 8 bytes of codes out per thread.
+template <int D, bool IS_BF16>
+__global__ void __launch_bounds__(256) kvcache_append_fp8_kernel(const AppendParams p, const KvQuant qs) {
+  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (c >= p.chunks) return;
+  const AppendChunk a = append_chunk<D>(p, c);
+  if (a.dst < 0) return;
+  const long long src = a.src + a.sub * 8;
+  const uint4 kx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.k_new) + src));
+  const uint4 vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.v_new) + src));
+  *reinterpret_cast<uint2*>(static_cast<uint8_t*>(p.k_cache) + a.dst + a.sub * 8) = quantize_chunk<IS_BF16>(kx, qs.k_scale);
+  *reinterpret_cast<uint2*>(static_cast<uint8_t*>(p.v_cache) + a.dst + a.sub * 8) = quantize_chunk<IS_BF16>(vx, qs.v_scale);
+}
+
+// kvcache_rotary_append_kernel into an e4m3 cache: rot(q) to q_rot as there, rot(k_new) and v_new quantized.
+template <int D, bool IS_BF16, bool INTERLEAVED>
+__global__ void __launch_bounds__(256) kvcache_rotary_append_fp8_kernel(const RotaryAppendParams p, const KvQuant qs) {
+  const long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  const AppendParams& a = p.ap;
+  if (c < p.q_chunks) {
+    rotary_q_chunk<D, IS_BF16, INTERLEAVED>(p, c);
+    return;
+  }
+  if (c - p.q_chunks >= a.chunks) return;
+  const AppendChunk k = append_chunk<D>(a, c - p.q_chunks);
+  if (k.dst < 0) return;
+  uint4 kx, vx;
+  rotary_kv_chunk<IS_BF16, INTERLEAVED>(p, k, kx, vx);
+  *reinterpret_cast<uint2*>(static_cast<uint8_t*>(a.k_cache) + k.dst + k.sub * 8) = quantize_chunk<IS_BF16>(kx, qs.k_scale);
+  *reinterpret_cast<uint2*>(static_cast<uint8_t*>(a.v_cache) + k.dst + k.sub * 8) = quantize_chunk<IS_BF16>(vx, qs.v_scale);
 }
 
 }  // namespace tfa

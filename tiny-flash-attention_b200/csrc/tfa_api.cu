@@ -18,6 +18,8 @@
 #include <mutex>
 #include <type_traits>
 #include <vector>
+#include <cfloat>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 
@@ -25,11 +27,24 @@
 int tfa_internal_launch_append(const tfa::AppendParams& p, int D, cudaStream_t stream);
 int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
                                       cudaStream_t stream);
+int tfa_internal_launch_append_fp8(const tfa::AppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
+                                   cudaStream_t stream);
+int tfa_internal_launch_rotary_append_fp8(const tfa::RotaryAppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
+                                          bool interleaved, cudaStream_t stream);
 // tfa_varlen_kvcache.cu: the variable-length cache forward, compiled apart from the other forward kernels
 extern template cudaError_t tfa::launch_forward<tfa::kVarlenCache>(int D, bool causal, bool bf16, bool f32,
                                                                    const CUtensorMap& tq, const CUtensorMap& tk,
                                                                    const CUtensorMap& tv, const tfa::FwdParams& p,
                                                                    int nblocks, bool persist, cudaStream_t stream);
+// tfa_kvcache_fp8.cu: the FP8-cache forwards, compiled apart from the other forward kernels
+extern template cudaError_t tfa::launch_forward<tfa::kCacheFp8>(int D, bool causal, bool bf16, bool f32,
+                                                                const CUtensorMap& tq, const CUtensorMap& tk,
+                                                                const CUtensorMap& tv, const tfa::FwdParams& p,
+                                                                int nblocks, bool persist, cudaStream_t stream);
+extern template cudaError_t tfa::launch_forward<tfa::kVarlenCacheFp8>(int D, bool causal, bool bf16, bool f32,
+                                                                      const CUtensorMap& tq, const CUtensorMap& tk,
+                                                                      const CUtensorMap& tv, const tfa::FwdParams& p,
+                                                                      int nblocks, bool persist, cudaStream_t stream);
 
 namespace {
 
@@ -72,25 +87,30 @@ void init_dbg() {
 
 // (B?,H?,S,D)-strided 16-bit tensor -> 4-D tiled map with dims (D, S, H, B); the kernel addresses it as
 // (x = head-dim offset, y = sequence row, z = head, w = batch).  Box = 64 x 128 elements, SWIZZLE_128B.
+// dtype TFA_FP8_E4M3: a 1-byte (e4m3) cache, box = D x 128 bytes, unswizzled (the converter reads it row by row).
 int make_tmap(CUtensorMap* m, const void* base, int dtype, int D, int S, int B, int H, long long sb,
               long long sh, long long ss) {
-  constexpr int box_rows = 128, box_cols = 64;
+  const bool fp8 = dtype == TFA_FP8_E4M3;
+  const int box_rows = 128, box_cols = fp8 ? D : 64;
+  const cuuint64_t esz = fp8 ? 1 : 2;
   auto encode = get_encode_fn();
   if (!encode) return TFA_EDRIVER;
-  const CUtensorMapDataType dt = (dtype == TFA_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                     : (dtype == TFA_BF16) ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                           : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const cuuint32_t box[4] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows), 1, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   const cuuint64_t dims[4] = {static_cast<cuuint64_t>(D), static_cast<cuuint64_t>(S), static_cast<cuuint64_t>(H),
                               static_cast<cuuint64_t>(B)};
   // size-1 dims may carry any stride; give them a legal one
-  const cuuint64_t s1 = static_cast<cuuint64_t>(ss) * 2;
-  const cuuint64_t s2 = (H > 1 ? static_cast<cuuint64_t>(sh) : static_cast<cuuint64_t>(ss) * S) * 2;
-  const cuuint64_t s3 = (B > 1 ? static_cast<cuuint64_t>(sb) : s2 / 2 * H) * 2;
+  const cuuint64_t s1 = static_cast<cuuint64_t>(ss) * esz;
+  const cuuint64_t s2 = (H > 1 ? static_cast<cuuint64_t>(sh) : static_cast<cuuint64_t>(ss) * S) * esz;
+  const cuuint64_t s3 = (B > 1 ? static_cast<cuuint64_t>(sb) : s2 / esz * H) * esz;
   const cuuint64_t strides[3] = {s1, s2, s3};
   for (int i = 0; i < 3; ++i)
     if ((strides[i] % 16) || strides[i] >= (1ull << 40)) return TFA_EINVAL_STRIDE;
   CUresult r = encode(m, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : TFA_EDRIVER;
 }
@@ -167,7 +187,7 @@ long long fwd_grid(long long nitems, int variant) {
 }
 
 // One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache /
-// kVarlenCache).
+// kVarlenCache / kCacheFp8 / kVarlenCacheFp8).
 template <int MODE>
 int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
@@ -349,7 +369,8 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   p.S = S;
   p.nsplit = plan.nsplit;
   p.split_tiles = plan.split_tiles;
-  set_output(p, a, S, plan.nsplit, MODE == tfa::kVarlen || MODE == tfa::kVarlenCache);
+  constexpr int M = tfa::base_mode(MODE);
+  set_output(p, a, S, plan.nsplit, M == tfa::kVarlen || M == tfa::kVarlenCache);
 
   const int variant = choose_kernel(causal, npairs, p.n_extra_dst);
   int rc = launch_fwd<MODE>(a.D, causal, bf16, f32 || plan.nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * plan.nsplit,
@@ -531,12 +552,13 @@ int validate_cache(const Args& ka) {
 // The cache side of a cache call whose arguments passed (a = its Problem, capacity = a.Sk): the K/V tensor maps over
 // the pages, the append of `n` rows per sequence (ap.chunks = 0 without k_new; the caller sets its k_new layout fields
 // n_sb / cu_q / total_q) and the cache fields of the forward but snew.
+// `cache_dtype`: a.dtype, or TFA_FP8_E4M3 for an FP8 cache.
 template <typename Args>
 int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtensorMap& tv, tfa::AppendParams& ap,
-                FwdParams& p) {
+                FwdParams& p, int cache_dtype) {
   const int page = ka.block_table ? ka.page_block_size : a.Sk;
-  if (int rc = make_tmap(&tk, a.k, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
-  if (int rc = make_tmap(&tv, a.v, a.dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
+  if (int rc = make_tmap(&tk, a.k, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
+  if (int rc = make_tmap(&tv, a.v, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
   ap = tfa::AppendParams{};
   ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
   ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
@@ -564,14 +586,36 @@ int validate_rotary(const tfa_attn_kvcache_args& ka, const Problem& a, const tfa
   return 0;
 }
 
+// The FP8-cache arguments of a cache call whose other arguments passed: the element type, the scales, and cache
+// strides that keep every 1-byte TMA row and box 16-byte aligned.  Sets a.scale to the effective softmax scale
+// s' = fp32(softmax_scale * k_scale), and `qs` to the scales.  s' must stay a normal fp32 number (or 0 with
+// softmax_scale = 0): an overflow, or an underflow that would silently turn the call into uniform attention, is
+// TFA_EINVAL_SCALE.
+int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
+  if (q.cache_dtype != TFA_FP8_E4M3) return TFA_EINVAL_KVQUANT;
+  if (!(q.k_scale > 0.0f) || !std::isfinite(q.k_scale) || !(q.v_scale > 0.0f) || !std::isfinite(q.v_scale))
+    return TFA_EINVAL_KVQUANT;
+  if ((a.ksb % 16) || (a.ksh % 16) || (a.kss % 16)) return TFA_EINVAL_KVQUANT;
+  const float s = a.scale * q.k_scale;
+  if (!(s <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
+  a.scale = s;
+  qs.k_scale = q.k_scale;
+  qs.v_scale = q.v_scale;
+  return 0;
+}
+
 // `ra` nullptr: the plain cache forward.  Otherwise q and k_new are rotated first (kvcache_rotary_append_kernel, in
-// place of the plain append) and the forward reads its queries from ra->q_rot.
-int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
+// place of the plain append) and the forward reads its queries from ra->q_rot.  `quant` nullptr: a 16-bit cache;
+// otherwise an FP8 one, appended to by the quantizing appends and read by the kCacheFp8 forward.
+int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant) {
   Problem a = from_kvcache_args(ka);
   int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if (ra && (rc = validate_rotary(ka, a, *ra))) return rc;
+  tfa::KvQuant qs{1.0f, 1.0f};
+  if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
   const int snew = ka.k_new ? ka.Snew : 0;
@@ -598,19 +642,27 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra) {
   tfa::AppendParams ap;
   FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(ka, a, snew, tk, tv, ap, p))) return rc;
+  if ((rc = setup_cache(ka, a, snew, tk, tv, ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
   ap.n_sb = ka.new_stride_b;
 
+  const bool bf16 = a.dtype == TFA_BF16;
   if (ra) {
     rp.ap = ap;
-    rc = tfa_internal_launch_rotary_append(rp, a.D, a.dtype == TFA_BF16, ra->interleaved != 0, a.stream);
+    rc = quant ? tfa_internal_launch_rotary_append_fp8(rp, qs, a.D, bf16, ra->interleaved != 0, a.stream)
+               : tfa_internal_launch_rotary_append(rp, a.D, bf16, ra->interleaved != 0, a.stream);
     if (rc) return rc;
   } else if (snew > 0) {
-    if ((rc = tfa_internal_launch_append(ap, a.D, a.stream))) return rc;
+    rc = quant ? tfa_internal_launch_append_fp8(ap, qs, a.D, bf16, a.stream)
+               : tfa_internal_launch_append(ap, a.D, a.stream);
+    if (rc) return rc;
   }
 
   p.snew = snew;
   // every split writes its rows (LSE = -inf where it saw no key): the combine reads all of them
+  if (quant) {
+    p.v_scale = qs.v_scale;
+    return run_forward<tfa::kCacheFp8>(a, p, a.Sq, tq, tk, tv, plan, false);
+  }
   return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan, false);
 }
 
@@ -631,13 +683,16 @@ Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
   return q;
 }
 
-int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va) {
-  const Problem a = from_varlen_kvcache_args(va);
+// `quant` as kvcache_impl.
+int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_kv_quant_args* quant) {
+  Problem a = from_varlen_kvcache_args(va);
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
   if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
+  tfa::KvQuant qs{1.0f, 1.0f};
+  if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
 
@@ -645,17 +700,23 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va) {
   tfa::AppendParams ap;
   FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, ap, p))) return rc;
+  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
   if (va.k_new) {
     ap.cu_q = va.cu_seqlens_q;
     ap.total_q = a.Sq;
-    if ((rc = tfa_internal_launch_append(ap, a.D, a.stream))) return rc;
+    rc = quant ? tfa_internal_launch_append_fp8(ap, qs, a.D, a.dtype == TFA_BF16, a.stream)
+               : tfa_internal_launch_append(ap, a.D, a.stream);
+    if (rc) return rc;
   }
 
   p.cu_q = va.cu_seqlens_q;
   p.total_q = a.Sq;
   p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
   // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
+  if (quant) {
+    p.v_scale = qs.v_scale;
+    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
+  }
   return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
 }
 
@@ -702,17 +763,28 @@ int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
 
 int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, nullptr);
+  return kvcache_impl(*args, nullptr, nullptr);
 }
 
 int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary) {
   if (!args || !rotary) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, rotary);
+  return kvcache_impl(*args, rotary, nullptr);
 }
 
 int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args);
+  return varlen_kvcache_impl(*args, nullptr);
+}
+
+int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary,
+                             const tfa_kv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return kvcache_impl(*args, rotary, quant);
+}
+
+int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args, quant);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -910,6 +982,9 @@ const char* tfa_error_string(int code) {
     case TFA_EINVAL_ROTARY:
       return "tfa: rotary needs non-null 16-byte aligned cos, sin and q_rot, rotary_dim a multiple of 16 in [16, D], "
              "seqlen_ro >= capacity, and k_new";
+    case TFA_EINVAL_KVQUANT:
+      return "tfa: an FP8 cache needs cache_dtype TFA_FP8_E4M3 (2), finite k_scale and v_scale > 0, and cache strides "
+             "that are multiples of 16 elements";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "tfa: unknown error";
   }
 }

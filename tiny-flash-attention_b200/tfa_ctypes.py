@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("TFA_LIB", os.path.join(HERE, "libtfa_b200.so"))   # TFA_LIB: tuning variants only
 
 TFA_BF16, TFA_FP16 = 0, 1
+TFA_FP8_E4M3 = 2
 _LIB = None
 _WORKSPACES = {}     # (device, stream) -> last split-KV workspace, see _split_workspace()
 
@@ -100,6 +101,11 @@ class VarlenKvcacheArgs(ctypes.Structure):
     ]
 
 
+class KvQuantArgs(ctypes.Structure):
+    """struct tfa_kv_quant_args (include/tfa_b200.h)."""
+    _fields_ = [("cache_dtype", ctypes.c_int32), ("k_scale", ctypes.c_float), ("v_scale", ctypes.c_float)]
+
+
 class RotaryArgs(ctypes.Structure):
     """struct tfa_rotary_args (include/tfa_b200.h)."""
     _fields_ = [
@@ -137,6 +143,11 @@ def lib():
         L.tfa_attn_kvcache_rotary_fwd.restype = ci
         L.tfa_attn_varlen_kvcache_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs)]
         L.tfa_attn_varlen_kvcache_fwd.restype = ci
+        L.tfa_attn_kvcache_fp8_fwd.argtypes = [ctypes.POINTER(KvcacheArgs), ctypes.POINTER(RotaryArgs),
+                                               ctypes.POINTER(KvQuantArgs)]
+        L.tfa_attn_kvcache_fp8_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_fp8_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(KvQuantArgs)]
+        L.tfa_attn_varlen_kvcache_fp8_fwd.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -276,9 +287,19 @@ def _cache_args(block_table, k_new, v_new, new_dims):
     return bt, k_new.data_ptr(), v_new.data_ptr(), k_new.stride()[:new_dims]
 
 
+def _quant(k_cache, k_scale, v_scale):
+    """The tfa_kv_quant_args of an FP8 (torch.float8_e4m3fn) cache, or None for a 16-bit one, which takes no scales."""
+    import torch
+    if k_cache.dtype != torch.float8_e4m3fn:
+        if k_scale != 1.0 or v_scale != 1.0:
+            raise ValueError(f"k_scale / v_scale apply to a float8_e4m3fn cache only; this cache is {k_cache.dtype}")
+        return None
+    return KvQuantArgs(TFA_FP8_E4M3, float(k_scale), float(v_scale))
+
+
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
                      scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
-                     rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None):
+                     rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None, k_scale=1.0, v_scale=1.0):
     """Attention against a KV cache through tfa_attn_kvcache_fwd(): q (B, Sq, Hq, D) with unit head_dim stride;
     k_cache / v_cache (num_blocks, page, Hkv, D) with a block_table (B, max_blocks_per_seq) int32, or (B, capacity,
     Hkv, D) with block_table None; cache_seqlens (B,) int32; optional k_new / v_new (B, Snew, Hkv, D) appended in
@@ -286,6 +307,7 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and k_new first, through
     tfa_attn_kvcache_rotary_fwd().  The rotated queries go to `q_rot`, a contiguous (B, Sq, Hq, D) tensor of q's dtype
     that holds them after the call, or to a buffer allocated here.
+    torch.float8_e4m3fn caches go through tfa_attn_kvcache_fp8_fwd() with the per-tensor k_scale / v_scale.
     Returns out (q's shape and strides) and lse (B, Hq, Sq)."""
     import torch
     assert q.is_cuda and q.dim() == 4 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -293,6 +315,7 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     assert cache_seqlens.dtype == torch.int32
     B, Sq, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
+    quant = _quant(k_cache, k_scale, v_scale)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 3)
     snew = k_new.shape[1] if k_new is not None else 0
     if scale is None:
@@ -311,9 +334,8 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
     n = _split_workspace(dense, a, q.device, st)
-    if rotary_cos is None:
-        check(lib().tfa_attn_kvcache_fwd(ctypes.byref(a)))
-    else:
+    r = None
+    if rotary_cos is not None:
         assert rotary_sin is not None and rotary_cos.dim() == 2 and rotary_cos.shape == rotary_sin.shape
         assert rotary_cos.is_contiguous() and rotary_sin.is_contiguous()
         if q_rot is None:
@@ -322,6 +344,12 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
         assert q_rot.shape == q.shape and q_rot.dtype == q.dtype and q_rot.is_contiguous()
         r = RotaryArgs(rotary_cos.data_ptr(), rotary_sin.data_ptr(), rotary_cos.shape[0], 2 * rotary_cos.shape[1],
                        int(bool(rotary_interleaved)), q_rot.data_ptr())
+    if quant is not None:
+        check(lib().tfa_attn_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
+                                             ctypes.byref(quant)))
+    elif r is None:
+        check(lib().tfa_attn_kvcache_fwd(ctypes.byref(a)))
+    else:
         check(lib().tfa_attn_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r)))
     if return_splits:
         return out, lse, n
@@ -329,11 +357,13 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
 
 
 def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
-                            v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None):
+                            v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None,
+                            k_scale=1.0, v_scale=1.0):
     """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
     (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
     and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
-    sharing cu_q, appended in place.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given
+    sharing cu_q, appended in place.  torch.float8_e4m3fn caches go through tfa_attn_varlen_kvcache_fp8_fwd() with
+    the per-tensor k_scale / v_scale.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given
     to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -341,6 +371,7 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
     assert cu_q.dtype == torch.int32 and cu_q.numel() >= 2 and cache_seqlens.dtype == torch.int32
     total_q, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
+    quant = _quant(k_cache, k_scale, v_scale)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 2)
     if scale is None:
         scale = D ** -0.5
@@ -354,7 +385,10 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
                           D, total_q, int(max_seqlen_q), nblk, page, mbps, q.stride(0), q.stride(1),
                           k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1], _dtype_code(q),
                           int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
-    check(lib().tfa_attn_varlen_kvcache_fwd(ctypes.byref(a)))
+    if quant is not None:
+        check(lib().tfa_attn_varlen_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(quant)))
+    else:
+        check(lib().tfa_attn_varlen_kvcache_fwd(ctypes.byref(a)))
     return out, lse
 
 
