@@ -366,49 +366,64 @@ KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, 
   return c;
 }
 
-// Under q's device guard: allocates out (q's strides; a non-dense q is replaced by its contiguous copy first) and lse,
-// fills `a`, and allocates the split-KV workspace (returned; the caller keeps it until the launch is enqueued).
-torch::Tensor fill_kvcache(KvcacheCall& c, bool is_causal, float softmax_scale, int64_t num_splits,
-                           tfa_attn_kvcache_args& a, torch::Tensor& out, torch::Tensor& lse) {
-  out = torch::empty_like(c.q);
-  if (out.strides() != c.q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
-    c.q = c.q.contiguous();
+// The dense-query cache call once every argument passed: allocates out (q's strides; a non-dense q is replaced by its
+// contiguous copy first), lse, the split-KV workspace and, with rotary (`r`), q_rot, and runs the call.  `quant`
+// nullptr: a 16-bit cache.
+std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float softmax_scale, int64_t num_splits,
+                                       tfa_rotary_args* r, const tfa_kv_quant_args* quant) {
+  torch::Tensor out, lse, ws, q_rot;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(c.q.device());
     out = torch::empty_like(c.q);
+    if (out.strides() != c.q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
+      c.q = c.q.contiguous();
+      out = torch::empty_like(c.q);
+    }
+    lse = torch::empty({c.B, c.Hq, c.Sq}, c.q.options().dtype(at::kFloat));
+    tfa_attn_kvcache_args a;
+    std::memset(&a, 0, sizeof(a));
+    a.q = c.q.data_ptr(); a.k_cache = c.k_cache.data_ptr(); a.v_cache = c.v_cache.data_ptr();
+    a.k_new = c.snew ? c.k_new->data_ptr() : nullptr;
+    a.v_new = c.snew ? c.v_new->data_ptr() : nullptr;
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.cache_seqlens = c.cache_seqlens.data_ptr<int32_t>();
+    a.block_table = c.block_table.has_value() ? c.block_table->data_ptr<int32_t>() : nullptr;
+    a.B = static_cast<int32_t>(c.B); a.Hq = static_cast<int32_t>(c.Hq); a.Hkv = static_cast<int32_t>(c.Hkv);
+    a.Sq = static_cast<int32_t>(c.Sq); a.D = static_cast<int32_t>(c.D);
+    a.num_blocks = static_cast<int32_t>(c.nblk); a.page_block_size = static_cast<int32_t>(c.page);
+    a.max_blocks_per_seq = static_cast<int32_t>(c.mbps); a.Snew = static_cast<int32_t>(c.snew);
+    a.q_stride_b = c.q.stride(0); a.q_stride_s = c.q.stride(1); a.q_stride_h = c.q.stride(2);
+    a.cache_stride_block = c.k_cache.stride(0); a.cache_stride_s = c.k_cache.stride(1);
+    a.cache_stride_h = c.k_cache.stride(2);
+    a.block_table_stride = c.bts;
+    if (c.snew) {
+      a.new_stride_b = c.k_new->stride(0); a.new_stride_s = c.k_new->stride(1); a.new_stride_h = c.k_new->stride(2);
+    }
+    a.dtype = c.q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.num_splits = static_cast<int32_t>(num_splits);
+    a.stream = at::cuda::getCurrentCUDAStream(c.q.device().index()).stream();
+    // split count and workspace: those of the dense problem with Sk = capacity
+    tfa_attn_args d;
+    std::memset(&d, 0, sizeof(d));
+    d.B = a.B; d.Hq = a.Hq; d.Hkv = a.Hkv; d.Sq = a.Sq; d.D = a.D;
+    d.Sk = static_cast<int32_t>(std::min<int64_t>(c.mbps * c.page, 0x7fffffff));
+    d.is_causal = a.is_causal;
+    d.num_splits = a.num_splits;
+    ws = split_workspace(d, c.q);
+    a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
+    if (r) {
+      q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
+      r->q_rot = q_rot.data_ptr();
+    }
+    rc = quant ? tfa_attn_kvcache_fp8_fwd(&a, r, quant)
+         : r   ? tfa_attn_kvcache_rotary_fwd(&a, r)
+               : tfa_attn_kvcache_fwd(&a);
   }
-  lse = torch::empty({c.B, c.Hq, c.Sq}, c.q.options().dtype(at::kFloat));
-  std::memset(&a, 0, sizeof(a));
-  a.q = c.q.data_ptr(); a.k_cache = c.k_cache.data_ptr(); a.v_cache = c.v_cache.data_ptr();
-  a.k_new = c.snew ? c.k_new->data_ptr() : nullptr;
-  a.v_new = c.snew ? c.v_new->data_ptr() : nullptr;
-  a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
-  a.cache_seqlens = c.cache_seqlens.data_ptr<int32_t>();
-  a.block_table = c.block_table.has_value() ? c.block_table->data_ptr<int32_t>() : nullptr;
-  a.B = static_cast<int32_t>(c.B); a.Hq = static_cast<int32_t>(c.Hq); a.Hkv = static_cast<int32_t>(c.Hkv);
-  a.Sq = static_cast<int32_t>(c.Sq); a.D = static_cast<int32_t>(c.D);
-  a.num_blocks = static_cast<int32_t>(c.nblk); a.page_block_size = static_cast<int32_t>(c.page);
-  a.max_blocks_per_seq = static_cast<int32_t>(c.mbps); a.Snew = static_cast<int32_t>(c.snew);
-  a.q_stride_b = c.q.stride(0); a.q_stride_s = c.q.stride(1); a.q_stride_h = c.q.stride(2);
-  a.cache_stride_block = c.k_cache.stride(0); a.cache_stride_s = c.k_cache.stride(1);
-  a.cache_stride_h = c.k_cache.stride(2);
-  a.block_table_stride = c.bts;
-  if (c.snew) {
-    a.new_stride_b = c.k_new->stride(0); a.new_stride_s = c.k_new->stride(1); a.new_stride_h = c.k_new->stride(2);
-  }
-  a.dtype = c.q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
-  a.is_causal = is_causal ? 1 : 0;
-  a.softmax_scale = softmax_scale;
-  a.num_splits = static_cast<int32_t>(num_splits);
-  a.stream = at::cuda::getCurrentCUDAStream(c.q.device().index()).stream();
-  // split count and workspace: those of the dense problem with Sk = capacity
-  tfa_attn_args d;
-  std::memset(&d, 0, sizeof(d));
-  d.B = a.B; d.Hq = a.Hq; d.Hkv = a.Hkv; d.Sq = a.Sq; d.D = a.D;
-  d.Sk = static_cast<int32_t>(std::min<int64_t>(c.mbps * c.page, 0x7fffffff));
-  d.is_causal = a.is_causal;
-  d.num_splits = a.num_splits;
-  torch::Tensor ws = split_workspace(d, c.q);
-  a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
-  return ws;
+  raise_on_error(rc);
+  return {out, lse};
 }
 
 }  // namespace
@@ -424,16 +439,7 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
                                                       std::optional<torch::Tensor> v_new, bool is_causal,
                                                       float softmax_scale, int64_t num_splits) {
   KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
-  torch::Tensor out, lse, ws;
-  int rc = 0;
-  {
-    c10::cuda::CUDAGuard guard(q.device());
-    tfa_attn_kvcache_args a;
-    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
-    rc = tfa_attn_kvcache_fwd(&a);
-  }
-  raise_on_error(rc);
-  return {out, lse};
+  return kvcache_fwd(c, is_causal, softmax_scale, num_splits, nullptr, nullptr);
 }
 
 namespace {
@@ -489,19 +495,8 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
     torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved, bool is_causal, float softmax_scale,
     int64_t num_splits) {
   KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
-  torch::Tensor out, lse, ws, q_rot;
   tfa_rotary_args r = check_rotary(c, rotary_cos, rotary_sin, rotary_interleaved);
-  int rc = 0;
-  {
-    c10::cuda::CUDAGuard guard(q.device());
-    tfa_attn_kvcache_args a;
-    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
-    q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
-    r.q_rot = q_rot.data_ptr();
-    rc = tfa_attn_kvcache_rotary_fwd(&a, &r);
-  }
-  raise_on_error(rc);
-  return {out, lse};
+  return kvcache_fwd(c, is_causal, softmax_scale, num_splits, &r, nullptr);
 }
 
 // flash_attention_v2_kvcache (and, with rotary_cos / rotary_sin, flash_attention_v2_kvcache_rotary) against an FP8
@@ -517,20 +512,7 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
   TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
   tfa_rotary_args r;
   if (rotary_cos.has_value()) r = check_rotary(c, *rotary_cos, *rotary_sin, rotary_interleaved);
-  torch::Tensor out, lse, ws, q_rot;
-  int rc = 0;
-  {
-    c10::cuda::CUDAGuard guard(q.device());
-    tfa_attn_kvcache_args a;
-    ws = fill_kvcache(c, is_causal, softmax_scale, num_splits, a, out, lse);
-    if (rotary_cos.has_value()) {
-      q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
-      r.q_rot = q_rot.data_ptr();
-    }
-    rc = tfa_attn_kvcache_fp8_fwd(&a, rotary_cos.has_value() ? &r : nullptr, &qa);
-  }
-  raise_on_error(rc);
-  return {out, lse};
+  return kvcache_fwd(c, is_causal, softmax_scale, num_splits, rotary_cos.has_value() ? &r : nullptr, &qa);
 }
 
 // A packed variable-length batch of queries against a (paged) KV cache (flash-attn's flash_attn_varlen_func with

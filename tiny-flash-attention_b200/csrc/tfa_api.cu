@@ -9,6 +9,7 @@
 // caller's stream is honoured, nothing synchronises the device, nothing calls exit().
 #include "../../include/tfa_b200.h"
 #include "fa_fwd_launch.cuh"
+#include "fa_kvcache_append.cuh"
 #include "fa_splitkv_combine.cuh"
 
 #include <cuda_runtime.h>
@@ -23,14 +24,9 @@
 #include <cstdlib>
 #include <cstring>
 
-// tfa_append.cu: the appends' launches, compiled apart from the forward kernels
-int tfa_internal_launch_append(const tfa::AppendParams& p, int D, cudaStream_t stream);
-int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
-                                      cudaStream_t stream);
-int tfa_internal_launch_append_fp8(const tfa::AppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
-                                   cudaStream_t stream);
-int tfa_internal_launch_rotary_append_fp8(const tfa::RotaryAppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
-                                          bool interleaved, cudaStream_t stream);
+// tfa_append.cu: the append's launch, compiled apart from the forward kernels
+int tfa_internal_launch_append(const tfa::AppendKernelParams& p, const tfa::KvQuant* qs, int D, bool bf16, bool rotary,
+                               bool interleaved, cudaStream_t stream);
 // tfa_varlen_kvcache.cu: the variable-length cache forward, compiled apart from the other forward kernels
 extern template cudaError_t tfa::launch_forward<tfa::kVarlenCache>(int D, bool causal, bool bf16, bool f32,
                                                                    const CUtensorMap& tq, const CUtensorMap& tk,
@@ -605,9 +601,9 @@ int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
   return 0;
 }
 
-// `ra` nullptr: the plain cache forward.  Otherwise q and k_new are rotated first (kvcache_rotary_append_kernel, in
-// place of the plain append) and the forward reads its queries from ra->q_rot.  `quant` nullptr: a 16-bit cache;
-// otherwise an FP8 one, appended to by the quantizing appends and read by the kCacheFp8 forward.
+// `ra` nullptr: the plain cache forward.  Otherwise the append also rotates q and k_new, and the forward reads its
+// queries from ra->q_rot.  `quant` nullptr: a 16-bit cache; otherwise an FP8 one, into which the append quantizes and
+// which the kCacheFp8 forward reads.
 int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant) {
   Problem a = from_kvcache_args(ka);
   int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
@@ -623,7 +619,7 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
   SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
   if ((rc = plan_splits(a, plan))) return rc;
 
-  tfa::RotaryAppendParams rp;
+  tfa::AppendKernelParams rp{};
   if (ra) {
     rp.q = a.q; rp.q_rot = ra->q_rot;
     rp.q_sb = a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
@@ -639,21 +635,13 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
   }
 
   CUtensorMap tq, tk, tv;
-  tfa::AppendParams ap;
   FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(ka, a, snew, tk, tv, ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
-  ap.n_sb = ka.new_stride_b;
-
-  const bool bf16 = a.dtype == TFA_BF16;
-  if (ra) {
-    rp.ap = ap;
-    rc = quant ? tfa_internal_launch_rotary_append_fp8(rp, qs, a.D, bf16, ra->interleaved != 0, a.stream)
-               : tfa_internal_launch_rotary_append(rp, a.D, bf16, ra->interleaved != 0, a.stream);
-    if (rc) return rc;
-  } else if (snew > 0) {
-    rc = quant ? tfa_internal_launch_append_fp8(ap, qs, a.D, bf16, a.stream)
-               : tfa_internal_launch_append(ap, a.D, a.stream);
+  if ((rc = setup_cache(ka, a, snew, tk, tv, rp.ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
+  rp.ap.n_sb = ka.new_stride_b;
+  if (snew > 0) {                       // rotary needs k_new (validate_rotary): every rotary call appends
+    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
+                                    ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
 
@@ -697,15 +685,14 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_kv_qua
   init_dbg();
 
   CUtensorMap tq, tk, tv;
-  tfa::AppendParams ap;
+  tfa::AppendKernelParams rp{};         // no rotary: only rp.ap is used
   FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
+  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
   if (va.k_new) {
-    ap.cu_q = va.cu_seqlens_q;
-    ap.total_q = a.Sq;
-    rc = quant ? tfa_internal_launch_append_fp8(ap, qs, a.D, a.dtype == TFA_BF16, a.stream)
-               : tfa_internal_launch_append(ap, a.D, a.stream);
+    rp.ap.cu_q = va.cu_seqlens_q;
+    rp.ap.total_q = a.Sq;
+    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, false, false, a.stream);
     if (rc) return rc;
   }
 
@@ -945,7 +932,7 @@ long long tfa_internal_varlen_append_offset(int raw, const int* block_table, lon
                                             long long cs_s, long long cs_h) {
   return tfa::append_offset(raw, block_table, bt_stride, b, i, h, page, capacity, n, num_blocks, cs_b, cs_s, cs_h);
 }
-// development aid (not in the public header): the rotary position rule of fa_splitkv_combine.cuh on the host
+// development aid (not in the public header): the rotary position rule of fa_kvcache_append.cuh on the host
 int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {
   return tfa::rotary_pos(cache_len, i, causal != 0, is_query != 0, seqlen_ro);
 }

@@ -1,11 +1,11 @@
-// tfa_append.cu -- instantiates and launches the KV-cache appends (kvcache_append_kernel,
-// kvcache_rotary_append_kernel and their FP8-cache variants, fa_splitkv_combine.cuh) for tfa_api.cu.
+// tfa_append.cu -- instantiates and launches the KV-cache append (kvcache_append_kernel, fa_kvcache_append.cuh) for
+// tfa_api.cu.
 //
 // A translation unit of its own: the device compiler optimises a translation unit as one module, and instantiating
-// the rotary kernels next to the forward changed the generated code of the KV-cache forward instantiations (same
+// the rotary appends next to the forward changed the generated code of the KV-cache forward instantiations (same
 // semantics, different SASS).  Kept apart, the forward's code is exactly what it was without the appends.
 #include "../../include/tfa_b200.h"
-#include "fa_splitkv_combine.cuh"
+#include "fa_kvcache_append.cuh"
 
 #include <cuda_runtime.h>
 
@@ -13,8 +13,12 @@ extern "C" void tfa_internal_count_launch(void);
 
 namespace {
 
-// One launch over `chunks` 16-byte chunks, 256 per block, with the kernel's arguments `args` (the FP8 appends take
-// their scales as a second one); counted like every other launch.
+using tfa::AppendKernelParams;
+using tfa::KvQuant;
+using tfa::kvcache_append_kernel;
+
+// One launch over `chunks` 16-byte chunks, 256 per block, with the kernel's arguments `args`; counted like every other
+// launch.
 template <typename... P>
 int launch(void (*kern)(P...), long long chunks, cudaStream_t stream, const P&... args) {
   const long long blocks = (chunks + 255) / 256;
@@ -24,50 +28,39 @@ int launch(void (*kern)(P...), long long chunks, cudaStream_t stream, const P&..
   return static_cast<int>(cudaGetLastError());
 }
 
-template <int D, bool IS_BF16>
-int launch_rotary_fp8(const tfa::RotaryAppendParams& p, const tfa::KvQuant& qs, bool interleaved, cudaStream_t stream) {
-  return launch(interleaved ? tfa::kvcache_rotary_append_fp8_kernel<D, IS_BF16, true>
-                            : tfa::kvcache_rotary_append_fp8_kernel<D, IS_BF16, false>,
-                p.q_chunks + p.ap.chunks, stream, p, qs);
+// The dtype and cache-type dispatch of one head dimension and rotary layout.  The 16-bit append without rotary copies
+// bits, so one instantiation serves both dtypes.
+template <int D, bool ROTARY, bool INTERLEAVED>
+int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool bf16, cudaStream_t stream) {
+  const long long chunks = p.q_chunks + p.ap.chunks;
+  if (qs)
+    return launch(bf16 ? kvcache_append_kernel<D, true, ROTARY, INTERLEAVED, true>
+                       : kvcache_append_kernel<D, false, ROTARY, INTERLEAVED, true>,
+                  chunks, stream, p, *qs);
+  if constexpr (!ROTARY)
+    return launch(kvcache_append_kernel<D, false, false, false, false>, chunks, stream, p, KvQuant{});
+  else
+    return launch(bf16 ? kvcache_append_kernel<D, true, true, INTERLEAVED, false>
+                       : kvcache_append_kernel<D, false, true, INTERLEAVED, false>,
+                  chunks, stream, p, KvQuant{});
 }
 
-template <int D, bool IS_BF16>
-int launch_rotary(const tfa::RotaryAppendParams& p, bool interleaved, cudaStream_t stream) {
-  return launch(interleaved ? tfa::kvcache_rotary_append_kernel<D, IS_BF16, true>
-                            : tfa::kvcache_rotary_append_kernel<D, IS_BF16, false>,
-                p.q_chunks + p.ap.chunks, stream, p);
+template <int D>
+int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool bf16, bool rotary, bool interleaved,
+                  cudaStream_t stream) {
+  if (!rotary) return launch_append<D, false, false>(p, qs, bf16, stream);
+  return interleaved ? launch_append<D, true, true>(p, qs, bf16, stream)
+                     : launch_append<D, true, false>(p, qs, bf16, stream);
 }
 
 }  // namespace
 
-// The append of either cache call, over p.chunks chunks.  Returns 0, a cudaError_t, or TFA_EINVAL_SHAPE when the grid
-// does not fit.
-int tfa_internal_launch_append(const tfa::AppendParams& p, int D, cudaStream_t stream) {
-  return launch(D == 64 ? tfa::kvcache_append_kernel<64> : tfa::kvcache_append_kernel<128>, p.chunks, stream, p);
-}
-
-// The rotary append, over q_chunks + ap.chunks chunks; returns as tfa_internal_launch_append.
-int tfa_internal_launch_rotary_append(const tfa::RotaryAppendParams& p, int D, bool bf16, bool interleaved,
-                                      cudaStream_t stream) {
-  if (D == 64) return bf16 ? launch_rotary<64, true>(p, interleaved, stream)
-                            : launch_rotary<64, false>(p, interleaved, stream);
-  return bf16 ? launch_rotary<128, true>(p, interleaved, stream) : launch_rotary<128, false>(p, interleaved, stream);
-}
-
-// The quantizing appends of an FP8 (e4m3) cache: as the two above, with k_new / v_new (and rot(k_new)) divided by their
-// scales and rounded to e4m3.
-int tfa_internal_launch_append_fp8(const tfa::AppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
-                                   cudaStream_t stream) {
-  if (D == 64) return launch(bf16 ? tfa::kvcache_append_fp8_kernel<64, true> : tfa::kvcache_append_fp8_kernel<64, false>,
-                             p.chunks, stream, p, qs);
-  return launch(bf16 ? tfa::kvcache_append_fp8_kernel<128, true> : tfa::kvcache_append_fp8_kernel<128, false>,
-                p.chunks, stream, p, qs);
-}
-
-int tfa_internal_launch_rotary_append_fp8(const tfa::RotaryAppendParams& p, const tfa::KvQuant& qs, int D, bool bf16,
-                                          bool interleaved, cudaStream_t stream) {
-  if (D == 64) return bf16 ? launch_rotary_fp8<64, true>(p, qs, interleaved, stream)
-                            : launch_rotary_fp8<64, false>(p, qs, interleaved, stream);
-  return bf16 ? launch_rotary_fp8<128, true>(p, qs, interleaved, stream)
-              : launch_rotary_fp8<128, false>(p, qs, interleaved, stream);
+// The append of either cache call, over p.q_chunks + p.ap.chunks chunks.  `qs` nullptr: a 16-bit cache; otherwise an
+// FP8 (e4m3) one, into which k_new / v_new (rot(k_new) with rotary) are quantized with its scales.  `rotary`: q and
+// k_new are rotated, with (2j, 2j+1) pairs when `interleaved`.  Returns 0, a cudaError_t, or TFA_EINVAL_SHAPE when the
+// grid does not fit.
+int tfa_internal_launch_append(const AppendKernelParams& p, const KvQuant* qs, int D, bool bf16, bool rotary,
+                               bool interleaved, cudaStream_t stream) {
+  return D == 64 ? launch_append<64>(p, qs, bf16, rotary, interleaved, stream)
+                 : launch_append<128>(p, qs, bf16, rotary, interleaved, stream);
 }
