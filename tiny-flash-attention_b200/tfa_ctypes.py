@@ -226,15 +226,21 @@ def _split_workspace(dense, args, device, stream):
     return n
 
 
-def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, stream=None, return_splits=False):
+def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, stream=None, return_splits=False,
+             out=None, lse=None):
     """Generalised problem through tfa_attn_fwd(): q (B,Hq,Sq,D), k/v (B,Hkv,Sk,D) contiguous device tensors,
-    bottom-right causal mask, optional split-KV (num_splits: 1 none, n > 1 as asked, 0 library heuristic)."""
+    bottom-right causal mask, optional split-KV (num_splits: 1 none, n > 1 as asked, 0 library heuristic).  `out`
+    (contiguous, q's shape) / `lse` (contiguous (B, Hq, Sq) fp32) may be given to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.is_contiguous() and k.is_contiguous() and v.is_contiguous()
     B, Hq, Sq, D = q.shape
     _, Hkv, Sk, _ = k.shape
-    out = torch.empty(q.shape, dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=q.device)
+    if out is None:
+        out = torch.empty(q.shape, dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+    if lse is None:
+        lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=q.device)
+    assert out.shape == q.shape and out.is_contiguous() and out.dtype == (torch.float32 if out_fp32 else q.dtype)
+    assert lse.shape == (B, Hq, Sq) and lse.is_contiguous() and lse.dtype == torch.float32
     st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
     a = AttnArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), B, Hq, Hkv, Sq, Sk, D,
                  Hq * Sq * D, Sq * D, D, Hkv * Sk * D, Sk * D, D, _dtype_code(q), int(bool(is_causal)),
