@@ -7,11 +7,11 @@ release points) and yield at every mbarrier wait.  A random scheduler interleave
 delays, and each warpgroup's wgmma groups complete in order after random delays (wgmma.wait_group N returns once at most
 N groups are still in flight).  One CTA walks a list of work items, as the persistent schedule does; a list of one item
 is the one-CTA-per-item schedule.  An item with no KV tiles is skipped by the producer; the softmax warpgroups skip it
-too, except for a variable-length item whose rows see no key (`empty`), for which they write O = 0 and LSE = +inf
-without waiting on any barrier.  For a KV-cache item (`vtail`) both warpgroups also WRITE into the ring: they zero
-the V rows past the sequence's keys in the slot of its last tile before PV reads it.  The stores take time (they span
-a scheduling point), and are legal only between that slot's kv_full and the warpgroup's release.  Shadow state
-catches what a deadlock-only test would miss:
+too, except for a live one (`empty`: every dense and cache item, and a variable-length item inside its sequence), for
+which they write O = 0 and LSE = +inf (-inf for a split-KV partial) without waiting on any barrier.  For a KV-cache
+item (`vtail`) both warpgroups also WRITE into the ring: they zero the V rows past the sequence's keys in the slot of
+its last tile before PV reads it.  The stores take time (they span a scheduling point), and are legal only between
+that slot's kv_full and the warpgroup's release.  Shadow state catches what a deadlock-only test would miss:
 
   * a Q buffer or ring slot overwritten by TMA while an issued, unfinished wgmma still reads it, or while a warpgroup
     still stores into it,
@@ -48,9 +48,11 @@ class Bar:
 
 
 class Sim:
-    def __init__(self, items, nstage, rng, empty=(), vtail=(), fp8=False, nraw=2):
-        self.items, self.N, self.rng = items, nstage, rng     # items: KV tiles per work item (0 = skipped)
-        self.empty = set(empty)                               # items with 0 tiles whose rows are still written
+    def __init__(self, items, nstage, rng, empty=None, vtail=(), fp8=False, nraw=2):
+        self.items, self.N, self.rng = items, nstage, rng     # items: KV tiles per work item (0 = none)
+        # items with 0 tiles whose rows are still written; None: all of them (the dense and cache rule), a list: those
+        # of a packed batch that lie inside their sequence (the others are skipped by every role)
+        self.empty = {i for i, n in enumerate(items) if n == 0} if empty is None else set(empty)
         self.fp8, self.R = fp8, nraw                          # FP8 cache: raw ring of nraw tiles + the converter
         # items whose last V tile the consumers zero in place (FP8: the converter zeroes it, not the consumers)
         self.vtail = set() if fp8 else set(vtail)
@@ -272,13 +274,15 @@ class Sim:
 
 
 def random_items(rng):
+    """Tiles per item of a dense problem.  Items without tiles (causal rows above the first key when Sq > Sk, or a split
+    past a Q tile's causal diagonal) are live: Sim's default writes their rows."""
     kind = rng.choice(["one", "causal", "noncausal", "split"])
     if kind == "one":
         return [rng.randint(1, 8)]
     items = []
     for _ in range(rng.randint(1, 9)):
         if kind == "causal":
-            items.append(rng.randint(1, 6))
+            items.append(rng.randint(0, 6))
         elif kind == "noncausal":
             items.append(4)
         else:

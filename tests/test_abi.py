@@ -192,3 +192,7 @@ def test_kernel_selection_rule_on_the_host(built):
     assert pick(4, 32, 4096, 64, True) == CLASSIC           # D=64 causal
     assert pick(32, 32, 512, 64, True) == PERSIST           # ... except short items
     assert pick(1, 32, 16384, 128, True, n_extra=1) == PERSIST   # the fused exchange keeps the persistent schedule
+    # causal Sq > Sk: chosen for the Sk rows that see a key
+    assert pick(4, 32, 8192, 128, True, Sk=128) == PERSIST
+    assert pick(4, 32, 8192, 128, True, Sk=4096) == CLASSIC
+    assert pick(4, 32, 8192, 128, False, Sk=128) == PERSIST

@@ -369,9 +369,8 @@ def _run_dense(tfa, w, kw):
     torch.cuda.synchronize()
     assert_guarded(ob, out)
     assert_guarded(lb, lse)
-    rows = min(Sq, Sk) if causal else Sq                      # causal Sq > Sk: the fill kernel writes the rest
     seqs = [(q[b:b + 1], k[b:b + 1], v[b:b + 1], out[b:b + 1], lse[b:b + 1]) for b in range(B)]
-    return dict(out=out, lse=lse, q_rot=None, variant=variant, items=-(-rows // 128) * B * Hq * n, seqs=seqs)
+    return dict(out=out, lse=lse, q_rot=None, variant=variant, items=-(-Sq // 128) * B * Hq * n, seqs=seqs)
 
 
 def _run_varlen(tfa, w, kw):

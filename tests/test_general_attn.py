@@ -169,6 +169,36 @@ def test_split_kv_matches_oracle_and_single_pass(tfa, B, Hq, Hkv, Sq, Sk, D, cau
     assert np.all(np.abs(o16.float().cpu().numpy() - one.float().cpu().numpy()) <= 2e-3 + 1.01 * ulp)
 
 
+@pytest.mark.parametrize("B,Hq,Hkv,Sq,Sk,D,kind,ns", [
+    (1, 4, 2, 1024, 1024, 128, "bf16", 4),      # the first Q tiles' rows see keys of split 0 only
+    (1, 2, 1, 700, 400, 64, "fp16", 2),         # and the first 300 rows see no key at all
+])
+def test_split_kv_result_does_not_depend_on_the_workspace(tfa, B, Hq, Hkv, Sq, Sk, D, kind, ns):
+    """Causal split-KV: every split writes the LSE of every row, a split without keys too (-inf), and the combine
+    reads them all.  A workspace full of NaN and a zeroed one give the same bits."""
+    q, k, v = make_inputs(B, Hq, Hkv, Sq, Sk, D, kind, seed=11)
+    L = tfa.lib()
+    st = torch.cuda.current_stream().cuda_stream
+    dtype = tfa.TFA_BF16 if kind == "bf16" else tfa.TFA_FP16
+    for f32 in (0, 1):
+        res = []
+        for fill in (float("nan"), 0.0):
+            out = torch.empty(q.shape, dtype=torch.float32 if f32 else q.dtype, device="cuda")
+            lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device="cuda")
+            a = tfa.AttnArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), B, Hq, Hkv, Sq,
+                             Sk, D, Hq * Sq * D, Sq * D, D, Hkv * Sk * D, Sk * D, D, dtype, 1, D ** -0.5, f32, ns, None,
+                             0, st)
+            assert L.tfa_attn_num_splits(ctypes.byref(a)) == ns
+            need = L.tfa_attn_workspace_bytes(ctypes.byref(a), ns)
+            ws = torch.full((need // 4,), fill, dtype=torch.float32, device="cuda")
+            a.workspace, a.workspace_bytes = ws.data_ptr(), need
+            tfa.check(L.tfa_attn_fwd(ctypes.byref(a)))
+            torch.cuda.synchronize()
+            res.append((out, lse))
+        (o_nan, l_nan), (o_zero, l_zero) = res
+        assert torch.equal(o_nan, o_zero) and torch.equal(l_nan, l_zero), f32
+
+
 def test_split_heuristic(tfa):
     """auto (num_splits=0): splits a long-key / few-row problem, leaves a grid that already fills the GPU alone."""
     q, k, v = make_inputs(1, 4, 4, 128, 16384, 128, "bf16")

@@ -91,8 +91,9 @@ __host__ __device__ __forceinline__ long long append_offset(int raw, const int* 
 }
 
 // Where a call's results go: row `row` of (batch b, head h) has its O at element b*sb + h*sh + row*ss of out and its
-// LSE at element b*lse_sb + h*lse_sh + row of lse.  The host builds it once per call (tfa_api.cu); the combine and the
-// empty-rows fill address out / lse through it, and set_output derives the forward's strides below from it.
+// LSE at element b*lse_sb + h*lse_sh + row of lse.  The host builds it once per call (tfa_api.cu); the forward and the
+// combine address out / lse through it.  Packed (varlen) layouts have sb = lse_sb = 0 and count `row` from the packed
+// tensors' first row.
 struct OutLayout {
   long long sb, sh, ss;
   long long lse_sb, lse_sh;
@@ -105,32 +106,33 @@ struct OutLayout {
 };
 
 struct FwdParams {
-  void* out;          // 16-bit output, element strides below
+  void* out;          // 16-bit output at `ol`
   // Fused exchange (multi-GPU): when n_extra_dst > 0 every 16-byte chunk of O is ALSO stored to these buffers
-  // (same strides) -- peer GPUs' copies of the gathered output, mapped over NVLink.  Replaces the all-gather.
+  // (same layout) -- peer GPUs' copies of the gathered output, mapped over NVLink.  Replaces the all-gather.
   void* extra_dst[7];
   int n_extra_dst;
-  float* out_f32;     // fp32 output (validation build), same strides
-  float* lse;         // (BH, S) fp32 or nullptr
-  long long o_stride_b, o_stride_h, o_stride_s;  // elements
+  float* out_f32;     // fp32 output (validation build, or the split-KV partials), at `ol`
+  float* lse;         // fp32 at `ol`, or nullptr
+  OutLayout ol;       // the caller's layout, or that of one split's partials in the workspace
   int H;             // query heads
   int S;             // query rows
   int npairs;         // ceil(S / 128): Q-tile pairs per (batch, head)
   // Generalised problem (SURVEY.md 8f rows 2-3; reference: flash_attention_c/csrc/attn.cpp:121-124,182-183 for
   // Sq != Sk with a bottom-right aligned causal mask, csrc/archive_)/attn.cpp:61,375 for grouped K/V heads):
-  int Sk;             // keys (== S for the reference's CuTe path)
-  int causal_off;     // Sk - S >= 0: query row i sees keys j <= i + causal_off
+  int Sk;             // keys (== S for the reference's CuTe path; may be < S)
+  int causal_off;     // Sk - S, negative when Sk < S: query row i sees keys j <= i + causal_off (rows i < -causal_off
+                      // see none)
   int kv_group;       // query heads per K/V head (1 = MHA)
   // split-KV: the grid carries nsplit work items per Q-tile pair, each covering split_tiles KV tiles and writing a
   // normalised fp32 partial O plus its LSE; tfa_splitkv_combine merges them.  nsplit == 1: split_tiles = all.
   int nsplit;
   int split_tiles;
   long long part_stride;      // out_f32 elements between consecutive splits
-  long long lse_stride_bh;    // lse elements between consecutive (b,h)
   long long lse_part_stride;  // lse elements between consecutive splits
   // launch order (decode_work below): heads are taken in chunks of `head_chunk`; total (batch*head) count `BH`
   int head_chunk;
   int BH;
+  int keyless_pairs;  // dense causal with Sq > Sk: the first Q-tile pairs of every (batch, head), which see no key
   int total_items;    // npairs * BH * nsplit
   float scale;        // softmax_scale
   float scale_log2;   // softmax_scale * log2(e)
@@ -261,8 +263,9 @@ __host__ __device__ __forceinline__ void decode_work(int block, int npairs, int 
 // One work item: both Q tiles walk the same KV tiles [jb, jb + n); rows a tile does not see are masked.
 // q0 / k0 are the sequence's first row in the (packed) q and k/v tensors, Sq / Sk / coff its own lengths and causal
 // offset: the whole tensor's (q0 = k0 = 0) for kDense, the cached length for kCache.  `live`: the item has rows to
-// write.  The producer loads an item iff n > 0, the softmax warpgroups wait on its barriers iff n > 0: n > 0 implies
-// live.
+// write -- every dense and cache item, and a packed item inside its sequence.  The producer loads an item iff n > 0,
+// the softmax warpgroups wait on its barriers iff n > 0: n > 0 implies live.  A live item with n == 0 writes O = 0 and
+// LSE = +inf (its rows see no key), or in a split-KV partial only LSE = -inf (its split holds none of their keys).
 struct Item {
   int bh, bidx, hidx, hkv, split, jb, row0, n;
   int q0, k0, Sq, Sk, coff;
@@ -275,7 +278,16 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
   constexpr bool QPACK = M == kVarlen || M == kVarlenCache;          // packed queries: items past a sequence skipped
   Item w;
   int pr;
-  decode_work(item, p.npairs, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
+  // dense: the items of the Q-tile pairs whose rows see no key follow all others, in decode_work order of their own.
+  // Interleaved with the rest, they would give some persistent CTAs up to twice the average share of keyed items.
+  const int keyless = M == kDense ? p.keyless_pairs : 0;
+  const int keyed_items = (p.npairs - keyless) * p.nsplit * p.BH;
+  if (keyless == 0 || item < keyed_items) {
+    decode_work(item, p.npairs - keyless, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
+    pr += keyless;
+  } else {
+    decode_work(item - keyed_items, keyless, p.nsplit, p.head_chunk, p.BH, w.bh, w.split, pr);
+  }
   w.bidx = w.bh / p.H;
   w.hidx = w.bh - w.bidx * p.H;
   w.hkv = w.hidx / p.kv_group;
@@ -317,15 +329,14 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.coff = p.causal_off;
   }
   const int nkv_total = (w.Sk + 127) >> 7;
-  // causal: the item's last row sees keys <= last (none when last < 0, which only varlen and cache sequences can have)
+  // causal: the item's last row sees keys <= last (none when last < 0)
   const int last = w.row0 + 127 + w.coff;
-  const int nfull = CAUSAL ? ((M != kDense && last < 0) ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
-  w.n = max(0, min(nfull - w.jb, p.split_tiles));   // 0: a split-KV item wholly above the causal diagonal
-  // dense: an item without tiles writes nothing (its rows belong to other splits); varlen: an item inside its sequence
-  // always writes its rows, as O = 0 and LSE = +inf when they see no key (n == 0); cache: every item writes its rows,
-  // a split without tiles too (LSE = -inf), so the combine can read every split's partial
-  w.live = QPACK ? w.row0 < w.Sq : (M == kCache || w.n > 0);
-  if (QPACK && !w.live) w.n = 0;     // past the sequence's end: the producer must skip it as the consumers do
+  const int nfull = CAUSAL ? (last < 0 ? 0 : min(nkv_total, last / 128 + 1)) : nkv_total;
+  w.n = max(0, min(nfull - w.jb, p.split_tiles));   // 0: rows that see no key, or a split past the causal diagonal
+  // every item writes its rows (a split without tiles their LSE), so the combine can read every split; only a packed
+  // item past its sequence's end has none
+  w.live = !QPACK || w.row0 < w.Sq;
+  if (!w.live) w.n = 0;              // past the sequence's end: the producer must skip it as the consumers do
   return w;
 }
 
@@ -618,9 +629,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
     };
 
-    // A varlen or cache item whose rows all see no key has no tiles: it waits on no barrier, its rows get O = 0 and
-    // LSE = +inf (-inf for a split-KV partial).
-    if (M == kDense || n > 0) {
+    // An item without tiles waits on no barrier: its rows get O = 0 and LSE = +inf (a split-KV partial: LSE = -inf).
+    if (n > 0) {
       mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
       ++qcnt;
       // ---- KV tile 0 ----
@@ -692,37 +702,27 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       inv_lo *= p.v_scale;
       inv_hi *= p.v_scale;
     }
-    const long long tile_off =
-        (QPACK ? static_cast<long long>(w.q0) * p.o_stride_s : static_cast<long long>(w.bidx) * p.o_stride_b) +
-        static_cast<long long>(w.hidx) * p.o_stride_h;
+    // the sequence's row 0; packed layouts have sb = lse_sb = 0, dense ones q0 = 0
+    const long long tile_off = p.ol.o(w.bidx, w.hidx, w.q0);
     if (p.lse != nullptr && tq == 0) {
-      if constexpr (QPACK) {
-        // (H, total_q); a row that saw no key (l == 0) gets +inf.  Not for split-KV partials, whose -inf tells the
-        // combine that the split holds nothing.
-        float* lrow = p.lse + static_cast<long long>(w.hidx) * p.lse_stride_bh + w.q0;
-        if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : INFINITY;
-        if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : INFINITY;
-      } else if constexpr (M == kCache) {
-        // (B, H, S) as dense; a row that saw no key gets +inf, or -inf in a split-KV partial (as above)
-        const float none = p.nsplit > 1 ? -INFINITY : INFINITY;
-        float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
-        if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : none;
-        if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : none;
-      } else {
-        float* lrow = p.lse + w.split * p.lse_part_stride + static_cast<long long>(w.bh) * p.lse_stride_bh;
-        if (row_lo < S) lrow[row_lo] = m_lo * p.scale + logf(l_lo);
-        if (row_hi < S) lrow[row_hi] = m_hi * p.scale + logf(l_hi);
-      }
+      // a row that saw no key (l == 0) gets +inf; in a split-KV partial -inf, which tells the combine that the split
+      // holds nothing for it
+      const float none = p.nsplit > 1 ? -INFINITY : INFINITY;
+      float* lrow = p.lse + w.split * p.lse_part_stride + p.ol.lse(w.bidx, w.hidx, w.q0);
+      if (row_lo < S) lrow[row_lo] = l_lo > 0.f ? m_lo * p.scale + logf(l_lo) : none;
+      if (row_hi < S) lrow[row_hi] = l_hi > 0.f ? m_hi * p.scale + logf(l_hi) : none;
     }
 
     if constexpr (OUT_F32) {
+      // a split-KV partial without tiles is never read: its LSE = -inf gives it weight 0 in the combine
+      const bool store = n > 0 || p.nsplit == 1;
       float* obase = p.out_f32 + w.split * p.part_stride + tile_off;
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int row = hr ? row_hi : row_lo;
         const float inv = hr ? inv_hi : inv_lo;
-        if (row < S) {
-          float* orow = obase + static_cast<long long>(row) * p.o_stride_s + 2 * tq;
+        if (store && row < S) {
+          float* orow = obase + static_cast<long long>(row) * p.ol.ss + 2 * tq;
 #pragma unroll
           for (int i = 0; i < D / 8; ++i)
             *reinterpret_cast<float2*>(orow + 8 * i) = make_float2(o[4 * i + 2 * hr] * inv, o[4 * i + 2 * hr + 1] * inv);
@@ -754,7 +754,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const uint4 v4 = *reinterpret_cast<const uint4*>(stg + rr * ROW_BYTES + phys * 16);
         const int rg = trow0 + rr;
         if (rg < S) {
-          const long long off = static_cast<long long>(rg) * p.o_stride_s * 2 + chunk * 16;
+          const long long off = static_cast<long long>(rg) * p.ol.ss * 2 + chunk * 16;
           st_global_v4(obase + off, v4);
           for (int d = 0; d < p.n_extra_dst; ++d)          // peer copies: posted stores over NVLink
             st_global_v4(reinterpret_cast<uint8_t*>(p.extra_dst[d]) + tile_off * 2 + off, v4);

@@ -15,7 +15,6 @@
 #include <cuda_runtime.h>
 #include <cudaTypedefs.h>
 #include <atomic>
-#include <cassert>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -163,7 +162,7 @@ int count_launch() {
   return static_cast<int>(cudaGetLastError());
 }
 
-// The fill, combine and append kernels: 256 threads per block, each block taking `per_block` of the `n` rows or chunks.
+// The combine and append kernels: 256 threads per block, each block taking `per_block` of the `n` rows or chunks.
 template <typename P>
 int launch_small(void (*kern)(P), long long n, int per_block, const P& prm, cudaStream_t stream) {
   const long long blocks = (n + per_block - 1) / per_block;
@@ -245,13 +244,16 @@ int validate(const Problem& a) {
   return 0;
 }
 
+// Query rows of a dense call that see at least one key: causal with Sq > Sk leaves the first Sq - Sk rows without
+// one.  The split count and the schedule are chosen for these rows: the items of the others load nothing.
+int keyed_rows(bool causal, int Sq, int Sk) { return (causal && Sk < Sq) ? Sk : Sq; }
+
 // Split-KV decision.  `want` 0 = auto: split only when the plain grid would leave more than half of the SMs idle,
 // into as many splits as still fit one wave of CTAs (one CTA more than the SMs would double the time), each with
 // >= 4 KV tiles;
 // n > 1 = as asked, clamped so that no split is empty.
 int resolve_splits(const Problem& a, int want, int sms) {
-  const int sq_eff = (a.causal && a.Sk < a.Sq) ? a.Sk : a.Sq;          // rows that see at least one key
-  const long long items = ((static_cast<long long>(sq_eff) + 127) / 128) * a.B * a.Hq;
+  const long long items = ((static_cast<long long>(keyed_rows(a.causal != 0, a.Sq, a.Sk)) + 127) / 128) * a.B * a.Hq;
   const int nkv = (a.Sk + 127) / 128;
   int n = want;
   if (n == 0) {
@@ -267,8 +269,7 @@ int resolve_splits(const Problem& a, int want, int sms) {
 }
 
 // Split-KV workspace: `nsplit` normalised fp32 partials of the (B, Hq, S, D) output, then their nsplit (B, Hq, S)
-// LSEs (set_output partitions it).  It is sized for the caller's Sq; a dense causal call with Sq > Sk fills it for the
-// Sk rows that see a key.
+// LSEs (set_output partitions it).  Every split writes the LSEs of all Sq rows.
 size_t splitkv_ws_bytes(const Problem& a, int nsplit) {
   if (nsplit <= 1) return 0;
   return static_cast<size_t>(nsplit) * a.B * a.Hq * a.Sq * (static_cast<size_t>(a.D) + 1) * sizeof(float);
@@ -299,43 +300,29 @@ int plan_splits(const Problem& a, SplitPlan& plan) {
 
 // Where the forward over S query rows per (batch, head) writes: the caller's out / lse in one pass; with split-KV,
 // contiguous (B, Hq, S, D) fp32 partials per split with their LSEs, which the combine merges into out / lse.
-void set_output(FwdParams& p, const Problem& a, int S, int nsplit, bool varlen) {
+void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
   if (nsplit > 1) {
     const long long rows = static_cast<long long>(a.B) * a.Hq * S;
     float* ws_o = static_cast<float*>(a.ws);
     p.out = nullptr;
     p.out_f32 = ws_o;
     p.lse = ws_o + static_cast<size_t>(nsplit) * rows * a.D;
-    p.o_stride_s = a.D;
-    p.o_stride_h = static_cast<long long>(S) * a.D;
-    p.o_stride_b = p.o_stride_h * a.Hq;
+    p.ol = {static_cast<long long>(a.Hq) * S * a.D, static_cast<long long>(S) * a.D, a.D,
+            static_cast<long long>(a.Hq) * S, S};
     p.part_stride = rows * a.D;
-    p.lse_stride_bh = S;
     p.lse_part_stride = rows;
   } else {
     const bool f32 = a.out_fp32 != 0;
     p.out = f32 ? nullptr : a.out;
     p.out_f32 = f32 ? static_cast<float*>(a.out) : nullptr;
     p.lse = a.lse;
-    p.o_stride_b = a.ol.sb;
-    p.o_stride_h = a.ol.sh;
-    p.o_stride_s = a.ol.ss;
+    p.ol = a.ol;
     p.part_stride = 0;
-    // The forward steps through lse in (batch*head) rows of lse_sh, or, for varlen, in head rows plus the sequence's
-    // first packed row; the combine and the fill read a.ol itself.  Both agree only for these layouts.
-    assert(a.ol.lse_sb == (varlen ? 0 : static_cast<long long>(a.Hq) * a.ol.lse_sh));
-    p.lse_stride_bh = a.ol.lse_sh;
     p.lse_part_stride = 0;
   }
 }
 
-// the fill and combine kernels take D / 4 threads per row
-template <int D>
-int launch_fill(const tfa::FillParams& fp, bool f32, cudaStream_t stream) {
-  return launch_small(f32 ? tfa::empty_rows_fill_kernel<D, true> : tfa::empty_rows_fill_kernel<D, false>, fp.rows,
-                      256 / (D / 4), fp, stream);
-}
-
+// the combine kernel takes D / 4 threads per row
 template <int D>
 int launch_combine(const tfa::CombineParams& cp, bool bf16, bool f32, cudaStream_t stream) {
   auto kern = f32 ? tfa::splitkv_combine_kernel<D, true, true>
@@ -345,13 +332,15 @@ int launch_combine(const tfa::CombineParams& cp, bool bf16, bool f32, cudaStream
 
 // The rest of every forward call.  `p` arrives zeroed with its mode's fields set (Sk / causal_off / extra_dst, cu_q /
 // cu_k, or the cache fields); this sets the fields all modes share, chooses the kernel, launches the forward over S
-// query rows per (batch, head) and, with split-KV, the combine.  With `combine_causal` the combine skips the splits
-// above a row's causal diagonal, which wrote nothing.
+// query rows per (batch, head) and, with split-KV, the combine.
 template <int MODE>
 int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, const CUtensorMap& tk,
-                const CUtensorMap& tv, SplitPlan plan, bool combine_causal) {
+                const CUtensorMap& tv, SplitPlan plan) {
   const bool causal = a.causal != 0, bf16 = a.dtype == TFA_BF16, f32 = a.out_fp32 != 0;
+  constexpr int M = tfa::base_mode(MODE);
   const long long npairs = (static_cast<long long>(S) + 127) / 128;
+  // dense: the schedule is chosen for the Q-tile pairs with keys, as the split count is (resolve_splits)
+  const int S_keyed = M == tfa::kDense ? keyed_rows(causal, S, a.Sk) : S;
   p.H = a.Hq;
   p.kv_group = a.Hq / a.Hkv;
   p.npairs = static_cast<int>(npairs);
@@ -365,10 +354,9 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   p.S = S;
   p.nsplit = plan.nsplit;
   p.split_tiles = plan.split_tiles;
-  constexpr int M = tfa::base_mode(MODE);
-  set_output(p, a, S, plan.nsplit, M == tfa::kVarlen || M == tfa::kVarlenCache);
+  set_output(p, a, S, plan.nsplit);
 
-  const int variant = choose_kernel(causal, npairs, p.n_extra_dst);
+  const int variant = choose_kernel(causal, (static_cast<long long>(S_keyed) + 127) / 128, p.n_extra_dst);
   int rc = launch_fwd<MODE>(a.D, causal, bf16, f32 || plan.nsplit > 1, tq, tk, tv, p, npairs * a.B * a.Hq * plan.nsplit,
                             variant, a.stream);
   if (rc || plan.nsplit == 1) return rc;
@@ -381,13 +369,11 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   cp.ol = a.ol;
   cp.rows = static_cast<long long>(a.B) * a.Hq * S;
   cp.H = a.Hq; cp.S = S;
-  cp.nsplit = plan.nsplit; cp.split_tiles = plan.split_tiles;
-  cp.nkv_total = (a.Sk + 127) / 128;
-  cp.causal = combine_causal ? 1 : 0; cp.causal_off = p.causal_off;
+  cp.nsplit = plan.nsplit;
   return (a.D == 64) ? launch_combine<64>(cp, bf16, f32, a.stream) : launch_combine<128>(cp, bf16, f32, a.stream);
 }
 
-int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
+int fwd_impl(const Problem& a, void* const* extra_dst = nullptr, int n_extra = 0) {
   int rc = validate(a);
   if (rc) return rc;
   if (!arch_ok()) return TFA_EARCH;
@@ -406,21 +392,6 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
   SplitPlan plan;
   if ((rc = plan_splits(a, plan))) return rc;
 
-  // causal with more queries than keys: rows [0, Sq-Sk) see nothing; the rest is a square causal problem
-  if (causal && a.Sk < a.Sq) {
-    const int n_empty = a.Sq - a.Sk;
-    tfa::FillParams fp;
-    fp.out = a.out; fp.lse = a.lse; fp.ol = a.ol;
-    fp.rows = static_cast<long long>(a.B) * a.Hq * n_empty;
-    fp.H = a.Hq; fp.n_empty = n_empty;
-    rc = (a.D == 64) ? launch_fill<64>(fp, f32, a.stream) : launch_fill<128>(fp, f32, a.stream);
-    if (rc) return rc;
-    a.q = static_cast<const char*>(a.q) + static_cast<size_t>(n_empty) * a.qss * 2;
-    a.out = static_cast<char*>(a.out) + static_cast<size_t>(n_empty) * a.ol.ss * (f32 ? 4 : 2);
-    if (a.lse) a.lse += n_empty;
-    a.Sq = a.Sk;
-  }
-
   CUtensorMap tq, tk, tv;
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
   if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
@@ -428,10 +399,11 @@ int fwd_impl(Problem a, void* const* extra_dst = nullptr, int n_extra = 0) {
 
   FwdParams p{};
   p.Sk = a.Sk;
-  p.causal_off = causal ? a.Sk - a.Sq : 0;             // >= 0 after the shift
+  p.causal_off = causal ? a.Sk - a.Sq : 0;             // < 0: the first Sq - Sk rows see no key
+  p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
   for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
   p.n_extra_dst = n_extra;
-  return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan, causal);
+  return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan);
 }
 
 Problem from_fwd_args(const tfa_fwd_args& a) {
@@ -496,7 +468,7 @@ int varlen_impl(const tfa_attn_varlen_args& va) {
   p.total_k = a.Sk;
   // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once.  One
   // split holds every KV tile of any sequence.
-  return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
+  return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
 }
 
 // The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
@@ -646,12 +618,11 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
   }
 
   p.snew = snew;
-  // every split writes its rows (LSE = -inf where it saw no key): the combine reads all of them
   if (quant) {
     p.v_scale = qs.v_scale;
-    return run_forward<tfa::kCacheFp8>(a, p, a.Sq, tq, tk, tv, plan, false);
+    return run_forward<tfa::kCacheFp8>(a, p, a.Sq, tq, tk, tv, plan);
   }
-  return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan, false);
+  return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan);
 }
 
 // The variable-length cache problem as the varlen one of total_q query rows (what validate() checks of q and out)
@@ -702,9 +673,9 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_kv_qua
   // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
   if (quant) {
     p.v_scale = qs.v_scale;
-    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
+    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
   }
-  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff}, false);
+  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
 }
 
 // ---- host-buffer path workspace ----
@@ -886,11 +857,11 @@ void tfa_host_release(void) {
 unsigned long long tfa_launch_count(void) { return g_launches.load(); }
 // development aid (not in the public header): which kernel the last forward launch used (0 classic, 4 persistent)
 int tfa_internal_last_variant(void) { return g_last_variant.load(); }
-// development aid (not in the public header): the kernel-selection rule as a host function (no device needed); it
-// takes the whole problem shape, of which the rule reads the mask, the query length and the exchange
+// development aid (not in the public header): the kernel-selection rule of a dense call as a host function (no device
+// needed); it takes the whole problem shape, of which the rule reads the mask, the rows with keys and the exchange
 int tfa_internal_choose_kernel(int D, int causal, int Sq, int Sk, int B, int Hq, int nsplit, int sms, int n_extra) {
-  (void)D; (void)Sk; (void)B; (void)Hq; (void)nsplit; (void)sms;
-  return choose_kernel(causal != 0, (static_cast<long long>(Sq) + 127) / 128, n_extra);
+  (void)D; (void)B; (void)Hq; (void)nsplit; (void)sms;
+  return choose_kernel(causal != 0, (static_cast<long long>(keyed_rows(causal != 0, Sq, Sk)) + 127) / 128, n_extra);
 }
 // exported for the self tests living in another translation unit
 void tfa_internal_count_launch(void) { g_launches.fetch_add(1, std::memory_order_relaxed); }
