@@ -38,7 +38,7 @@ extern "C" {
 /* dtype codes (reference: Qkv_params::is_bf16, flash.h:27) */
 #define TFA_BF16 0
 #define TFA_FP16 1
-#define TFA_FP8_E4M3 2  /* cache element type of the quantized cache calls only (tfa_kv_quant_args) */
+#define TFA_FP8_E4M3 2  /* input element type of the quantized calls only (tfa_kv_quant_args, tfa_qkv_quant_args) */
 
 /* argument errors */
 #define TFA_EINVAL_PTR    (-1)  /* null or not 16-byte aligned pointer           */
@@ -60,6 +60,8 @@ extern "C" {
                                       in [16, D], seqlen_ro < capacity, or no k_new */
 #define TFA_EINVAL_KVQUANT (-15)   /* FP8 cache: cache_dtype not TFA_FP8_E4M3, k_scale / v_scale not finite and > 0, or
                                       cache strides not multiples of 16 elements */
+#define TFA_EINVAL_QKVQUANT (-16)  /* FP8 attention: qkv_dtype not TFA_FP8_E4M3, q_scale / k_scale / v_scale not finite and
+                                      > 0, or q / k / v strides not multiples of 16 elements */
 
 /* Extended argument block (POD), the analogue of Flash_fwd_params (flash.h:29-60).
  * Strides are in ELEMENTS.  The innermost (head_dim) stride must be 1.
@@ -363,6 +365,31 @@ int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary
                              const tfa_kv_quant_args* quant);
 int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant);
 
+/* ---- attention on FP8 (e4m3) q, k and v with per-tensor scales, both products on FP8 tensor cores (FlashAttention-3's
+ * descale_q / descale_k / descale_v) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_fp8_fwd.  The problem of tfa_attn_fwd(), unchanged -- grouped K/V heads, Sq != Sk with the bottom-right
+ * causal mask, key-less rows out = 0 / lse = +inf, split-KV through num_splits / workspace (tfa_attn_num_splits() and
+ * tfa_attn_workspace_bytes() on the same args), out_fp32 -- with q, k and v holding one byte per element.
+ *
+ *   q, k, v  : e4m3 codes (torch.float8_e4m3fn).  Strides are in elements, so in bytes, and must be multiples of 16.
+ *   dtype    : the OUTPUT dtype, TFA_BF16 or TFA_FP16 (or fp32 with out_fp32).  out uses q's element strides; lse is
+ *              fp32 (B, Hq, Sq) as everywhere.
+ *   scales   : a code x8 stands for q_scale * x8 in Q, k_scale * x8 in K, v_scale * x8 in V; out and lse are those of
+ *              the dequantized problem.  The kernel computes S = Q8 K8^T on e4m3 wgmma with fp32 accumulation, takes the
+ *              softmax with scale s' = fp32(fp32(softmax_scale * q_scale) * k_scale) (that order), rounds P to e4m3
+ *              (round to nearest even; P <= 2^8), computes P8 V8 on e4m3 wgmma and multiplies O by v_scale.
+ * s' must stay a normal fp32 number: when it overflows, or when softmax_scale > 0 and it underflows below FLT_MIN, the
+ * call returns TFA_EINVAL_SCALE.  Every check runs before any device work, those of tfa_attn_fwd() first, in its order,
+ * then TFA_EINVAL_QKVQUANT, then TFA_EINVAL_SCALE for s'.  Launches: 1, + 1 with split-KV.  Callers quantize, e.g.
+ * (x / s).clamp(-448, 448).to(torch.float8_e4m3fn). */
+typedef struct tfa_qkv_quant_args {
+  int32_t qkv_dtype;                 /* TFA_FP8_E4M3 */
+  float q_scale, k_scale, v_scale;   /* finite, > 0 */
+} tfa_qkv_quant_args;
+
+int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant);
+
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on
  * `n_streams` internal streams so H2D, compute and D2H overlap, copies out, and
@@ -402,6 +429,16 @@ int tfa_selftest_tma(const void* src, int D, int S, int BH, int x0, int y0, int 
  *              (bit0: swap packing order of the two 16-bit halves of register A). */
 int tfa_selftest_umma(const void* a, const void* b, float* c, int N, int K, int mode,
                       int dtype, const int* knobs, void* stream);
+
+/* e4m3 wgmma chains with fp32 accumulation, C(128 x N) += chain x A(128 x K) * B, two m64 halves, K in {64, 128}: the
+ * accumulator starts at c's contents and takes the K-deep chain `chain` times (1..4096), chain x K / 32 k-steps.
+ *   mode 0: SS, A (128 x K) and B (N x K) both K-major e4m3, staged by TMA with the 128-byte (K = 128) or 64-byte
+ *           (K = 64) swizzle; N = 128 (the Q K^T contraction).
+ *   mode 1: RS, A (128 x 128 keys) in registers, packed from the fp32 accumulator layout in fp8_p_key order, and B
+ *           (N x 128 keys) K-major in shared memory with its keys in the same order, written by the V^T converter from
+ *           the (128 keys x N) row-major b; N in {64, 128} (the P V contraction).  K must be 128.
+ * a, b hold e4m3 codes (row-major as described), c fp32 (128 x N), read and overwritten. */
+int tfa_selftest_wgmma_fp8(const void* a, const void* b, float* c, int N, int K, int mode, int chain, void* stream);
 
 #ifdef __cplusplus
 }

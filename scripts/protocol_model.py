@@ -26,6 +26,15 @@ kv_full and releases the raw tile.  The softmax warpgroups are unchanged, but do
 writes those rows as zeros).  Shadow state adds: a raw tile overwritten by TMA while the converter reads it, and the
 converter storing into a slot a wgmma still reads.
 
+DenseFp8Sim models kDenseFp8 (Q, K and V in e4m3) with three rings of their own depths and barriers: K (nk slots,
+filled by TMA: k_full one arrival, k_empty one per warpgroup), raw V (nraw slots, filled by TMA: raw_full one arrival;
+raw_empty one per converter warp) and V^T (nvt slots, written by the converter: vt_full one arrival per converter warp,
+vt_empty one per warpgroup).  Tile j of the running tile count takes slot j % depth of each ring.  The three converter
+warps are roles of their own: each waits on the tile's raw_full and its V^T slot's vt_empty, stores its part (spanning
+a scheduling point), then arrives on vt_full and raw_empty.  Shadow state adds: a V^T slot read by a wgmma before every
+converter warp's part of that tile is stored, or while one still stores into it, and a converter warp storing into a
+slot a wgmma still reads.
+
 Run:  python scripts/protocol_model.py [trials]      (exit code 0 = no violation found)
 """
 import random
@@ -273,6 +282,203 @@ class Sim:
             assert self.finished[t] == done
 
 
+class DenseFp8Sim:
+    """kDenseFp8: the TMA lane (Q, K, raw V), three converter warps (raw V -> V^T) and the two softmax warpgroups."""
+    WARPS = 3                                                 # converter warps (producer warps 1-3)
+
+    def __init__(self, items, nk, nraw, nvt, rng):
+        self.items, self.NK, self.R, self.V, self.rng = items, nk, nraw, nvt, rng
+        self.empty = {i for i, n in enumerate(items) if n == 0}
+        self.q_full, self.q_empty = Bar("q_full", 1), Bar("q_empty", 2)
+        self.k_full = [Bar(f"k_full{i}", 1) for i in range(nk)]
+        self.k_empty = [Bar(f"k_empty{i}", 2) for i in range(nk)]
+        self.raw_full = [Bar(f"raw_full{i}", 1) for i in range(nraw)]
+        self.raw_empty = [Bar(f"raw_empty{i}", self.WARPS) for i in range(nraw)]
+        self.vt_full = [Bar(f"vt_full{i}", self.WARPS) for i in range(nvt)]
+        self.vt_empty = [Bar(f"vt_empty{i}", 2) for i in range(nvt)]
+        # shadow state
+        self.q_buf, self.q_readers = None, 0
+        self.k_buf, self.k_readers = [None] * nk, [0] * nk
+        self.raw_buf, self.raw_readers = [None] * nraw, [0] * nraw
+        self.vt_part = [[None] * self.WARPS for _ in range(nvt)]   # the tile each warp's part of the slot holds
+        self.vt_readers, self.vt_writers = [0] * nvt, [0] * nvt
+        self.tma_q, self.mma_q = [], [[], []]
+        self.seen, self.finished = [[], []], [[], []]
+
+    tma = Sim.tma
+    tick = Sim.tick
+    in_flight = Sim.in_flight
+
+    def producer(self):
+        NK, R, tile, qcnt = self.NK, self.R, 0, 0
+        for item, n in enumerate(self.items):
+            if n == 0:
+                continue
+            if qcnt > 0:
+                yield lambda p=(qcnt - 1) & 1: self.q_empty.done(p)
+            qcnt += 1
+            assert self.q_readers == 0, f"Q buffer overwritten while a wgmma reads it (item {item})"
+            self.q_buf = "busy"
+
+            def q_landed(item=item):
+                assert self.q_readers == 0, "Q buffer written under a reader"
+                self.q_buf = item
+                self.q_full.arrive()
+            self.tma(q_landed)
+            for j in range(n):
+                ks, rs, tag = tile % NK, tile % R, (item, j)
+                yield lambda s=ks, p=((tile // NK) & 1) ^ 1: self.k_empty[s].done(p)
+                assert self.k_readers[ks] == 0, f"K slot {ks} overwritten while a wgmma reads it"
+                self.k_buf[ks] = "busy"
+
+                def k_landed(ks=ks, tag=tag):
+                    assert self.k_readers[ks] == 0, "K slot written under a reader"
+                    self.k_buf[ks] = tag
+                    self.k_full[ks].arrive()
+                self.tma(k_landed)
+                yield lambda s=rs, p=((tile // R) & 1) ^ 1: self.raw_empty[s].done(p)
+                assert self.raw_readers[rs] == 0, f"raw tile {rs} overwritten while the converter reads it"
+                self.raw_buf[rs] = "busy"
+
+                def raw_landed(rs=rs, tag=tag):
+                    assert self.raw_readers[rs] == 0, "raw tile written under the converter"
+                    self.raw_buf[rs] = tag
+                    self.raw_full[rs].arrive()
+                self.tma(raw_landed)
+                tile += 1
+
+    def _store_vt(self, w, vs, rs, tag):
+        """Converter warp w's part of the transpose of raw tile rs into V^T slot vs: the stores span a scheduling
+        point."""
+        assert self.raw_buf[rs] == tag, f"converter {w}: raw tile {rs} holds {self.raw_buf[rs]}, not {tag}"
+        assert self.vt_readers[vs] == 0, f"converter {w} stores into V^T slot {vs} while a wgmma reads it"
+        self.raw_readers[rs] += 1
+        self.vt_writers[vs] += 1
+        self.vt_part[vs][w] = "converting"
+        yield lambda: True
+        assert self.vt_readers[vs] == 0, f"V^T slot {vs} read by a wgmma under converter {w}'s stores"
+        self.vt_part[vs][w] = tag
+        self.vt_writers[vs] -= 1
+        self.raw_readers[rs] -= 1
+
+    def converter(self, w):
+        R, V, tile = self.R, self.V, 0
+        for item, n in enumerate(self.items):
+            for j in range(n):
+                rs, vs, tag = tile % R, tile % V, (item, j)
+                yield lambda s=rs, p=(tile // R) & 1: self.raw_full[s].done(p)
+                yield lambda s=vs, p=((tile // V) & 1) ^ 1: self.vt_empty[s].done(p)
+                yield from self._store_vt(w, vs, rs, tag)
+                self.vt_full[vs].arrive()                     # after the last store (and its proxy fence)
+                self.raw_empty[rs].arrive()
+                tile += 1
+
+    def consumer(self, t):
+        NK, V, ent, qcnt = self.NK, self.V, 0, 0
+
+        def issue(reads):
+            for what, slot, tag in reads:
+                if what == "Q":
+                    assert self.q_buf == tag, f"wg{t}: Q buffer holds {self.q_buf}, expected item {tag}"
+                    self.q_readers += 1
+                elif what == "K":
+                    assert self.k_buf[slot] == tag, f"wg{t}: K slot {slot} holds {self.k_buf[slot]}, expected {tag}"
+                    self.k_readers[slot] += 1
+                else:
+                    assert self.vt_writers[slot] == 0 and self.vt_part[slot] == [tag] * self.WARPS, \
+                        f"wg{t}: V^T slot {slot} holds {self.vt_part[slot]}, expected {tag}"
+                    self.vt_readers[slot] += 1
+
+            def done():
+                for what, slot, _ in reads:
+                    if what == "Q":
+                        self.q_readers -= 1
+                    elif what == "K":
+                        self.k_readers[slot] -= 1
+                    else:
+                        self.vt_readers[slot] -= 1
+            self.mma_q[t].append([self.rng.randint(1, 6), done])
+
+        def wait_group(k):
+            yield lambda: self.in_flight(t) <= k
+
+        def wait_k(e):
+            yield lambda s=e % NK, p=(e // NK) & 1: self.k_full[s].done(p)
+
+        def wait_vt(e):
+            yield lambda s=e % V, p=(e // V) & 1: self.vt_full[s].done(p)
+
+        for item, n in enumerate(self.items):
+            if n == 0:
+                yield lambda: True                            # epilogue only: no barrier is touched
+                self.finished[t].append(item)
+                continue
+            yield lambda p=qcnt & 1: self.q_full.done(p)
+            qcnt += 1
+            yield from wait_k(ent)
+            issue([("Q", None, item), ("K", ent % NK, (item, 0))])
+            self.seen[t].append((item, 0))
+            yield from wait_group(0)
+            self.k_empty[ent % NK].arrive()
+            if n == 1:
+                self.q_empty.arrive()
+            for j in range(1, n):
+                ek, ev = ent + j, ent + j - 1
+                yield from wait_k(ek)
+                issue([("Q", None, item), ("K", ek % NK, (item, j))])
+                self.seen[t].append((item, j))
+                yield from wait_vt(ev)
+                issue([("VT", ev % V, (item, j - 1))])
+                yield from wait_group(1)
+                self.k_empty[ek % NK].arrive()
+                if j == n - 1:
+                    self.q_empty.arrive()
+                yield from wait_group(0)
+                self.vt_empty[ev % V].arrive()
+            ev = ent + n - 1
+            yield from wait_vt(ev)
+            issue([("VT", ev % V, (item, n - 1))])
+            yield from wait_group(0)
+            self.vt_empty[ev % V].arrive()
+            ent += n
+            self.finished[t].append(item)
+
+    def run(self, max_steps=200000):
+        roles = [self.producer(), self.consumer(0), self.consumer(1)] + [self.converter(w) for w in range(self.WARPS)]
+        nr = len(roles)
+        waits, alive = [None] * nr, [True] * nr
+        for _ in range(max_steps):
+            ready = [i for i in range(nr) if alive[i] and (waits[i] is None or waits[i]())]
+            busy = bool(self.tma_q) or any(self.mma_q)
+            if not ready and not busy:
+                if not any(alive):
+                    break
+                raise AssertionError("deadlock: " + ", ".join(f"role{i}" for i in range(nr) if alive[i]))
+            if ready and (not busy or self.rng.random() < 0.6):
+                i = self.rng.choice(ready)
+                try:
+                    waits[i] = next(roles[i])
+                except StopIteration:
+                    alive[i] = False
+                    waits[i] = None
+            else:
+                self.tick()
+        else:
+            raise AssertionError("did not finish")
+        want = [(it, j) for it, n in enumerate(self.items) for j in range(n)]
+        done = list(range(len(self.items)))
+        for t in range(2):
+            assert self.seen[t] == want, f"wg{t} consumed {self.seen[t]}, expected {want}"
+            assert self.finished[t] == done
+
+
+def random_dense_fp8(rng):
+    """kDenseFp8: the dense items of random_items and ring depths (K, raw V, V^T), the shipped 4 / 3 / 4 and 8 / 4 / 8
+    among them."""
+    depths = rng.choice([(4, 3, 4), (8, 4, 8), (1, 1, 1), (2, 3, 1), (3, 1, 2)])
+    return random_items(rng), depths
+
+
 def random_items(rng):
     """Tiles per item of a dense problem.  Items without tiles (causal rows above the first key when Sq > Sk, or a split
     past a Q tile's causal diagonal) are live: Sim's default writes their rows."""
@@ -363,6 +569,9 @@ def main():
         for varlen in (False, True):
             items, empty, vtail, nraw = random_fp8_cache_items(rng, varlen)
             Sim(items, rng.choice([4, 8]), rng, empty, vtail, fp8=True, nraw=nraw).run()
+        rng8 = random.Random(2000003 + trial)             # kDenseFp8, on a generator of its own
+        items, depths = random_dense_fp8(rng8)
+        DenseFp8Sim(items, *depths, rng8).run()
     print(f"{trials} trials: no violation")
 
 

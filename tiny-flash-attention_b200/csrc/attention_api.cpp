@@ -210,6 +210,57 @@ std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Te
   return {out, lse};
 }
 
+// FP8 attention (tfa_attn_fp8_fwd): q, k, v as flash_attention_v2_general but float8_e4m3fn, with the per-tensor scales
+// their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is the output's.
+std::vector<torch::Tensor> flash_attention_v2_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v, double q_scale,
+                                                  double k_scale, double v_scale, bool is_causal, float softmax_scale,
+                                                  at::ScalarType out_dtype, int64_t num_splits) {
+  TFA_CHECK_INPUT(q);
+  TFA_CHECK_INPUT(k);
+  TFA_CHECK_INPUT(v);
+  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q, k, v must have 4 dimensions");
+  TORCH_CHECK(q.scalar_type() == at::kFloat8_e4m3fn && k.scalar_type() == at::kFloat8_e4m3fn &&
+              v.scalar_type() == at::kFloat8_e4m3fn, "q, k, v must be float8_e4m3fn");
+  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on one device");
+  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf, "out_dtype must be bfloat16 or float16");
+  TORCH_CHECK(k.sizes() == v.sizes(), "k and v must have identical shapes");
+  TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), "k/v must share batch and head_dim with q");
+  const int64_t B = q.size(0), Hq = q.size(1), Sq = q.size(2), D = q.size(3), Hkv = k.size(1), Sk = k.size(2);
+  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
+  TORCH_CHECK(B >= 1 && Hq >= 1 && Hkv >= 1 && Sq >= 1 && Sk >= 1, "empty tensors are not supported");
+  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(num_splits >= 0 && num_splits <= 1024, "num_splits must be in [0, 1024]");
+
+  torch::Tensor out, lse, ws;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    out = torch::empty(q.sizes(), q.options().dtype(out_dtype));
+    lse = torch::empty({B, Hq, Sq}, q.options().dtype(at::kFloat));
+    tfa_attn_args a;
+    a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
+    a.Sq = static_cast<int32_t>(Sq); a.Sk = static_cast<int32_t>(Sk); a.D = static_cast<int32_t>(D);
+    a.q_stride_b = Hq * Sq * D; a.q_stride_h = Sq * D; a.q_stride_s = D;
+    a.kv_stride_b = Hkv * Sk * D; a.kv_stride_h = Sk * D; a.kv_stride_s = D;
+    a.dtype = out_dtype == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.out_fp32 = 0;
+    a.num_splits = static_cast<int32_t>(num_splits);
+    a.workspace = nullptr; a.workspace_bytes = 0;
+    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    ws = split_workspace(a, q);
+    tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
+                          static_cast<float>(v_scale)};
+    rc = tfa_attn_fp8_fwd(&a, &qa);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
 // Variable-length batch (the packed cu_seqlens interface of flash-attn's varlen forward): q (total_q, Hq, D),
 // k, v (total_k, Hkv, D), unit head_dim stride (views of one packed (total, 3, H, D) qkv tensor need no copy);
 // cu_seqlens_q / cu_seqlens_k int32 of B + 1 offsets on q's device.  Returns out (total_q, Hq, D) contiguous and
@@ -621,6 +672,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_fp32out", &flash_attention_v2_fp32out, "same op, fp32 output (validation)");
   m.def("flash_attention_v2_general", &flash_attention_v2_general,
         "grouped K/V heads, Sq != Sk (bottom-right causal), optional split-KV: (q, k, v, is_causal, scale, num_splits)");
+  m.def("flash_attention_v2_fp8", &flash_attention_v2_fp8,
+        "FP8 attention: float8_e4m3fn q, k, v with per-tensor scales, e4m3 tensor cores -> [out (out_dtype), lse]",
+        py::arg("q"), py::arg("k"), py::arg("v"), py::arg("q_scale"), py::arg("k_scale"), py::arg("v_scale"),
+        py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"), py::arg("num_splits") = 1);
   m.def("flash_attention_v2_varlen", &flash_attention_v2_varlen,
         "packed variable-length batch: (q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, scale)");
   m.def("flash_attention_v2_kvcache", &flash_attention_v2_kvcache,

@@ -43,12 +43,30 @@
 
 namespace tfa {
 
-enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5 };
+enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5, kDenseFp8 = 6 };
 // The problem an FP8-cache mode solves is that of its 16-bit mode: they differ only in how K/V reach the ring.
 __host__ __device__ constexpr bool fp8_mode(int mode) { return mode == kCacheFp8 || mode == kVarlenCacheFp8; }
+// kDenseFp8 solves the dense problem with Q, K and V in e4m3 and both products on 8-bit wgmma (fp8_mode() is false
+// for it: that predicate means "widen K/V to 16 bits").
 __host__ __device__ constexpr int base_mode(int mode) {
-  return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode;
+  return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode == kDenseFp8 ? kDense : mode;
 }
+
+// ---- kDenseFp8: P as the 8-bit A operand without shuffles ----
+// The fp32 accumulator gives thread (g, tq) keys 8i + 2tq, +1 of rows g and g + 8; the 8-bit A fragment wants of it
+// columns 4tq .. 4tq + 3 (and 16 + those) of each 32-key k-step.  So A column c of a 32-key block holds key
+// pi(c) = 8 (x >> 1) + 2 tq + (x & 1) for c = 4 tq + x < 16, and pi(16 + c) = 16 + pi(c): every thread packs only its
+// own values, and the converter writes V^T's keys in the same order.  The sum over keys does not depend on it.
+__host__ __device__ constexpr int fp8_p_key(int c) {
+  return (c & 16) + 8 * ((c >> 1) & 1) + 2 * ((c >> 2) & 3) + (c & 1);
+}
+// The packer: byte x of A register r (0..3) of a k-step is accumulator element s[16 kk + fp8_pack_src(r, x)] (the
+// fp32 layout: s[4 i + 2 h + e] = row g + 8 h, key 8 i + 2 tq + e).  Derived from pi at tq = 0: 2 tq only shifts keys.
+__host__ __device__ constexpr int fp8_pack_src(int r, int x) {
+  return 4 * (fp8_p_key(16 * (r >> 1) + x) >> 3) + 2 * (r & 1) + (fp8_p_key(16 * (r >> 1) + x) & 1);
+}
+// The converter: position p (0..127) of a V^T row holds key fp8_vt_key(p) of the 128-key tile.
+__host__ __device__ constexpr int fp8_vt_key(int p) { return (p & ~31) + fp8_p_key(p & 31); }
 
 // ---- KV-cache address math, host-callable so that a CPU test can check it exhaustively (tests/test_kvcache.py) ----
 // Keys attended by sequence b: its cached length clamped to [0, capacity - snew], plus the snew appended keys.  The
@@ -197,8 +215,40 @@ struct Fp8Cfg {
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a block may use");
   static constexpr int CONVERTER_WARPS = 3;   // producer warps 1..3
 };
+// Shared-memory plan of kDenseFp8: Q (128 rows x D bytes), the 16-bit O staging of FwdCfg, then three rings of
+// 128 x D-byte tiles -- K (filled by TMA, SWIZZLE_128B at D = 128, SWIZZLE_64B at D = 64), raw V (unswizzled, as TMA
+// loads it) and V^T (D rows x 128 keys, SWIZZLE_128B, written by the converter) -- then the barriers: q_full, q_empty,
+// k_full / k_empty[NK], raw_full / raw_empty[NRAW], vt_full / vt_empty[NVT].  Each ring has its own barriers, so each
+// full barrier has one arrival count: 1 (TMA with its transaction bytes) for K and raw V, CONVERTER_WARPS for V^T.
+// Tile j of the running tile count takes slot j % N of each ring.  The D = 128 depths (4 + 3 + 4) are the largest that
+// fit with the K and V^T rings as deep as the 16-bit ring; they have not been A/B-measured against other splits, which
+// TFA_FP8F_K128 / _RAW128 / _VT128 build.  D = 64 has room for 8 + 4 + 8.
+#ifndef TFA_FP8F_K128
+#define TFA_FP8F_K128 4
+#endif
+#ifndef TFA_FP8F_RAW128
+#define TFA_FP8F_RAW128 3
+#endif
+#ifndef TFA_FP8F_VT128
+#define TFA_FP8F_VT128 4
+#endif
+template <int D>
+struct DenseFp8Cfg {
+  using C = FwdCfg<D>;
+  static constexpr int Q_BYTES = 128 * D;           // the item's two Q tiles
+  static constexpr int TILE8 = 128 * D;             // one K, raw V or V^T tile
+  static constexpr int NK = (D == 128) ? TFA_FP8F_K128 : 8;
+  static constexpr int NRAW = (D == 128) ? TFA_FP8F_RAW128 : 4;
+  static constexpr int NVT = (D == 128) ? TFA_FP8F_VT128 : 8;
+  static constexpr int NUM_BARS = 2 + 2 * (NK + NRAW + NVT);
+  static constexpr int SMEM_BYTES = 1024 + Q_BYTES + C::TILE_BYTES + (NK + NRAW + NVT) * TILE8 + NUM_BARS * 8;
+  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a block may use");
+  static constexpr int CONVERTER_WARPS = 3;         // producer warps 1..3
+};
 template <int D, int MODE>
-__host__ __device__ constexpr int fwd_smem_bytes() { return fp8_mode(MODE) ? Fp8Cfg<D>::SMEM_BYTES : FwdCfg<D>::SMEM_BYTES; }
+__host__ __device__ constexpr int fwd_smem_bytes() {
+  return MODE == kDenseFp8 ? DenseFp8Cfg<D>::SMEM_BYTES : fp8_mode(MODE) ? Fp8Cfg<D>::SMEM_BYTES : FwdCfg<D>::SMEM_BYTES;
+}
 
 // 8 e4m3 codes (bytes of r, element 0 in the low byte of r.x) -> 8 16-bit values, exactly: the code's sign and its
 // 7 exponent-mantissa bits placed at the top of the 16-bit type's exponent-mantissa field give x8 * 2^-(bias gap), and
@@ -225,6 +275,47 @@ __device__ __forceinline__ uint4 widen_e4m3x8(uint2 r) {
   return make_uint4(out[0], out[1], out[2], out[3]);
 }
 
+// kDenseFp8's converter, one unit u (0 <= u < 2 D) of a tile: keys [16 kc, 16 kc + 16) -- one 16-byte chunk of every
+// V^T row -- x columns [4 dc, 4 dc + 4) of the raw tile at `raw` (128 keys x D bytes, row-major) into the V^T slot at
+// `dst` (D rows x 128 keys, positions in fp8_vt_key order, SWIZZLE_128B).  Consecutive units take two chunks x 16
+// columns per warp: its loads hit two rows per bank, its stores (8 lanes: four chunks x two rows) distinct bank groups.
+template <int D>
+__device__ __forceinline__ void vt_convert_unit(uint32_t raw, uint32_t dst, int u) {
+  constexpr int DC = D / 4;
+  const int kc = 2 * (u / (2 * DC)) + (u & 1), dc = (u >> 1) % DC;
+  uint32_t L[16];                                     // L[k] = columns 4 dc .. +3 of key 16 kc + k
+#pragma unroll
+  for (int k = 0; k < 16; ++k)
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(L[k]) : "r"(raw + (16 * kc + k) * D + 4 * dc));
+  // row 4 dc + e, positions 16 kc + 4 x4 + x: key fp8_vt_key(16 kc + 4 x4 + x) = 16 kc + fp8_p_key(4 x4 + x), byte e
+  // (one row at a time: the converter runs on kRegsProducerFp8 registers)
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    uint32_t W[4];
+#pragma unroll
+    for (int x4 = 0; x4 < 4; ++x4) {
+      const uint32_t sel = e | ((e + 4) << 4);       // byte e of the first operand, then byte e of the second
+      const uint32_t ab = __byte_perm(L[fp8_p_key(4 * x4 + 0)], L[fp8_p_key(4 * x4 + 1)], sel);
+      const uint32_t cd = __byte_perm(L[fp8_p_key(4 * x4 + 2)], L[fp8_p_key(4 * x4 + 3)], sel);
+      W[x4] = __byte_perm(ab, cd, 0x5410);
+    }
+    const int r = 4 * dc + e;                         // SWIZZLE_128B: chunk kc of row r at kc ^ (r & 7)
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst + r * 128 + ((kc ^ (r & 7)) * 16)),
+                 "r"(W[0]), "r"(W[1]), "r"(W[2]), "r"(W[3]) : "memory");
+  }
+}
+// P (s[64], the fp32 accumulator layout of a 128-key tile) -> the A registers of its 4 k-steps of 32 keys, each
+// thread's own values in fp8_p_key order.
+__device__ __forceinline__ void pack_p_e4m3(const float* s, uint32_t* pf) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+      pf[4 * kk + r] = pack_e4m3x4(s[16 * kk + fp8_pack_src(r, 0)], s[16 * kk + fp8_pack_src(r, 1)],
+                                   s[16 * kk + fp8_pack_src(r, 2)], s[16 * kk + fp8_pack_src(r, 3)]);
+  }
+}
+
 // watchdog call sites
 enum : uint32_t { SITE_LOAD_EMPTY = 1, SITE_LOAD_Q = 2, SITE_MMA_Q = 3, SITE_MMA_K = 4, SITE_MMA_V = 5, SITE_CONV_RAW = 6 };
 
@@ -239,6 +330,12 @@ static_assert((2 * kRegsSoftmax + kRegsProducer) * 128 <= 384 * 168, "setmaxnreg
 constexpr uint32_t kRegsSoftmaxFp8 = 232;
 constexpr uint32_t kRegsProducerFp8 = 40;
 static_assert((2 * kRegsSoftmaxFp8 + kRegsProducerFp8) * 128 <= 384 * 168,
+              "setmaxnreg budget exceeds the CTA register pool");
+// kDenseFp8: the converter transposes every V tile (sixteen 4-byte rows live per unit) and the softmax warpgroups hold
+// P in 16 registers instead of 32 (2 x 224 + 56 = 504).
+constexpr uint32_t kRegsSoftmaxDenseFp8 = 224;
+constexpr uint32_t kRegsProducerDenseFp8 = 56;
+static_assert((2 * kRegsSoftmaxDenseFp8 + kRegsProducerDenseFp8) * 128 <= 384 * 168,
               "setmaxnreg budget exceeds the CTA register pool");
 
 // work item -> (batch*head, split, Q-tile pair).  CTAs are handed to SMs in blockIdx order (and the persistent kernel
@@ -352,22 +449,35 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   using F = Fp8Cfg<D>;
   constexpr int TILE = C::TILE_BYTES;
   constexpr int NSTAGE = FP8 ? F::NSTAGE : C::NSTAGE;          // 16-bit K/V ring depth
+  constexpr bool DF8 = MODE == kDenseFp8;                       // Q, K, V in e4m3 and 8-bit wgmma
+  using F8 = DenseFp8Cfg<D>;
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operands need 1024-byte alignment (the swizzle is a function of address bits 7..9)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                       // the item's two Q tiles: rows [0,64) tile 0, [64,128) tile 1
-  uint8_t* sStg = smem + TILE;              // epilogue staging, 128 rows x D 16-bit
+  uint8_t* sStg = smem + (DF8 ? F8::Q_BYTES : TILE);   // epilogue staging, 128 rows x D 16-bit
   uint8_t* sKV = smem + 2 * TILE;           // NSTAGE tiles
   // FP8: the raw e4m3 ring sits between the K/V ring and the barriers, its barriers after the others
   uint8_t* sRaw = sKV + NSTAGE * TILE;      // [NRAW] tiles of 128 keys x D bytes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + NSTAGE * TILE + (FP8 ? F::NRAW * F::RAW_BYTES : 0));
+  // kDenseFp8: the K, raw V and V^T rings after Q and the staging, their barriers after those
+  uint8_t* sK8 = smem + F8::Q_BYTES + TILE;
+  uint8_t* sRaw8 = sK8 + F8::NK * F8::TILE8;
+  uint8_t* sVt = sRaw8 + F8::NRAW * F8::TILE8;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(DF8 ? sVt + F8::NVT * F8::TILE8
+                                                   : sKV + NSTAGE * TILE + (FP8 ? F::NRAW * F::RAW_BYTES : 0));
   uint64_t* q_full = bars;
   uint64_t* q_empty = bars + 1;
   uint64_t* kv_full = bars + 2;             // [NSTAGE]
   uint64_t* kv_empty = kv_full + NSTAGE;    // [NSTAGE]
   uint64_t* raw_full = kv_empty + NSTAGE;   // [NRAW] (FP8 only)
   uint64_t* raw_empty = raw_full + F::NRAW; // [NRAW]
+  uint64_t* k_full = bars + 2;              // kDenseFp8: [NK]
+  uint64_t* k_empty = k_full + F8::NK;      // [NK]
+  uint64_t* raw8_full = k_empty + F8::NK;   // [NRAW]
+  uint64_t* raw8_empty = raw8_full + F8::NRAW;
+  uint64_t* vt_full = raw8_empty + F8::NRAW;   // [NVT]
+  uint64_t* vt_empty = vt_full + F8::NVT;      // [NVT]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -381,14 +491,29 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
     mbar_init(q_empty, 8);             // one arrival per softmax warp
-    for (int i = 0; i < NSTAGE; ++i) {
-      mbar_init(&kv_full[i], FP8 ? F::CONVERTER_WARPS : 1);   // FP8: one arrival per converter warp
-      mbar_init(&kv_empty[i], 8);
-    }
-    if constexpr (FP8) {
-      for (int i = 0; i < F::NRAW; ++i) {
-        mbar_init(&raw_full[i], 1);
-        mbar_init(&raw_empty[i], F::CONVERTER_WARPS);
+    if constexpr (DF8) {
+      for (int i = 0; i < F8::NK; ++i) {
+        mbar_init(&k_full[i], 1);
+        mbar_init(&k_empty[i], 8);
+      }
+      for (int i = 0; i < F8::NRAW; ++i) {
+        mbar_init(&raw8_full[i], 1);
+        mbar_init(&raw8_empty[i], F8::CONVERTER_WARPS);
+      }
+      for (int i = 0; i < F8::NVT; ++i) {
+        mbar_init(&vt_full[i], F8::CONVERTER_WARPS);       // one arrival per converter warp
+        mbar_init(&vt_empty[i], 8);
+      }
+    } else {
+      for (int i = 0; i < NSTAGE; ++i) {
+        mbar_init(&kv_full[i], FP8 ? F::CONVERTER_WARPS : 1);   // FP8: one arrival per converter warp
+        mbar_init(&kv_empty[i], 8);
+      }
+      if constexpr (FP8) {
+        for (int i = 0; i < F::NRAW; ++i) {
+          mbar_init(&raw_full[i], 1);
+          mbar_init(&raw_empty[i], F::CONVERTER_WARPS);
+        }
       }
     }
     fence_mbar_init();
@@ -397,7 +522,57 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
   if (warp < 4) {
     // =========================== TMA producer ===========================
-    setmaxnreg_dec<FP8 ? kRegsProducerFp8 : kRegsProducer>();
+    setmaxnreg_dec<DF8 ? kRegsProducerDenseFp8 : FP8 ? kRegsProducerFp8 : kRegsProducer>();
+    if constexpr (DF8) {
+      if (warp > 0) {
+        // ---- the converter (warps 1..3): raw V tile (128 keys x D bytes) -> V^T slot (D rows x 128 keys, keys in
+        // fp8_vt_key order, SWIZZLE_128B), walking the TMA lane's tiles.  Keys past Sk arrive as TMA's zero fill. ----
+        const int ct = threadIdx.x - 32;                          // 0 .. 95
+        uint32_t tile = 0;
+        for (int item = first; item < p.total_items; item += stride) {
+          const Item w = decode_item<CAUSAL, MODE>(item, p);
+#pragma unroll 1
+          for (int j = 0; j < w.n; ++j, ++tile) {
+            const uint32_t rslot = tile % F8::NRAW, vslot = tile % F8::NVT;
+            mbar_wait(&raw8_full[rslot], (tile / F8::NRAW) & 1, p.dbg, SITE_CONV_RAW, tile);
+            mbar_wait(&vt_empty[vslot], ((tile / F8::NVT) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
+            const uint32_t raw = smem_u32(sRaw8) + rslot * F8::TILE8;
+            const uint32_t dst = smem_u32(sVt) + vslot * F8::TILE8;
+#pragma unroll 1
+            for (int u = ct; u < 2 * D; u += 32 * F8::CONVERTER_WARPS) vt_convert_unit<D>(raw, dst, u);
+            fence_proxy_async_smem();                             // generic-proxy stores -> the wgmma's operand reads
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(&vt_full[vslot]);
+              mbar_arrive(&raw8_empty[rslot]);
+            }
+          }
+        }
+      } else if (lane == 0) {
+        // ---- the TMA lane: the item's Q (one 128-row box), then per KV tile K into the K ring and V raw ----
+        uint32_t tile = 0;     // running KV tile (never reset between items)
+        uint32_t qcnt = 0;
+        for (int item = first; item < p.total_items; item += stride) {
+          const Item w = decode_item<CAUSAL, MODE>(item, p);
+          if (w.n == 0) continue;
+          if (qcnt > 0) mbar_wait(q_empty, (qcnt - 1) & 1, p.dbg, SITE_LOAD_Q, qcnt);
+          ++qcnt;
+          mbar_arrive_expect_tx(q_full, F8::Q_BYTES);
+          tma_load_4d(sQ, &tmQ, q_full, 0, w.row0, w.hidx, w.bidx);
+          for (int j = 0; j < w.n; ++j, ++tile) {
+            const int ky = (w.jb + j) * C::BN;
+            const uint32_t kslot = tile % F8::NK, rslot = tile % F8::NRAW;
+            mbar_wait(&k_empty[kslot], ((tile / F8::NK) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
+            mbar_arrive_expect_tx(&k_full[kslot], F8::TILE8);
+            tma_load_4d(sK8 + kslot * F8::TILE8, &tmK, &k_full[kslot], 0, ky, w.hkv, w.bidx);
+            mbar_wait(&raw8_empty[rslot], ((tile / F8::NRAW) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
+            mbar_arrive_expect_tx(&raw8_full[rslot], F8::TILE8);
+            tma_load_4d(sRaw8 + rslot * F8::TILE8, &tmV, &raw8_full[rslot], 0, ky, w.hkv, w.bidx);
+          }
+        }
+      }
+      return;
+    }
     if constexpr (FP8) {
       if (warp > 0) {
         // ---- the converter (warps 1..3): raw ring entry -> 16-bit K/V ring slot, walking the TMA lane's entries ----
@@ -489,7 +664,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
 
   // ================= softmax / wgmma / epilogue warpgroup t =================
-  setmaxnreg_inc<FP8 ? kRegsSoftmaxFp8 : kRegsSoftmax>();
+  setmaxnreg_inc<DF8 ? kRegsSoftmaxDenseFp8 : FP8 ? kRegsSoftmaxFp8 : kRegsSoftmax>();
   using MmaS = Wgmma<128, IS_BF16>;
   using MmaO = Wgmma<D, IS_BF16>;
   const int t = (warp >> 2) - 1;                 // Q tile
@@ -510,21 +685,40 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const int row_lo = w.row0 + r_lo, row_hi = row_lo + 8;    // query rows of the sequence
 
     // S = Q K^T over D/16 k-steps; K-major operands advance 32 B per k-step inside a slab, one slab per 4 k-steps
+    // kDenseFp8: D/32 k-steps of 32 bytes inside the tile's D-byte rows (128-byte swizzle at D = 128, 64-byte at 64)
     auto issue_S = [&](float* s, uint32_t kslot) {
-      const uint32_t k_addr = sKV_addr + kslot * TILE;
+      if constexpr (DF8) {
+        const uint32_t q_addr = smem_u32(sQ) + t * 64 * D, k_addr = smem_u32(sK8) + kslot * F8::TILE8;
 #pragma unroll
-      for (int kk = 0; kk < D / 16; ++kk) {
-        const uint32_t off = (kk / 4) * C::SLAB_BYTES + (kk % 4) * 32;
-        MmaS::template ss<0>(s, gmma_desc(sQ_addr + off, 16, 1024), gmma_desc(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+        for (int kk = 0; kk < D / 32; ++kk) {
+          const uint64_t dq = D == 128 ? gmma_desc(q_addr + kk * 32, 16, 1024) : gmma_desc_sw64(q_addr + kk * 32, 512);
+          const uint64_t dk = D == 128 ? gmma_desc(k_addr + kk * 32, 16, 1024) : gmma_desc_sw64(k_addr + kk * 32, 512);
+          WgmmaE4m3<128>::ss(s, dq, dk, kk > 0 ? 1u : 0u);
+        }
+      } else {
+        const uint32_t k_addr = sKV_addr + kslot * TILE;
+#pragma unroll
+        for (int kk = 0; kk < D / 16; ++kk) {
+          const uint32_t off = (kk / 4) * C::SLAB_BYTES + (kk % 4) * 32;
+          MmaS::template ss<0>(s, gmma_desc(sQ_addr + off, 16, 1024), gmma_desc(k_addr + off, 16, 1024), kk > 0 ? 1u : 0u);
+        }
       }
       wgmma_commit();
     };
     // O += P V over 8 k-steps of 16 keys; V is MN-major: 16 key rows = 2048 B per k-step, LBO = next 64-column slab
+    // kDenseFp8: 4 k-steps of 32 keys; V^T is K-major, 32 B per k-step inside its 128-byte rows
     auto issue_PV = [&](float* o, const uint32_t* pf, uint32_t vslot, bool acc) {
-      const uint32_t v_addr = sKV_addr + vslot * TILE;
+      if constexpr (DF8) {
+        const uint32_t vt_addr = smem_u32(sVt) + vslot * F8::TILE8;
 #pragma unroll
-      for (int kk = 0; kk < C::BN / 16; ++kk)
-        MmaO::rs(o, pf + 4 * kk, gmma_desc(v_addr + kk * 2048, C::SLAB_BYTES, 1024), (acc || kk > 0) ? 1u : 0u);
+        for (int kk = 0; kk < C::BN / 32; ++kk)
+          WgmmaE4m3<D>::rs(o, pf + 4 * kk, gmma_desc(vt_addr + kk * 32, 16, 1024), (acc || kk > 0) ? 1u : 0u);
+      } else {
+        const uint32_t v_addr = sKV_addr + vslot * TILE;
+#pragma unroll
+        for (int kk = 0; kk < C::BN / 16; ++kk)
+          MmaO::rs(o, pf + 4 * kk, gmma_desc(v_addr + kk * 2048, C::SLAB_BYTES, 1024), (acc || kk > 0) ? 1u : 0u);
+      }
       wgmma_commit();
     };
     auto release = [&](uint64_t* bar) {
@@ -555,7 +749,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
     float s[64];             // S tile: 16 column groups of 8 keys x {row_lo: [0],[1], row_hi: [2],[3]}
     float o[D / 2];          // O tile, same layout over D columns
-    uint32_t pf[32];         // P as the A operand: 8 k-steps x 4 registers of 16-bit pairs
+    uint32_t pf[DF8 ? 16 : 32];   // P as the A operand: 8 k-steps x 4 registers of 16-bit pairs (e4m3: 4 x 4 of e4m3x4)
     float m_lo = 0.f, m_hi = 0.f;     // reference max the exponentials are taken against (raw score units)
     float l_lo = 0.f, l_hi = 0.f;     // this thread's part of the running sum of exp2((s - m) * c)
 #pragma unroll
@@ -619,18 +813,78 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
     };
     // P (fp32 accumulator layout) -> A-operand registers: k-step kk = column groups 2kk, 2kk+1
+    // kDenseFp8: P <= 2^8 < 448 (the lazy rescale's bound) is in e4m3 range
     auto pack_P = [&]() {
+      if constexpr (DF8) {
+        pack_p_e4m3(s, pf);
+      } else {
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        pf[4 * kk + 0] = pack_16x2<IS_BF16>(s[8 * kk + 0], s[8 * kk + 1]);
-        pf[4 * kk + 1] = pack_16x2<IS_BF16>(s[8 * kk + 2], s[8 * kk + 3]);
-        pf[4 * kk + 2] = pack_16x2<IS_BF16>(s[8 * kk + 4], s[8 * kk + 5]);
-        pf[4 * kk + 3] = pack_16x2<IS_BF16>(s[8 * kk + 6], s[8 * kk + 7]);
+        for (int kk = 0; kk < 8; ++kk) {
+          pf[4 * kk + 0] = pack_16x2<IS_BF16>(s[8 * kk + 0], s[8 * kk + 1]);
+          pf[4 * kk + 1] = pack_16x2<IS_BF16>(s[8 * kk + 2], s[8 * kk + 3]);
+          pf[4 * kk + 2] = pack_16x2<IS_BF16>(s[8 * kk + 4], s[8 * kk + 5]);
+          pf[4 * kk + 3] = pack_16x2<IS_BF16>(s[8 * kk + 6], s[8 * kk + 7]);
+        }
       }
     };
 
     // An item without tiles waits on no barrier: its rows get O = 0 and LSE = +inf (a split-KV partial: LSE = -inf).
-    if (n > 0) {
+    if (DF8 && n > 0) {
+      // kDenseFp8: K_j on k_full[(ent + j) % NK], V^T_j on vt_full[(ent + j) % NVT]; ent counts earlier items' tiles
+      mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
+      ++qcnt;
+      {
+        const uint32_t kslot = ent % F8::NK;
+        mbar_wait(&k_full[kslot], (ent / F8::NK) & 1, p.dbg, SITE_MMA_K, ent);
+        wgmma_fence();
+        issue_S(s, kslot);
+        wgmma_wait<0>();
+        reg_fence(s);
+        release(&k_empty[kslot]);
+        if (n == 1) release(q_empty);
+        bool rs;
+        float a0, a1;
+        softmax(0, rs, a0, a1);
+        pack_P();
+      }
+      for (int j = 1; j < n; ++j) {
+        const uint32_t ek = ent + j, ev = ent + j - 1;
+        const uint32_t kslot = ek % F8::NK, vslot = ev % F8::NVT;
+        mbar_wait(&k_full[kslot], (ek / F8::NK) & 1, p.dbg, SITE_MMA_K, ek);
+        wgmma_fence();
+        issue_S(s, kslot);
+        mbar_wait(&vt_full[vslot], (ev / F8::NVT) & 1, p.dbg, SITE_MMA_V, ev);
+        issue_PV(o, pf, vslot, j > 1);
+        wgmma_wait<1>();                               // S_j done
+        reg_fence(s);
+        release(&k_empty[kslot]);
+        if (j == n - 1) release(q_empty);
+        bool rs;
+        float a_lo, a_hi;
+        softmax(j, rs, a_lo, a_hi);
+        wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
+        reg_fence(o);
+        release(&vt_empty[vslot]);
+        if (rs) {
+#pragma unroll
+          for (int i = 0; i < D / 8; ++i) {
+            o[4 * i + 0] *= a_lo; o[4 * i + 1] *= a_lo;
+            o[4 * i + 2] *= a_hi; o[4 * i + 3] *= a_hi;
+          }
+        }
+        pack_P();
+      }
+      {
+        const uint32_t ev = ent + n - 1, vslot = ev % F8::NVT;
+        mbar_wait(&vt_full[vslot], (ev / F8::NVT) & 1, p.dbg, SITE_MMA_V, ev);
+        wgmma_fence();
+        issue_PV(o, pf, vslot, n > 1);
+        wgmma_wait<0>();
+        reg_fence(o);
+        release(&vt_empty[vslot]);
+      }
+      ent += n;
+    } else if (n > 0) {
       mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
       ++qcnt;
       // ---- KV tile 0 ----
@@ -698,7 +952,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
     float inv_lo = (l_lo > 0.f) ? 1.0f / l_lo : 0.f;
     float inv_hi = (l_hi > 0.f) ? 1.0f / l_hi : 0.f;
-    if constexpr (FP8) {          // V = v_scale * V8: O = (P V8 / l) * v_scale; a split's partial too (the combine is linear)
+    if constexpr (FP8 || DF8) {   // V = v_scale * V8: O = (P V8 / l) * v_scale; a split's partial too (the combine is linear)
       inv_lo *= p.v_scale;
       inv_hi *= p.v_scale;
     }

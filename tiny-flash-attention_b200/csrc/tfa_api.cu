@@ -40,6 +40,11 @@ extern template cudaError_t tfa::launch_forward<tfa::kVarlenCacheFp8>(int D, boo
                                                                       const CUtensorMap& tq, const CUtensorMap& tk,
                                                                       const CUtensorMap& tv, const tfa::FwdParams& p,
                                                                       int nblocks, bool persist, cudaStream_t stream);
+// tfa_fp8_fwd.cu: the FP8 attention forward, compiled apart from the other forward kernels
+extern template cudaError_t tfa::launch_forward<tfa::kDenseFp8>(int D, bool causal, bool bf16, bool f32,
+                                                                const CUtensorMap& tq, const CUtensorMap& tk,
+                                                                const CUtensorMap& tv, const tfa::FwdParams& p,
+                                                                int nblocks, bool persist, cudaStream_t stream);
 
 namespace {
 
@@ -83,9 +88,14 @@ void init_dbg() {
 // (B?,H?,S,D)-strided 16-bit tensor -> 4-D tiled map with dims (D, S, H, B); the kernel addresses it as
 // (x = head-dim offset, y = sequence row, z = head, w = batch).  Box = 64 x 128 elements, SWIZZLE_128B.
 // dtype TFA_FP8_E4M3: a 1-byte (e4m3) cache, box = D x 128 bytes, unswizzled (the converter reads it row by row).
+// `operand8`: a 1-byte tensor the 8-bit wgmma reads in place (kDenseFp8's Q and K), box = D x 128 bytes with the swizzle
+// that matches its D-byte rows, SWIZZLE_128B (D = 128) or SWIZZLE_64B (D = 64).
 int make_tmap(CUtensorMap* m, const void* base, int dtype, int D, int S, int B, int H, long long sb,
-              long long sh, long long ss) {
+              long long sh, long long ss, bool operand8 = false) {
   const bool fp8 = dtype == TFA_FP8_E4M3;
+  const CUtensorMapSwizzle swz = !fp8 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                 : !operand8 ? CU_TENSOR_MAP_SWIZZLE_NONE
+                                 : D == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   const int box_rows = 128, box_cols = fp8 ? D : 64;
   const cuuint64_t esz = fp8 ? 1 : 2;
   auto encode = get_encode_fn();
@@ -104,9 +114,8 @@ int make_tmap(CUtensorMap* m, const void* base, int dtype, int D, int S, int B, 
   const cuuint64_t strides[3] = {s1, s2, s3};
   for (int i = 0; i < 3; ++i)
     if ((strides[i] % 16) || strides[i] >= (1ull << 40)) return TFA_EINVAL_STRIDE;
-  CUresult r = encode(m, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      fp8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = encode(m, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : TFA_EDRIVER;
 }
 
@@ -371,6 +380,48 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   cp.H = a.Hq; cp.S = S;
   cp.nsplit = plan.nsplit;
   return (a.D == 64) ? launch_combine<64>(cp, bf16, f32, a.stream) : launch_combine<128>(cp, bf16, f32, a.stream);
+}
+
+// The FP8-attention arguments of a call whose 16-bit checks passed: the element type, the scales and q / k / v strides
+// that keep every 1-byte TMA row and box 16-byte aligned.  Sets a.scale to s' = fp32(fp32(softmax_scale * q_scale) *
+// k_scale), which must stay a normal fp32 number (or 0 with softmax_scale = 0), as validate_quant's s'.
+int validate_qkv_quant(const tfa_qkv_quant_args& q, Problem& a) {
+  if (q.qkv_dtype != TFA_FP8_E4M3) return TFA_EINVAL_QKVQUANT;
+  for (const float x : {q.q_scale, q.k_scale, q.v_scale})
+    if (!(x > 0.0f) || !std::isfinite(x)) return TFA_EINVAL_QKVQUANT;
+  if ((a.qsb % 16) || (a.qsh % 16) || (a.qss % 16) || (a.ksb % 16) || (a.ksh % 16) || (a.kss % 16))
+    return TFA_EINVAL_QKVQUANT;
+  const float qs = a.scale * q.q_scale;
+  const float s = qs * q.k_scale;
+  if (!(s <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
+  a.scale = s;
+  return 0;
+}
+
+// The dense problem of tfa_attn_fwd() on e4m3 q / k / v: its checks in its order, then the quantization's, then the
+// kDenseFp8 forward over 8-bit swizzled Q / K maps and the raw V map the converter transposes.
+int fp8_impl(Problem a, const tfa_qkv_quant_args& quant) {
+  int rc = validate(a);
+  if (rc) return rc;
+  if ((rc = validate_qkv_quant(quant, a))) return rc;
+  if (!arch_ok()) return TFA_EARCH;
+  init_dbg();
+
+  SplitPlan plan;
+  if ((rc = plan_splits(a, plan))) return rc;
+
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, TFA_FP8_E4M3, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, true))) return rc;
+  if ((rc = make_tmap(&tk, a.k, TFA_FP8_E4M3, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss, true))) return rc;
+  if ((rc = make_tmap(&tv, a.v, TFA_FP8_E4M3, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+
+  FwdParams p{};
+  p.Sk = a.Sk;
+  p.causal_off = a.causal ? a.Sk - a.Sq : 0;
+  p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
+  p.v_scale = quant.v_scale;
+  return run_forward<tfa::kDenseFp8>(a, p, a.Sq, tq, tk, tv, plan);
 }
 
 int fwd_impl(const Problem& a, void* const* extra_dst = nullptr, int n_extra = 0) {
@@ -745,6 +796,11 @@ int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, co
   return varlen_kvcache_impl(*args, quant);
 }
 
+int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return fp8_impl(from_attn_args(*args), *quant);
+}
+
 int tfa_attn_num_splits(const tfa_attn_args* args) {
   if (!args) return 1;
   const Problem a = from_attn_args(*args);
@@ -907,6 +963,12 @@ long long tfa_internal_varlen_append_offset(int raw, const int* block_table, lon
 int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {
   return tfa::rotary_pos(cache_len, i, causal != 0, is_query != 0, seqlen_ro);
 }
+// development aid (not in the public header): kDenseFp8's key order of P (fa_fwd_sm90.cuh) on the host -- pi of a
+// 32-key block's A column, the accumulator element the packer puts into byte x of A register r, and the key the
+// converter writes at position p of a V^T row
+int tfa_internal_fp8_p_key(int c) { return tfa::fp8_p_key(c); }
+int tfa_internal_fp8_pack_src(int r, int x) { return tfa::fp8_pack_src(r, x); }
+int tfa_internal_fp8_vt_key(int p) { return tfa::fp8_vt_key(p); }
 
 int tfa_debug_record(unsigned int out[8]) {
   if (!out) return TFA_EINVAL_PTR;
@@ -943,6 +1005,9 @@ const char* tfa_error_string(int code) {
     case TFA_EINVAL_KVQUANT:
       return "tfa: an FP8 cache needs cache_dtype TFA_FP8_E4M3 (2), finite k_scale and v_scale > 0, and cache strides "
              "that are multiples of 16 elements";
+    case TFA_EINVAL_QKVQUANT:
+      return "tfa: FP8 attention needs qkv_dtype TFA_FP8_E4M3 (2), finite q_scale, k_scale and v_scale > 0, and q / k / v "
+             "strides that are multiples of 16 elements";
     default: return code > 0 ? cudaGetErrorString(static_cast<cudaError_t>(code)) : "tfa: unknown error";
   }
 }

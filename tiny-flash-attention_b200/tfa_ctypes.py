@@ -106,6 +106,12 @@ class KvQuantArgs(ctypes.Structure):
     _fields_ = [("cache_dtype", ctypes.c_int32), ("k_scale", ctypes.c_float), ("v_scale", ctypes.c_float)]
 
 
+class QkvQuantArgs(ctypes.Structure):
+    """struct tfa_qkv_quant_args (include/tfa_b200.h)."""
+    _fields_ = [("qkv_dtype", ctypes.c_int32), ("q_scale", ctypes.c_float), ("k_scale", ctypes.c_float),
+                ("v_scale", ctypes.c_float)]
+
+
 class RotaryArgs(ctypes.Structure):
     """struct tfa_rotary_args (include/tfa_b200.h)."""
     _fields_ = [
@@ -148,6 +154,10 @@ def lib():
         L.tfa_attn_kvcache_fp8_fwd.restype = ci
         L.tfa_attn_varlen_kvcache_fp8_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(KvQuantArgs)]
         L.tfa_attn_varlen_kvcache_fp8_fwd.restype = ci
+        L.tfa_attn_fp8_fwd.argtypes = [ctypes.POINTER(AttnArgs), ctypes.POINTER(QkvQuantArgs)]
+        L.tfa_attn_fp8_fwd.restype = ci
+        L.tfa_selftest_wgmma_fp8.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp]
+        L.tfa_selftest_wgmma_fp8.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
         L.tfa_fwd_host.restype = ci
         L.tfa_host_release.restype = None
@@ -226,27 +236,49 @@ def _split_workspace(dense, args, device, stream):
     return n
 
 
+def _qkv_quant(q, q_scale, k_scale, v_scale, out_dtype):
+    """(tfa_qkv_quant_args, output dtype) for float8_e4m3fn q / k / v, or (None, q's dtype) for 16-bit ones, which
+    take no scales."""
+    import torch
+    if q.dtype != torch.float8_e4m3fn:
+        if (q_scale, k_scale, v_scale) != (1.0, 1.0, 1.0) or out_dtype not in (None, q.dtype):
+            raise ValueError(f"q_scale / k_scale / v_scale / out_dtype apply to float8_e4m3fn inputs only; q is {q.dtype}")
+        return None, q.dtype
+    if out_dtype not in (torch.bfloat16, torch.float16):
+        raise TypeError(f"float8_e4m3fn inputs need out_dtype bfloat16 or float16, got {out_dtype}")
+    return QkvQuantArgs(TFA_FP8_E4M3, float(q_scale), float(k_scale), float(v_scale)), out_dtype
+
+
 def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, stream=None, return_splits=False,
-             out=None, lse=None):
+             out=None, lse=None, q_scale=1.0, k_scale=1.0, v_scale=1.0, out_dtype=None):
     """Generalised problem through tfa_attn_fwd(): q (B,Hq,Sq,D), k/v (B,Hkv,Sk,D) contiguous device tensors,
     bottom-right causal mask, optional split-KV (num_splits: 1 none, n > 1 as asked, 0 library heuristic).  `out`
-    (contiguous, q's shape) / `lse` (contiguous (B, Hq, Sq) fp32) may be given to write into caller-owned buffers."""
+    (contiguous, q's shape) / `lse` (contiguous (B, Hq, Sq) fp32) may be given to write into caller-owned buffers.
+    torch.float8_e4m3fn q / k / v go through tfa_attn_fp8_fwd() with the per-tensor q_scale / k_scale / v_scale and
+    the output dtype out_dtype (bfloat16 or float16)."""
     import torch
     assert q.is_cuda and q.is_contiguous() and k.is_contiguous() and v.is_contiguous()
     B, Hq, Sq, D = q.shape
     _, Hkv, Sk, _ = k.shape
+    if not (q.dtype == k.dtype == v.dtype):
+        raise TypeError(f"q, k and v must share one dtype, got {q.dtype}, {k.dtype}, {v.dtype}")
+    quant, odt = _qkv_quant(q, q_scale, k_scale, v_scale, out_dtype)
     if out is None:
-        out = torch.empty(q.shape, dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+        out = torch.empty(q.shape, dtype=torch.float32 if out_fp32 else odt, device=q.device)
     if lse is None:
         lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=q.device)
-    assert out.shape == q.shape and out.is_contiguous() and out.dtype == (torch.float32 if out_fp32 else q.dtype)
+    assert out.shape == q.shape and out.is_contiguous() and out.dtype == (torch.float32 if out_fp32 else odt)
     assert lse.shape == (B, Hq, Sq) and lse.is_contiguous() and lse.dtype == torch.float32
     st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
     a = AttnArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), B, Hq, Hkv, Sq, Sk, D,
-                 Hq * Sq * D, Sq * D, D, Hkv * Sk * D, Sk * D, D, _dtype_code(q), int(bool(is_causal)),
-                 float(softmax_scale), int(bool(out_fp32)), int(num_splits), None, 0, st)
+                 Hq * Sq * D, Sq * D, D, Hkv * Sk * D, Sk * D, D,
+                 (TFA_BF16 if odt == torch.bfloat16 else TFA_FP16) if quant else _dtype_code(q),
+                 int(bool(is_causal)), float(softmax_scale), int(bool(out_fp32)), int(num_splits), None, 0, st)
     n = _split_workspace(a, a, q.device, st)
-    check(lib().tfa_attn_fwd(ctypes.byref(a)))
+    if quant is not None:
+        check(lib().tfa_attn_fp8_fwd(ctypes.byref(a), ctypes.byref(quant)))
+    else:
+        check(lib().tfa_attn_fwd(ctypes.byref(a)))
     if return_splits:
         return out, lse, n
     return out, lse
