@@ -390,6 +390,26 @@ typedef struct tfa_qkv_quant_args {
 
 int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant);
 
+/* ---- the variable-length batch on FP8 (e4m3) q, k and v with per-tensor scales (FlashAttention-3's
+ * flash_attn_varlen_func with descale_q / descale_k / descale_v) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_varlen_fp8_fwd.  The problem of tfa_attn_varlen_fwd(), unchanged -- packed q (total_q, Hq, D) and k / v
+ * (total_k, Hkv, D), cu_seqlens_q / cu_seqlens_k read on the device only, grouped K/V heads, the bottom-right causal
+ * mask per sequence, key-less rows out = 0 / lse = +inf, rows beyond max_seqlen_q untouched, out_fp32, no split-KV --
+ * with q, k and v holding one byte per element, and the arithmetic and scales of tfa_attn_fp8_fwd().
+ *
+ *   q, k, v  : e4m3 codes (torch.float8_e4m3fn).  Strides are in elements, so in bytes, and must be multiples of 16.
+ *   dtype    : the OUTPUT dtype, TFA_BF16 or TFA_FP16 (or fp32 with out_fp32).  out is (total_q, Hq, D) contiguous;
+ *              lse is fp32 (Hq, total_q) as for tfa_attn_varlen_fwd().
+ *   scales   : as tfa_attn_fp8_fwd(): s' = fp32(fp32(softmax_scale * q_scale) * k_scale), P rounded to e4m3, O multiplied
+ *              by v_scale.  Each sequence's out and lse are bit-identical to tfa_attn_fp8_fwd() (num_splits = 1) on that
+ *              sequence alone; the keys of the neighbouring sequences may hold any byte, NaN codes 0x7f / 0xff included,
+ *              and do not change the result.
+ * Every check runs before any device work: those of tfa_attn_varlen_fwd() first, in its order, then
+ * TFA_EINVAL_QKVQUANT, then TFA_EINVAL_SCALE for s'.  Launches: 1.  Nothing is read back to the host: the call can be
+ * captured in a CUDA graph and replayed with new cu_seqlens contents of the same totals. */
+int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant);
+
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on
  * `n_streams` internal streams so H2D, compute and D2H overlap, copies out, and

@@ -33,7 +33,8 @@ vt_empty one per warpgroup).  Tile j of the running tile count takes slot j % de
 warps are roles of their own: each waits on the tile's raw_full and its V^T slot's vt_empty, stores its part (spanning
 a scheduling point), then arrives on vt_full and raw_empty.  Shadow state adds: a V^T slot read by a wgmma before every
 converter warp's part of that tile is stored, or while one still stores into it, and a converter warp storing into a
-slot a wgmma still reads.
+slot a wgmma still reads.  With `empty` (kVarlenFp8) an item without tiles is written only when listed there; the
+others lie past their sequence's end and every role skips them, as in Sim.
 
 Run:  python scripts/protocol_model.py [trials]      (exit code 0 = no violation found)
 """
@@ -283,12 +284,13 @@ class Sim:
 
 
 class DenseFp8Sim:
-    """kDenseFp8: the TMA lane (Q, K, raw V), three converter warps (raw V -> V^T) and the two softmax warpgroups."""
+    """kDenseFp8 / kVarlenFp8: the TMA lane (Q, K, raw V), three converter warps (raw V -> V^T) and the two softmax
+    warpgroups.  `empty` as Sim's: the tile-less items whose rows are written (default: every one)."""
     WARPS = 3                                                 # converter warps (producer warps 1-3)
 
-    def __init__(self, items, nk, nraw, nvt, rng):
+    def __init__(self, items, nk, nraw, nvt, rng, empty=None):
         self.items, self.NK, self.R, self.V, self.rng = items, nk, nraw, nvt, rng
-        self.empty = {i for i, n in enumerate(items) if n == 0}
+        self.empty = {i for i, n in enumerate(items) if n == 0} if empty is None else set(empty)
         self.q_full, self.q_empty = Bar("q_full", 1), Bar("q_empty", 2)
         self.k_full = [Bar(f"k_full{i}", 1) for i in range(nk)]
         self.k_empty = [Bar(f"k_empty{i}", 2) for i in range(nk)]
@@ -410,9 +412,10 @@ class DenseFp8Sim:
 
         for item, n in enumerate(self.items):
             if n == 0:
-                yield lambda: True                            # epilogue only: no barrier is touched
-                self.finished[t].append(item)
-                continue
+                if item in self.empty:                        # live without tiles: epilogue only, no barrier
+                    yield lambda: True
+                    self.finished[t].append(item)
+                continue                                      # else past its sequence's end: skipped
             yield lambda p=qcnt & 1: self.q_full.done(p)
             qcnt += 1
             yield from wait_k(ent)
@@ -466,7 +469,7 @@ class DenseFp8Sim:
         else:
             raise AssertionError("did not finish")
         want = [(it, j) for it, n in enumerate(self.items) for j in range(n)]
-        done = list(range(len(self.items)))
+        done = [it for it, n in enumerate(self.items) if n > 0 or it in self.empty]
         for t in range(2):
             assert self.seen[t] == want, f"wg{t} consumed {self.seen[t]}, expected {want}"
             assert self.finished[t] == done
@@ -477,6 +480,15 @@ def random_dense_fp8(rng):
     among them."""
     depths = rng.choice([(4, 3, 4), (8, 4, 8), (1, 1, 1), (2, 3, 1), (3, 1, 2)])
     return random_items(rng), depths
+
+
+def random_varlen_fp8(rng):
+    """kVarlenFp8: the items of a packed batch as random_varlen_items draws them -- past a sequence's end (skipped by
+    every role), inside it without a key (causal Sq_b > Sk_b, or Sk_b = 0: written without a barrier), with tiles --
+    and ring depths as random_dense_fp8.  Returns (items, empty, depths)."""
+    depths = rng.choice([(4, 3, 4), (8, 4, 8), (1, 1, 1), (2, 3, 1), (3, 1, 2)])
+    items, empty = random_varlen_items(rng)
+    return items, empty, depths
 
 
 def random_items(rng):
@@ -572,6 +584,9 @@ def main():
         rng8 = random.Random(2000003 + trial)             # kDenseFp8, on a generator of its own
         items, depths = random_dense_fp8(rng8)
         DenseFp8Sim(items, *depths, rng8).run()
+        rngv = random.Random(3000003 + trial)             # kVarlenFp8, on a generator of its own
+        items, empty, depths = random_varlen_fp8(rngv)
+        DenseFp8Sim(items, *depths, rngv, empty).run()
     print(f"{trials} trials: no violation")
 
 

@@ -34,7 +34,7 @@ LIB_NAME = "libtfa_b200.so"
 EXT_NAME = "attention_cutlass" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so")
 
 CU_SOURCES = ["tfa_api.cu", "tfa_append.cu", "tfa_varlen_kvcache.cu", "tfa_kvcache_fp8.cu", "tfa_fp8_fwd.cu",
-              "tfa_selftest.cu", "tfa_selftest_fp8.cu"]
+              "tfa_varlen_fp8.cu", "tfa_selftest.cu", "tfa_selftest_fp8.cu"]
 CU_HEADERS = ["ptx_sm90.cuh", "fa_fwd_sm90.cuh", "fa_fwd_launch.cuh", "fa_splitkv_combine.cuh", "fa_kvcache_append.cuh"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [

@@ -325,6 +325,75 @@ std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Ten
   return {out, lse};
 }
 
+// FP8 variable-length batch (tfa_attn_varlen_fp8_fwd): q, k, v as flash_attention_v2_varlen but float8_e4m3fn, with the
+// per-tensor scales their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is
+// the output's.  Returns out (total_q, Hq, D) contiguous and lse (Hq, total_q).
+std::vector<torch::Tensor> flash_attention_v2_varlen_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v,
+                                                         torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
+                                                         int64_t max_seqlen_q, double q_scale, double k_scale,
+                                                         double v_scale, bool is_causal, float softmax_scale,
+                                                         at::ScalarType out_dtype) {
+  // the element types and devices first, then the CUDA checks: a wrong dtype is reported as such wherever q lives
+  TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3, "q, k, v must have 3 dimensions (total, heads, head_dim)");
+  TORCH_CHECK(q.scalar_type() == at::kFloat8_e4m3fn && k.scalar_type() == at::kFloat8_e4m3fn &&
+              v.scalar_type() == at::kFloat8_e4m3fn, "q, k, v must be float8_e4m3fn");
+  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf, "out_dtype must be bfloat16 or float16");
+  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
+  TFA_CHECK_CUDA(q);
+  TORCH_CHECK(k.sizes() == v.sizes() && k.strides() == v.strides(), "k and v must have identical shapes and strides");
+  TORCH_CHECK(k.size(2) == q.size(2), "k/v must share head_dim with q");
+  TORCH_CHECK(q.stride(2) == 1 && k.stride(2) == 1, "q, k, v must have a unit head_dim stride");
+  TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt && cu_seqlens_k.scalar_type() == at::kInt,
+              "cu_seqlens_q and cu_seqlens_k must be int32");
+  TORCH_CHECK(cu_seqlens_q.device() == q.device() && cu_seqlens_k.device() == q.device(),
+              "cu_seqlens_q and cu_seqlens_k must be on q's device");
+  TORCH_CHECK(cu_seqlens_q.dim() == 1 && cu_seqlens_q.is_contiguous() && cu_seqlens_k.dim() == 1 &&
+                  cu_seqlens_k.is_contiguous(),
+              "cu_seqlens_q and cu_seqlens_k must be contiguous 1-D tensors");
+  TORCH_CHECK(cu_seqlens_q.numel() >= 2 && cu_seqlens_k.numel() == cu_seqlens_q.numel(),
+              fmt_msg("cu_seqlens_q and cu_seqlens_k must both hold B + 1 >= 2 offsets, got %lld and %lld",
+                      static_cast<long long>(cu_seqlens_q.numel()), static_cast<long long>(cu_seqlens_k.numel())));
+  const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2), total_k = k.size(0), Hkv = k.size(1);
+  const int64_t B = cu_seqlens_q.numel() - 1;
+  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
+  TORCH_CHECK(total_q >= 1 && total_k >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
+  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
+                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
+  TORCH_CHECK(max_seqlen_q >= 1 && max_seqlen_q <= total_q,
+              fmt_msg("max_seqlen_q must be in [1, total_q = %lld], got %lld", static_cast<long long>(total_q),
+                      static_cast<long long>(max_seqlen_q)));
+  TORCH_CHECK(total_q < (1LL << 31) && total_k < (1LL << 31) && B < (1LL << 31), "tensors too large");
+
+  torch::Tensor out, lse;
+  int rc = 0;
+  {
+    c10::cuda::CUDAGuard guard(q.device());
+    out = torch::empty({total_q, Hq, D}, q.options().dtype(out_dtype));
+    lse = torch::empty({Hq, total_q}, q.options().dtype(at::kFloat));
+    tfa_attn_varlen_args a;
+    a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
+    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
+    a.cu_seqlens_q = cu_seqlens_q.data_ptr<int32_t>();
+    a.cu_seqlens_k = cu_seqlens_k.data_ptr<int32_t>();
+    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
+    a.D = static_cast<int32_t>(D);
+    a.total_q = static_cast<int32_t>(total_q); a.total_k = static_cast<int32_t>(total_k);
+    a.max_seqlen_q = static_cast<int32_t>(max_seqlen_q);
+    a.q_stride_s = q.stride(0); a.q_stride_h = q.stride(1);
+    a.kv_stride_s = k.stride(0); a.kv_stride_h = k.stride(1);
+    a.dtype = out_dtype == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.is_causal = is_causal ? 1 : 0;
+    a.softmax_scale = softmax_scale;
+    a.out_fp32 = 0;
+    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
+                          static_cast<float>(v_scale)};
+    rc = tfa_attn_varlen_fp8_fwd(&a, &qa);
+  }
+  raise_on_error(rc);
+  return {out, lse};
+}
+
 namespace {
 
 // The cache's shape as the cache entry points pass it to the library.
@@ -678,6 +747,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"), py::arg("num_splits") = 1);
   m.def("flash_attention_v2_varlen", &flash_attention_v2_varlen,
         "packed variable-length batch: (q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, scale)");
+  m.def("flash_attention_v2_varlen_fp8", &flash_attention_v2_varlen_fp8,
+        "FP8 packed variable-length batch: float8_e4m3fn q, k, v with per-tensor scales, e4m3 tensor cores -> [out "
+        "(out_dtype), lse]",
+        py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_seqlens_q"), py::arg("cu_seqlens_k"),
+        py::arg("max_seqlen_q"), py::arg("q_scale"), py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"),
+        py::arg("softmax_scale"), py::arg("out_dtype"));
   m.def("flash_attention_v2_kvcache", &flash_attention_v2_kvcache,
         "attention against a (paged) KV cache with an optional in-place append: (q, k_cache, v_cache, cache_seqlens, "
         "block_table, k_new, v_new, is_causal, scale, num_splits)");

@@ -3,8 +3,9 @@
 // dispatch.  The caller sizes the grid and counts the launch.
 //
 // tfa_varlen_kvcache.cu explicitly instantiates launch_forward<kVarlenCache>, tfa_kvcache_fp8.cu launch_forward<
-// kCacheFp8> and launch_forward<kVarlenCacheFp8>, and tfa_api.cu declares those instantiations `extern template`, so
-// that each mode's 32 kernels are compiled in that unit only (the comment there says why).
+// kCacheFp8> and launch_forward<kVarlenCacheFp8>, tfa_fp8_fwd.cu launch_forward<kDenseFp8> and tfa_varlen_fp8.cu
+// launch_forward<kVarlenFp8>, and tfa_api.cu declares those instantiations `extern template`, so that each mode's 32
+// kernels are compiled in that unit only (the comment there says why).
 #pragma once
 #include "fa_fwd_sm90.cuh"
 

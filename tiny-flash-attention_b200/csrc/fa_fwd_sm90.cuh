@@ -37,19 +37,24 @@
 // both at once, a packed variable-length batch of queries (cu_seqlens) against a (paged) KV cache.  kCacheFp8 and
 // kVarlenCacheFp8 are kCache and kVarlenCache against an FP8 (e4m3) cache: the TMA lane loads raw e4m3 tiles into a
 // ring of their own, and producer warps 1-3 (the converter) widen each into the 16-bit K/V ring slot the softmax
-// warpgroups read, exactly, in the layout TMA gives a 16-bit tile; their code does not change.
+// warpgroups read, exactly, in the layout TMA gives a 16-bit tile; their code does not change.  kDenseFp8 and
+// kVarlenFp8 are kDense and kVarlen with Q, K and V in e4m3 and both products on 8-bit wgmma (qkv8_mode()).
 #pragma once
 #include "ptx_sm90.cuh"
 
 namespace tfa {
 
-enum : int { kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5, kDenseFp8 = 6 };
+enum : int {
+  kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5, kDenseFp8 = 6, kVarlenFp8 = 7
+};
 // The problem an FP8-cache mode solves is that of its 16-bit mode: they differ only in how K/V reach the ring.
 __host__ __device__ constexpr bool fp8_mode(int mode) { return mode == kCacheFp8 || mode == kVarlenCacheFp8; }
-// kDenseFp8 solves the dense problem with Q, K and V in e4m3 and both products on 8-bit wgmma (fp8_mode() is false
-// for it: that predicate means "widen K/V to 16 bits").
+// kDenseFp8 / kVarlenFp8 solve the dense / varlen problem with Q, K and V in e4m3 and both products on 8-bit wgmma
+// (fp8_mode() is false for them: that predicate means "widen K/V to 16 bits").
+__host__ __device__ constexpr bool qkv8_mode(int mode) { return mode == kDenseFp8 || mode == kVarlenFp8; }
 __host__ __device__ constexpr int base_mode(int mode) {
-  return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode == kDenseFp8 ? kDense : mode;
+  return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode == kDenseFp8 ? kDense
+       : mode == kVarlenFp8 ? kVarlen : mode;
 }
 
 // ---- kDenseFp8: P as the 8-bit A operand without shuffles ----
@@ -215,7 +220,7 @@ struct Fp8Cfg {
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a block may use");
   static constexpr int CONVERTER_WARPS = 3;   // producer warps 1..3
 };
-// Shared-memory plan of kDenseFp8: Q (128 rows x D bytes), the 16-bit O staging of FwdCfg, then three rings of
+// Shared-memory plan of kDenseFp8 and kVarlenFp8: Q (128 rows x D bytes), the 16-bit O staging of FwdCfg, then three rings of
 // 128 x D-byte tiles -- K (filled by TMA, SWIZZLE_128B at D = 128, SWIZZLE_64B at D = 64), raw V (unswizzled, as TMA
 // loads it) and V^T (D rows x 128 keys, SWIZZLE_128B, written by the converter) -- then the barriers: q_full, q_empty,
 // k_full / k_empty[NK], raw_full / raw_empty[NRAW], vt_full / vt_empty[NVT].  Each ring has its own barriers, so each
@@ -247,7 +252,7 @@ struct DenseFp8Cfg {
 };
 template <int D, int MODE>
 __host__ __device__ constexpr int fwd_smem_bytes() {
-  return MODE == kDenseFp8 ? DenseFp8Cfg<D>::SMEM_BYTES : fp8_mode(MODE) ? Fp8Cfg<D>::SMEM_BYTES : FwdCfg<D>::SMEM_BYTES;
+  return qkv8_mode(MODE) ? DenseFp8Cfg<D>::SMEM_BYTES : fp8_mode(MODE) ? Fp8Cfg<D>::SMEM_BYTES : FwdCfg<D>::SMEM_BYTES;
 }
 
 // 8 e4m3 codes (bytes of r, element 0 in the low byte of r.x) -> 8 16-bit values, exactly: the code's sign and its
@@ -275,18 +280,26 @@ __device__ __forceinline__ uint4 widen_e4m3x8(uint2 r) {
   return make_uint4(out[0], out[1], out[2], out[3]);
 }
 
-// kDenseFp8's converter, one unit u (0 <= u < 2 D) of a tile: keys [16 kc, 16 kc + 16) -- one 16-byte chunk of every
+// The converter of kDenseFp8 / kVarlenFp8, one unit u (0 <= u < 2 D) of a tile: keys [16 kc, 16 kc + 16) -- one 16-byte chunk of every
 // V^T row -- x columns [4 dc, 4 dc + 4) of the raw tile at `raw` (128 keys x D bytes, row-major) into the V^T slot at
 // `dst` (D rows x 128 keys, positions in fp8_vt_key order, SWIZZLE_128B).  Consecutive units take two chunks x 16
 // columns per warp: its loads hit two rows per bank, its stores (8 lanes: four chunks x two rows) distinct bank groups.
-template <int D>
-__device__ __forceinline__ void vt_convert_unit(uint32_t raw, uint32_t dst, int u) {
+// TAIL (kVarlenFp8): keys >= `valid` are written as zeros -- in a packed tile they are the next sequence's, any byte.
+template <int D, bool TAIL = false>
+__device__ __forceinline__ void vt_convert_unit(uint32_t raw, uint32_t dst, int u, int valid = 128) {
   constexpr int DC = D / 4;
   const int kc = 2 * (u / (2 * DC)) + (u & 1), dc = (u >> 1) % DC;
   uint32_t L[16];                                     // L[k] = columns 4 dc .. +3 of key 16 kc + k
 #pragma unroll
   for (int k = 0; k < 16; ++k)
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(L[k]) : "r"(raw + (16 * kc + k) * D + 4 * dc));
+  if constexpr (TAIL) {
+    if (16 * kc + 16 > valid) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (16 * kc + k >= valid) L[k] = 0u;
+    }
+  }
   // row 4 dc + e, positions 16 kc + 4 x4 + x: key fp8_vt_key(16 kc + 4 x4 + x) = 16 kc + fp8_p_key(4 x4 + x), byte e
   // (one row at a time: the converter runs on kRegsProducerFp8 registers)
 #pragma unroll
@@ -401,6 +414,9 @@ __device__ __forceinline__ Item decode_item(int item, const FwdParams& p) {
     w.Sq = max(q1 - q0, 0);
     w.Sk = max(k1 - k0, 0);
     w.coff = w.Sk - w.Sq;           // may be negative: the sequence's first rows see no key
+    // kVarlenFp8 stores only the rows the header promises, the first max_seqlen_q = S (the grid covers up to the next
+    // multiple of 128); the causal offset stays that of all Sq_b rows, as for kVarlen
+    if constexpr (MODE == kVarlenFp8) w.Sq = min(w.Sq, p.S);
   } else if constexpr (M == kCache) {
     w.q0 = 0;
     w.k0 = 0;
@@ -449,7 +465,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   using F = Fp8Cfg<D>;
   constexpr int TILE = C::TILE_BYTES;
   constexpr int NSTAGE = FP8 ? F::NSTAGE : C::NSTAGE;          // 16-bit K/V ring depth
-  constexpr bool DF8 = MODE == kDenseFp8;                       // Q, K, V in e4m3 and 8-bit wgmma
+  constexpr bool DF8 = qkv8_mode(MODE);                         // Q, K, V in e4m3 and 8-bit wgmma
   using F8 = DenseFp8Cfg<D>;
 
   extern __shared__ uint8_t smem_raw[];
@@ -526,7 +542,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     if constexpr (DF8) {
       if (warp > 0) {
         // ---- the converter (warps 1..3): raw V tile (128 keys x D bytes) -> V^T slot (D rows x 128 keys, keys in
-        // fp8_vt_key order, SWIZZLE_128B), walking the TMA lane's tiles.  Keys past Sk arrive as TMA's zero fill. ----
+        // fp8_vt_key order, SWIZZLE_128B), walking the TMA lane's tiles.  Dense: keys past Sk arrive as TMA's zero fill.
+        // Packed: they are the next sequence's keys, any byte, NaN codes included (P = 0 does not cancel 0 * NaN), so
+        // they are written as zeros, which also makes a sequence's result that of the dense call on it alone. ----
         const int ct = threadIdx.x - 32;                          // 0 .. 95
         uint32_t tile = 0;
         for (int item = first; item < p.total_items; item += stride) {
@@ -538,8 +556,14 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             mbar_wait(&vt_empty[vslot], ((tile / F8::NVT) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             const uint32_t raw = smem_u32(sRaw8) + rslot * F8::TILE8;
             const uint32_t dst = smem_u32(sVt) + vslot * F8::TILE8;
+            if constexpr (QPACK) {
+              const int valid = w.Sk - (w.jb + j) * C::BN;
 #pragma unroll 1
-            for (int u = ct; u < 2 * D; u += 32 * F8::CONVERTER_WARPS) vt_convert_unit<D>(raw, dst, u);
+              for (int u = ct; u < 2 * D; u += 32 * F8::CONVERTER_WARPS) vt_convert_unit<D, true>(raw, dst, u, valid);
+            } else {
+#pragma unroll 1
+              for (int u = ct; u < 2 * D; u += 32 * F8::CONVERTER_WARPS) vt_convert_unit<D>(raw, dst, u);
+            }
             fence_proxy_async_smem();                             // generic-proxy stores -> the wgmma's operand reads
             __syncwarp();
             if (lane == 0) {
@@ -558,16 +582,25 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           if (qcnt > 0) mbar_wait(q_empty, (qcnt - 1) & 1, p.dbg, SITE_LOAD_Q, qcnt);
           ++qcnt;
           mbar_arrive_expect_tx(q_full, F8::Q_BYTES);
-          tma_load_4d(sQ, &tmQ, q_full, 0, w.row0, w.hidx, w.bidx);
+          // packed (kVarlenFp8): the tensors are one batch entry, the sequence starts at row q0 / k0.  Rows a box takes
+          // in past the sequence's end are never stored (queries) or get -inf from the edge mask (keys; their V^T
+          // entries the converter writes as zeros)
+          int qy = w.row0, k0 = 0, wz = w.bidx;
+          if constexpr (QPACK) {
+            qy += w.q0;
+            k0 = w.k0;
+            wz = 0;
+          }
+          tma_load_4d(sQ, &tmQ, q_full, 0, qy, w.hidx, wz);
           for (int j = 0; j < w.n; ++j, ++tile) {
-            const int ky = (w.jb + j) * C::BN;
+            const int ky = k0 + (w.jb + j) * C::BN;
             const uint32_t kslot = tile % F8::NK, rslot = tile % F8::NRAW;
             mbar_wait(&k_empty[kslot], ((tile / F8::NK) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             mbar_arrive_expect_tx(&k_full[kslot], F8::TILE8);
-            tma_load_4d(sK8 + kslot * F8::TILE8, &tmK, &k_full[kslot], 0, ky, w.hkv, w.bidx);
+            tma_load_4d(sK8 + kslot * F8::TILE8, &tmK, &k_full[kslot], 0, ky, w.hkv, wz);
             mbar_wait(&raw8_empty[rslot], ((tile / F8::NRAW) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             mbar_arrive_expect_tx(&raw8_full[rslot], F8::TILE8);
-            tma_load_4d(sRaw8 + rslot * F8::TILE8, &tmV, &raw8_full[rslot], 0, ky, w.hkv, w.bidx);
+            tma_load_4d(sRaw8 + rslot * F8::TILE8, &tmV, &raw8_full[rslot], 0, ky, w.hkv, wz);
           }
         }
       }

@@ -45,6 +45,11 @@ extern template cudaError_t tfa::launch_forward<tfa::kDenseFp8>(int D, bool caus
                                                                 const CUtensorMap& tq, const CUtensorMap& tk,
                                                                 const CUtensorMap& tv, const tfa::FwdParams& p,
                                                                 int nblocks, bool persist, cudaStream_t stream);
+// tfa_varlen_fp8.cu: the FP8 variable-length attention forward, compiled apart from the other forward kernels
+extern template cudaError_t tfa::launch_forward<tfa::kVarlenFp8>(int D, bool causal, bool bf16, bool f32,
+                                                                 const CUtensorMap& tq, const CUtensorMap& tk,
+                                                                 const CUtensorMap& tv, const tfa::FwdParams& p,
+                                                                 int nblocks, bool persist, cudaStream_t stream);
 
 namespace {
 
@@ -191,7 +196,7 @@ long long fwd_grid(long long nitems, int variant) {
 }
 
 // One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache /
-// kVarlenCache / kCacheFp8 / kVarlenCacheFp8).
+// kVarlenCache / kCacheFp8 / kVarlenCacheFp8 / kDenseFp8 / kVarlenFp8).
 template <int MODE>
 int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
@@ -522,6 +527,36 @@ int varlen_impl(const tfa_attn_varlen_args& va) {
   return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
 }
 
+// The variable-length problem of tfa_attn_varlen_fwd() on e4m3 q / k / v: its checks in its order, then the
+// quantization's, then the kVarlenFp8 forward over the packed tensors as one batch entry of 8-bit swizzled Q / K maps
+// and the raw V map the converter transposes.
+int varlen_fp8_impl(const tfa_attn_varlen_args& va, const tfa_qkv_quant_args& quant) {
+  Problem a = from_varlen_args(va);
+  int rc = validate(a);
+  if (rc) return rc;
+  if (!va.cu_seqlens_q || !va.cu_seqlens_k ||
+      ((reinterpret_cast<uintptr_t>(va.cu_seqlens_q) | reinterpret_cast<uintptr_t>(va.cu_seqlens_k)) & 3u))
+    return TFA_EINVAL_SEQLENS;
+  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
+  if ((rc = validate_qkv_quant(quant, a))) return rc;
+  if (!arch_ok()) return TFA_EARCH;
+  init_dbg();
+
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, TFA_FP8_E4M3, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, true))) return rc;
+  if ((rc = make_tmap(&tk, a.k, TFA_FP8_E4M3, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss, true))) return rc;
+  if ((rc = make_tmap(&tv, a.v, TFA_FP8_E4M3, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
+
+  FwdParams p{};
+  p.cu_q = va.cu_seqlens_q;
+  p.cu_k = va.cu_seqlens_k;
+  p.total_q = a.Sq;
+  p.total_k = a.Sk;
+  p.v_scale = quant.v_scale;
+  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
+  return run_forward<tfa::kVarlenFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+}
+
 // The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
 Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   Problem q;
@@ -799,6 +834,11 @@ int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, co
 int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
   return fp8_impl(from_attn_args(*args), *quant);
+}
+
+int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return varlen_fp8_impl(*args, *quant);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {

@@ -156,6 +156,8 @@ def lib():
         L.tfa_attn_varlen_kvcache_fp8_fwd.restype = ci
         L.tfa_attn_fp8_fwd.argtypes = [ctypes.POINTER(AttnArgs), ctypes.POINTER(QkvQuantArgs)]
         L.tfa_attn_fp8_fwd.restype = ci
+        L.tfa_attn_varlen_fp8_fwd.argtypes = [ctypes.POINTER(VarlenArgs), ctypes.POINTER(QkvQuantArgs)]
+        L.tfa_attn_varlen_fp8_fwd.restype = ci
         L.tfa_selftest_wgmma_fp8.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp]
         L.tfa_selftest_wgmma_fp8.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
@@ -285,27 +287,37 @@ def attn_fwd(q, k, v, is_causal, softmax_scale, num_splits=1, out_fp32=False, st
 
 
 def attn_varlen_fwd(q, k, v, cu_q, cu_k, max_seqlen_q, is_causal, scale, out_fp32=False, out=None, lse=None,
-                    stream=None):
+                    stream=None, q_scale=1.0, k_scale=1.0, v_scale=1.0, out_dtype=None):
     """Packed variable-length batch through tfa_attn_varlen_fwd(): q (total_q, Hq, D), k/v (total_k, Hkv, D) device
     tensors with unit head_dim stride (views of a packed qkv tensor are fine; k and v share strides), cu_q / cu_k
     int32 device tensors of B + 1 offsets.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be
-    given to write into caller-owned buffers."""
+    given to write into caller-owned buffers.
+    torch.float8_e4m3fn q / k / v go through tfa_attn_varlen_fp8_fwd() with the per-tensor q_scale / k_scale / v_scale
+    and the output dtype out_dtype (bfloat16 or float16)."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k.dim() == 3 and k.shape == v.shape and k.stride() == v.stride()
     assert q.stride(2) == 1 and k.stride(2) == 1
     assert cu_q.dtype == torch.int32 and cu_k.dtype == torch.int32 and cu_q.numel() == cu_k.numel() >= 2
     total_q, Hq, D = q.shape
     total_k, Hkv, _ = k.shape
+    fp8 = [t.dtype == torch.float8_e4m3fn for t in (q, k, v)]
+    if any(fp8) and not all(fp8):
+        raise TypeError(f"q, k and v must all be float8_e4m3fn or none, got {q.dtype}, {k.dtype}, {v.dtype}")
+    quant, odt = _qkv_quant(q, q_scale, k_scale, v_scale, out_dtype)
     if out is None:
-        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else odt, device=q.device)
     if lse is None:
         lse = torch.empty((Hq, total_q), dtype=torch.float32, device=q.device)
     st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
     a = VarlenArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), lse.data_ptr(), cu_q.data_ptr(),
                    cu_k.data_ptr(), cu_q.numel() - 1, Hq, Hkv, D, total_q, total_k, int(max_seqlen_q),
-                   q.stride(0), q.stride(1), k.stride(0), k.stride(1), _dtype_code(q), int(bool(is_causal)),
-                   float(scale), int(bool(out_fp32)), st)
-    check(lib().tfa_attn_varlen_fwd(ctypes.byref(a)))
+                   q.stride(0), q.stride(1), k.stride(0), k.stride(1),
+                   (TFA_BF16 if odt == torch.bfloat16 else TFA_FP16) if quant else _dtype_code(q),
+                   int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
+    if quant is not None:
+        check(lib().tfa_attn_varlen_fp8_fwd(ctypes.byref(a), ctypes.byref(quant)))
+    else:
+        check(lib().tfa_attn_varlen_fwd(ctypes.byref(a)))
     return out, lse
 
 
