@@ -49,7 +49,8 @@ extern "C" {
 #define TFA_EDRIVER       (-6)  /* cuTensorMapEncodeTiled unavailable / failed    */
 #define TFA_EARCH         (-7)  /* device is not compute capability 9.0           */
 #define TFA_EDEVICE_FAULT (-8)  /* kernel watchdog fired; see tfa_debug_record()  */
-#define TFA_EINVAL_SCALE  (-9)  /* softmax_scale negative, NaN or infinite         */
+#define TFA_EINVAL_SCALE  (-9)  /* softmax_scale negative or NaN, or fp32(scale * log2 e) infinite: the largest
+                                   accepted scale is about FLT_MAX / log2 e = 2.3587e38 (FP8 calls: of s') */
 #define TFA_EINVAL_HEADS  (-10) /* Hq not a multiple of Hkv                         */
 #define TFA_EINVAL_WORKSPACE (-11) /* split-KV asked for but workspace missing/small */
 #define TFA_EINVAL_SEQLENS (-12)   /* cu_seqlens null / not 4-byte aligned, or max_seqlen_q not in [1, total_q] */
@@ -71,7 +72,10 @@ extern "C" {
  *   stride_b = S*H*D, stride_h = D,   stride_s = H*D.
  * q, k, v and out all use the same strides (the reference also assumes this:
  * flash_attention.cu:409-424). lse is always (B,H,S) contiguous fp32, natural log:
- *   lse = scale*max + ln(sum)   (flash_attention.cu:623). */
+ *   lse = scale*max + ln(sum)   (flash_attention.cu:623).
+ * Scale range: the kernels take exponents as fp32 scale * log2 e * score, so every call accepts 0 <= scale (s' for FP8)
+ * while fp32(scale * log2 e) is finite.  Rows without a visible key give exactly out = 0, lse = +inf at every accepted
+ * scale; the other rows are accurate while |scale * log2 e * score| stays within fp32 range. */
 typedef struct tfa_fwd_args {
   const void* q;
   const void* k;
@@ -352,8 +356,8 @@ int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args);
  *                  k8.to(q dtype) / v8.to(q dtype) with softmax_scale = s', its out multiplied by v_scale; for other
  *                  v_scale they differ by the rounding of that product.  Slots past K_b may hold any byte, NaN codes
  *                  0x7f / 0xff included, and do not change the result.
- * s' must stay a normal fp32 number: when it overflows, or when softmax_scale > 0 and it underflows below FLT_MIN (which
- * would make the attention uniform), the call returns TFA_EINVAL_SCALE.
+ * s' must stay a normal fp32 number with fp32(s' * log2 e) finite: when it overflows that, or when softmax_scale > 0
+ * and it underflows below FLT_MIN (which would make the attention uniform), the call returns TFA_EINVAL_SCALE.
  * Every check runs before any device work, those of the 16-bit call first (TFA_EINVAL_KVQUANT after them).  Launches
  * and CUDA-graph capture as the 16-bit calls; split-KV as tfa_attn_kvcache_fwd() (the varlen call has none). */
 typedef struct tfa_kv_quant_args {
@@ -379,10 +383,10 @@ int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, co
  *              the dequantized problem.  The kernel computes S = Q8 K8^T on e4m3 wgmma with fp32 accumulation, takes the
  *              softmax with scale s' = fp32(fp32(softmax_scale * q_scale) * k_scale) (that order), rounds P to e4m3
  *              (round to nearest even; P <= 2^8), computes P8 V8 on e4m3 wgmma and multiplies O by v_scale.
- * s' must stay a normal fp32 number: when it overflows, or when softmax_scale > 0 and it underflows below FLT_MIN, the
- * call returns TFA_EINVAL_SCALE.  Every check runs before any device work, those of tfa_attn_fwd() first, in its order,
- * then TFA_EINVAL_QKVQUANT, then TFA_EINVAL_SCALE for s'.  Launches: 1, + 1 with split-KV.  Callers quantize, e.g.
- * (x / s).clamp(-448, 448).to(torch.float8_e4m3fn). */
+ * s' must stay a normal fp32 number with fp32(s' * log2 e) finite: when it overflows that, or when softmax_scale > 0
+ * and it underflows below FLT_MIN, the call returns TFA_EINVAL_SCALE.  Every check runs before any device work, those
+ * of tfa_attn_fwd() first, in its order, then TFA_EINVAL_QKVQUANT, then TFA_EINVAL_SCALE for s'.  Launches: 1, + 1
+ * with split-KV.  Callers quantize, e.g. (x / s).clamp(-448, 448).to(torch.float8_e4m3fn). */
 typedef struct tfa_qkv_quant_args {
   int32_t qkv_dtype;                 /* TFA_FP8_E4M3 */
   float q_scale, k_scale, v_scale;   /* finite, > 0 */

@@ -159,6 +159,7 @@ struct FwdParams {
   int total_items;    // npairs * BH * nsplit
   float scale;        // softmax_scale
   float scale_log2;   // softmax_scale * log2(e)
+  float m_none;       // running max of a row without a key: -FLT_MAX / max(scale_log2, 1), rounded toward zero
   DebugRecord* dbg;
   // Variable length (VARLEN = true): batch entry b is the problem of rows [cu_q[b], cu_q[b+1]) of the packed q/out
   // and rows [cu_k[b], cu_k[b+1]) of the packed k/v; S is max_seqlen_q and Sk / causal_off are unused.  The arrays are
@@ -705,6 +706,11 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const int g = lane >> 2, tq = lane & 3;        // this thread: rows 16 wq + g and + 8, columns 8 i + 2 tq (+1)
   const int r_lo = t * 64 + wq * 16 + g;         // row inside the item (0..127); r_hi = r_lo + 8
   const float c = p.scale_log2;
+  // The running max of a row that sees no key in its first tile (p.m_none): finite, so that
+  // P = exp2(fmaf(-inf, c, -m * c)) = 0 rather than exp2(-inf + inf) = NaN, with -m * c <= FLT_MAX at every accepted c
+  // (a fixed -1e30 overflows it for c > 3.4e8).  m_none * c lies within an ulp of the lowest finite logit, so the
+  // clamp leaves every real max alone, and a later tile's first key rescales such a row by alpha = 0.
+  const float m_none = p.m_none;
   const uint32_t sQ_addr = smem_u32(sQ) + t * 64 * 128;   // this tile's rows inside each slab
   const uint32_t sKV_addr = smem_u32(sKV);
 
@@ -822,8 +828,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       a_lo = a_hi = 1.f;
       rescale = false;
       if (j == 0) {
-        m_lo = fmaxf(mx_lo, -1.0e30f);             // a fully masked row (split-KV) must not give -inf
-        m_hi = fmaxf(mx_hi, -1.0e30f);
+        m_lo = fmaxf(mx_lo, m_none);               // a row that sees no key yet (key-less, or masked in this split)
+        m_hi = fmaxf(mx_hi, m_none);
       } else {
         // lazy rescale of l and O: only when the row max moved by more than 2^8 (warp-uniform branch, rare)
         const bool n_lo = (mx_lo - m_lo) * c > kRescaleThresholdLog2;

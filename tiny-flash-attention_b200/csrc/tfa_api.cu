@@ -241,6 +241,11 @@ struct Problem {
   cudaStream_t stream;
 };
 
+// The kernels take exponents in log2 units, c = fp32(scale * log2 e): a scale >= 0 is accepted while c is finite,
+// i.e. up to about FLT_MAX / log2 e = 2.3587e38 (beyond it c = +inf turns every result into NaN).
+constexpr float kLog2e = 1.4426950408889634f;
+bool scale_in_range(float s) { return s >= 0.0f && std::isfinite(s * kLog2e); }
+
 int validate(const Problem& a) {
   if (!a.q || !a.k || !a.v || !a.out) return TFA_EINVAL_PTR;
   if ((reinterpret_cast<uintptr_t>(a.q) | reinterpret_cast<uintptr_t>(a.k) | reinterpret_cast<uintptr_t>(a.v) |
@@ -251,7 +256,7 @@ int validate(const Problem& a) {
   if (a.Hq % a.Hkv) return TFA_EINVAL_HEADS;
   if (a.dtype != TFA_BF16 && a.dtype != TFA_FP16) return TFA_EINVAL_DTYPE;
   // the running max is taken on unscaled scores (as in the reference, flash_attention.cu:228,295): scale must be >= 0
-  if (!(a.scale >= 0.0f) || !(a.scale <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (!scale_in_range(a.scale)) return TFA_EINVAL_SCALE;
   if (a.qss < a.D || (a.qss % 8) || (a.qsh % 8) || (a.qsb % 8)) return TFA_EINVAL_STRIDE;
   if (a.kss < a.D || (a.kss % 8) || (a.ksh % 8) || (a.ksb % 8)) return TFA_EINVAL_STRIDE;
   if (a.num_splits < 0) return TFA_EINVAL_SHAPE;
@@ -363,7 +368,10 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   p.scale = a.scale;
   // scale == 0 is legal (uniform attention over the visible keys): a tiny positive exponent scale keeps
   // masked scores at -inf (0 * -inf would be NaN) while every visible score still maps to exp2(0) = 1
-  p.scale_log2 = fmaxf(a.scale * 1.4426950408889634f, 1.0e-30f);
+  p.scale_log2 = fmaxf(a.scale * kLog2e, 1.0e-30f);
+  p.m_none = -FLT_MAX / fmaxf(p.scale_log2, 1.0f);
+  if (static_cast<double>(p.m_none) * fmaxf(p.scale_log2, 1.0f) < -static_cast<double>(FLT_MAX))
+    p.m_none = std::nextafter(p.m_none, 0.0f);          // rounded toward zero: -m_none * c stays finite
   p.dbg = g_dbg_dev;
   p.S = S;
   p.nsplit = plan.nsplit;
@@ -398,7 +406,7 @@ int validate_qkv_quant(const tfa_qkv_quant_args& q, Problem& a) {
     return TFA_EINVAL_QKVQUANT;
   const float qs = a.scale * q.q_scale;
   const float s = qs * q.k_scale;
-  if (!(s <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (!scale_in_range(s)) return TFA_EINVAL_SCALE;
   if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
   a.scale = s;
   return 0;
@@ -651,7 +659,7 @@ int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
     return TFA_EINVAL_KVQUANT;
   if ((a.ksb % 16) || (a.ksh % 16) || (a.kss % 16)) return TFA_EINVAL_KVQUANT;
   const float s = a.scale * q.k_scale;
-  if (!(s <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (!scale_in_range(s)) return TFA_EINVAL_SCALE;
   if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
   a.scale = s;
   qs.k_scale = q.k_scale;
@@ -882,7 +890,7 @@ int tfa_fwd_host(const void* q, const void* k, const void* v, void* out, float* 
   if (D != 64 && D != 128) return TFA_EINVAL_DIM;
   if (B < 1 || H < 1 || S < 1) return TFA_EINVAL_SHAPE;
   if (dtype != TFA_BF16 && dtype != TFA_FP16) return TFA_EINVAL_DTYPE;
-  if (!(softmax_scale >= 0.0f) || !(softmax_scale <= 3.0e38f)) return TFA_EINVAL_SCALE;
+  if (!scale_in_range(softmax_scale)) return TFA_EINVAL_SCALE;
   const int dev = current_device();
   if (dev < 0) return static_cast<int>(cudaErrorInvalidDevice);
   std::lock_guard<std::mutex> lk(g_ws_mu);
@@ -1031,7 +1039,9 @@ const char* tfa_error_string(int code) {
     case TFA_EDRIVER: return "tfa: cuTensorMapEncodeTiled unavailable or failed";
     case TFA_EARCH: return "tfa: this library only runs on compute capability 9.0 (H100, sm_90a)";
     case TFA_EDEVICE_FAULT: return "tfa: kernel watchdog fired (see tfa_debug_record)";
-    case TFA_EINVAL_SCALE: return "tfa: softmax_scale must be finite and >= 0";
+    case TFA_EINVAL_SCALE:
+      return "tfa: softmax_scale (for FP8: the effective scale s') must be >= 0 with scale * log2(e) finite in fp32 "
+             "(at most about 2.3587e38)";
     case TFA_EINVAL_HEADS: return "tfa: query heads must be a multiple of K/V heads";
     case TFA_EINVAL_WORKSPACE: return "tfa: split-KV needs a 16-byte aligned workspace of tfa_attn_workspace_bytes()";
     case TFA_EINVAL_SEQLENS:
