@@ -47,11 +47,18 @@ std::string fmt_msg(const char* fmt, long long a = 0, long long b = 0, long long
 }
 
 // q is fp16 or bf16, and the other two tensors share its dtype and device; `names` names all three in the messages.
+// With `fp8_out` the three are float8_e4m3fn instead, and *fp8_out, the output's dtype, is bfloat16 or float16.
 void check_dtype_device(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v,
-                        const std::string& names) {
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
-  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
-              names + " must have the same dtype");
+                        const std::string& names, std::optional<at::ScalarType> fp8_out = std::nullopt) {
+  if (fp8_out) {
+    TORCH_CHECK(q.scalar_type() == at::kFloat8_e4m3fn && k.scalar_type() == at::kFloat8_e4m3fn &&
+                v.scalar_type() == at::kFloat8_e4m3fn, names + " must be float8_e4m3fn");
+    TORCH_CHECK(*fp8_out == at::kBFloat16 || *fp8_out == at::kHalf, "out_dtype must be bfloat16 or float16");
+  } else {
+    TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
+    TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(),
+                names + " must have the same dtype");
+  }
   TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), names + " must be on the same device");
 }
 
@@ -164,65 +171,17 @@ std::vector<torch::Tensor> flash_attention_v2_fp32out(torch::Tensor q, torch::Te
   return fwd_generic(q, k, v, is_causal, softmax_scale, /*bshd=*/false, /*out_fp32=*/true);
 }
 
-// Generalised problem (SURVEY.md 8f rows 2-3): k, v are (B, Hkv, Sk, D) with Hq % Hkv == 0 and any Sk; causal is
-// bottom-right aligned (flash_attention_c/csrc/attn.cpp:121-124; head grouping csrc/archive_)/attn.cpp:61,375).
-// num_splits: 1 = single pass, n > 1 = split-KV with an LSE merge, 0 = let the library decide.
-std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Tensor k, torch::Tensor v, bool is_causal,
-                                                      float softmax_scale, int64_t num_splits) {
+namespace {
+
+// flash_attention_v2_general, or with `quant` flash_attention_v2_fp8: e4m3 q, k, v and the output in out_dtype.
+std::vector<torch::Tensor> attn_fwd(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v,
+                                    bool is_causal, float softmax_scale, int64_t num_splits, at::ScalarType out_dtype,
+                                    const tfa_qkv_quant_args* quant) {
   TFA_CHECK_INPUT(q);
   TFA_CHECK_INPUT(k);
   TFA_CHECK_INPUT(v);
   TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q, k, v must have 4 dimensions");
-  check_dtype_device(q, k, v, "q, k, v");
-  TORCH_CHECK(k.sizes() == v.sizes(), "k and v must have identical shapes");
-  TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), "k/v must share batch and head_dim with q");
-  const int64_t B = q.size(0), Hq = q.size(1), Sq = q.size(2), D = q.size(3), Hkv = k.size(1), Sk = k.size(2);
-  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
-  TORCH_CHECK(B >= 1 && Hq >= 1 && Hkv >= 1 && Sq >= 1 && Sk >= 1, "empty tensors are not supported");
-  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
-                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
-  TORCH_CHECK(num_splits >= 0 && num_splits <= 1024, "num_splits must be in [0, 1024]");
-
-  torch::Tensor out, lse, ws;
-  int rc = 0;
-  {
-    c10::cuda::CUDAGuard guard(q.device());
-    out = torch::empty_like(q);
-    lse = torch::empty({B, Hq, Sq}, q.options().dtype(at::kFloat));
-    tfa_attn_args a;
-    a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
-    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
-    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
-    a.Sq = static_cast<int32_t>(Sq); a.Sk = static_cast<int32_t>(Sk); a.D = static_cast<int32_t>(D);
-    a.q_stride_b = Hq * Sq * D; a.q_stride_h = Sq * D; a.q_stride_s = D;
-    a.kv_stride_b = Hkv * Sk * D; a.kv_stride_h = Sk * D; a.kv_stride_s = D;
-    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
-    a.is_causal = is_causal ? 1 : 0;
-    a.softmax_scale = softmax_scale;
-    a.out_fp32 = 0;
-    a.num_splits = static_cast<int32_t>(num_splits);
-    a.workspace = nullptr; a.workspace_bytes = 0;
-    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    ws = split_workspace(a, q);
-    rc = tfa_attn_fwd(&a);
-  }
-  raise_on_error(rc);
-  return {out, lse};
-}
-
-// FP8 attention (tfa_attn_fp8_fwd): q, k, v as flash_attention_v2_general but float8_e4m3fn, with the per-tensor scales
-// their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is the output's.
-std::vector<torch::Tensor> flash_attention_v2_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v, double q_scale,
-                                                  double k_scale, double v_scale, bool is_causal, float softmax_scale,
-                                                  at::ScalarType out_dtype, int64_t num_splits) {
-  TFA_CHECK_INPUT(q);
-  TFA_CHECK_INPUT(k);
-  TFA_CHECK_INPUT(v);
-  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q, k, v must have 4 dimensions");
-  TORCH_CHECK(q.scalar_type() == at::kFloat8_e4m3fn && k.scalar_type() == at::kFloat8_e4m3fn &&
-              v.scalar_type() == at::kFloat8_e4m3fn, "q, k, v must be float8_e4m3fn");
-  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on one device");
-  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf, "out_dtype must be bfloat16 or float16");
+  check_dtype_device(q, k, v, "q, k, v", quant ? std::optional<at::ScalarType>(out_dtype) : std::nullopt);
   TORCH_CHECK(k.sizes() == v.sizes(), "k and v must have identical shapes");
   TORCH_CHECK(k.size(0) == q.size(0) && k.size(3) == q.size(3), "k/v must share batch and head_dim with q");
   const int64_t B = q.size(0), Hq = q.size(1), Sq = q.size(2), D = q.size(3), Hkv = k.size(1), Sk = k.size(2);
@@ -253,92 +212,25 @@ std::vector<torch::Tensor> flash_attention_v2_fp8(torch::Tensor q, torch::Tensor
     a.workspace = nullptr; a.workspace_bytes = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
     ws = split_workspace(a, q);
-    tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
-                          static_cast<float>(v_scale)};
-    rc = tfa_attn_fp8_fwd(&a, &qa);
+    rc = quant ? tfa_attn_fp8_fwd(&a, quant) : tfa_attn_fwd(&a);
   }
   raise_on_error(rc);
   return {out, lse};
 }
 
-// Variable-length batch (the packed cu_seqlens interface of flash-attn's varlen forward): q (total_q, Hq, D),
-// k, v (total_k, Hkv, D), unit head_dim stride (views of one packed (total, 3, H, D) qkv tensor need no copy);
-// cu_seqlens_q / cu_seqlens_k int32 of B + 1 offsets on q's device.  Returns out (total_q, Hq, D) contiguous and
-// lse (Hq, total_q).  max_seqlen_k is not taken: the kernel has no use for it.
-std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Tensor k, torch::Tensor v,
-                                                     torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
-                                                     int64_t max_seqlen_q, bool is_causal, float softmax_scale) {
-  TFA_CHECK_CUDA(q);
-  TFA_CHECK_CUDA(k);
-  TFA_CHECK_CUDA(v);
-  TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3, "q, k, v must have 3 dimensions (total, heads, head_dim)");
-  check_dtype_device(q, k, v, "q, k, v");
-  TORCH_CHECK(k.sizes() == v.sizes() && k.strides() == v.strides(), "k and v must have identical shapes and strides");
-  TORCH_CHECK(k.size(2) == q.size(2), "k/v must share head_dim with q");
-  TORCH_CHECK(q.stride(2) == 1 && k.stride(2) == 1, "q, k, v must have a unit head_dim stride");
-  TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt && cu_seqlens_k.scalar_type() == at::kInt,
-              "cu_seqlens_q and cu_seqlens_k must be int32");
-  TORCH_CHECK(cu_seqlens_q.device() == q.device() && cu_seqlens_k.device() == q.device(),
-              "cu_seqlens_q and cu_seqlens_k must be on q's device");
-  TORCH_CHECK(cu_seqlens_q.dim() == 1 && cu_seqlens_q.is_contiguous() && cu_seqlens_k.dim() == 1 &&
-                  cu_seqlens_k.is_contiguous(),
-              "cu_seqlens_q and cu_seqlens_k must be contiguous 1-D tensors");
-  TORCH_CHECK(cu_seqlens_q.numel() >= 2 && cu_seqlens_k.numel() == cu_seqlens_q.numel(),
-              fmt_msg("cu_seqlens_q and cu_seqlens_k must both hold B + 1 >= 2 offsets, got %lld and %lld",
-                      static_cast<long long>(cu_seqlens_q.numel()), static_cast<long long>(cu_seqlens_k.numel())));
-  const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2), total_k = k.size(0), Hkv = k.size(1);
-  const int64_t B = cu_seqlens_q.numel() - 1;
-  TORCH_CHECK(D == 64 || D == 128, fmt_msg("head_dim must be 64 or 128, got %lld", static_cast<long long>(D)));
-  TORCH_CHECK(total_q >= 1 && total_k >= 1 && Hq >= 1 && Hkv >= 1, "empty tensors are not supported");
-  TORCH_CHECK(Hq % Hkv == 0, fmt_msg("query heads (%lld) must be a multiple of K/V heads (%lld)",
-                                     static_cast<long long>(Hq), static_cast<long long>(Hkv)));
-  TORCH_CHECK(max_seqlen_q >= 1 && max_seqlen_q <= total_q,
-              fmt_msg("max_seqlen_q must be in [1, total_q = %lld], got %lld", static_cast<long long>(total_q),
-                      static_cast<long long>(max_seqlen_q)));
-  TORCH_CHECK(total_q < (1LL << 31) && total_k < (1LL << 31) && B < (1LL << 31), "tensors too large");
-
-  torch::Tensor out, lse;
-  int rc = 0;
-  {
-    c10::cuda::CUDAGuard guard(q.device());
-    out = torch::empty({total_q, Hq, D}, q.options());
-    lse = torch::empty({Hq, total_q}, q.options().dtype(at::kFloat));
-    tfa_attn_varlen_args a;
-    a.q = q.data_ptr(); a.k = k.data_ptr(); a.v = v.data_ptr();
-    a.out = out.data_ptr(); a.lse = lse.data_ptr<float>();
-    a.cu_seqlens_q = cu_seqlens_q.data_ptr<int32_t>();
-    a.cu_seqlens_k = cu_seqlens_k.data_ptr<int32_t>();
-    a.B = static_cast<int32_t>(B); a.Hq = static_cast<int32_t>(Hq); a.Hkv = static_cast<int32_t>(Hkv);
-    a.D = static_cast<int32_t>(D);
-    a.total_q = static_cast<int32_t>(total_q); a.total_k = static_cast<int32_t>(total_k);
-    a.max_seqlen_q = static_cast<int32_t>(max_seqlen_q);
-    a.q_stride_s = q.stride(0); a.q_stride_h = q.stride(1);
-    a.kv_stride_s = k.stride(0); a.kv_stride_h = k.stride(1);
-    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
-    a.is_causal = is_causal ? 1 : 0;
-    a.softmax_scale = softmax_scale;
-    a.out_fp32 = 0;
-    a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    rc = tfa_attn_varlen_fwd(&a);
+// flash_attention_v2_varlen, or with `quant` flash_attention_v2_varlen_fp8: e4m3 q, k, v and the output in out_dtype.
+std::vector<torch::Tensor> varlen_fwd(const torch::Tensor& q, const torch::Tensor& k, const torch::Tensor& v,
+                                      const torch::Tensor& cu_seqlens_q, const torch::Tensor& cu_seqlens_k,
+                                      int64_t max_seqlen_q, bool is_causal, float softmax_scale,
+                                      at::ScalarType out_dtype, const tfa_qkv_quant_args* quant) {
+  if (!quant) {
+    TFA_CHECK_CUDA(q);
+    TFA_CHECK_CUDA(k);
+    TFA_CHECK_CUDA(v);
   }
-  raise_on_error(rc);
-  return {out, lse};
-}
-
-// FP8 variable-length batch (tfa_attn_varlen_fp8_fwd): q, k, v as flash_attention_v2_varlen but float8_e4m3fn, with the
-// per-tensor scales their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is
-// the output's.  Returns out (total_q, Hq, D) contiguous and lse (Hq, total_q).
-std::vector<torch::Tensor> flash_attention_v2_varlen_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v,
-                                                         torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
-                                                         int64_t max_seqlen_q, double q_scale, double k_scale,
-                                                         double v_scale, bool is_causal, float softmax_scale,
-                                                         at::ScalarType out_dtype) {
-  // the element types and devices first, then the CUDA checks: a wrong dtype is reported as such wherever q lives
   TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3, "q, k, v must have 3 dimensions (total, heads, head_dim)");
-  TORCH_CHECK(q.scalar_type() == at::kFloat8_e4m3fn && k.scalar_type() == at::kFloat8_e4m3fn &&
-              v.scalar_type() == at::kFloat8_e4m3fn, "q, k, v must be float8_e4m3fn");
-  TORCH_CHECK(out_dtype == at::kBFloat16 || out_dtype == at::kHalf, "out_dtype must be bfloat16 or float16");
-  TORCH_CHECK(k.device() == q.device() && v.device() == q.device(), "q, k, v must be on the same device");
+  check_dtype_device(q, k, v, "q, k, v", quant ? std::optional<at::ScalarType>(out_dtype) : std::nullopt);
+  // FP8: the element types and devices first, then the CUDA check: a wrong dtype is reported as such wherever q lives
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(k.sizes() == v.sizes() && k.strides() == v.strides(), "k and v must have identical shapes and strides");
   TORCH_CHECK(k.size(2) == q.size(2), "k/v must share head_dim with q");
@@ -386,12 +278,54 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_fp8(torch::Tensor q, torch:
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
-                          static_cast<float>(v_scale)};
-    rc = tfa_attn_varlen_fp8_fwd(&a, &qa);
+    rc = quant ? tfa_attn_varlen_fp8_fwd(&a, quant) : tfa_attn_varlen_fwd(&a);
   }
   raise_on_error(rc);
   return {out, lse};
+}
+
+}  // namespace
+
+// Generalised problem (SURVEY.md 8f rows 2-3): k, v are (B, Hkv, Sk, D) with Hq % Hkv == 0 and any Sk; causal is
+// bottom-right aligned (flash_attention_c/csrc/attn.cpp:121-124; head grouping csrc/archive_)/attn.cpp:61,375).
+// num_splits: 1 = single pass, n > 1 = split-KV with an LSE merge, 0 = let the library decide.
+std::vector<torch::Tensor> flash_attention_v2_general(torch::Tensor q, torch::Tensor k, torch::Tensor v, bool is_causal,
+                                                      float softmax_scale, int64_t num_splits) {
+  return attn_fwd(q, k, v, is_causal, softmax_scale, num_splits, q.scalar_type(), nullptr);
+}
+
+// FP8 attention (tfa_attn_fp8_fwd): q, k, v as flash_attention_v2_general but float8_e4m3fn, with the per-tensor scales
+// their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is the output's.
+std::vector<torch::Tensor> flash_attention_v2_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v, double q_scale,
+                                                  double k_scale, double v_scale, bool is_causal, float softmax_scale,
+                                                  at::ScalarType out_dtype, int64_t num_splits) {
+  const tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
+                              static_cast<float>(v_scale)};
+  return attn_fwd(q, k, v, is_causal, softmax_scale, num_splits, out_dtype, &qa);
+}
+
+// Variable-length batch (the packed cu_seqlens interface of flash-attn's varlen forward): q (total_q, Hq, D),
+// k, v (total_k, Hkv, D), unit head_dim stride (views of one packed (total, 3, H, D) qkv tensor need no copy);
+// cu_seqlens_q / cu_seqlens_k int32 of B + 1 offsets on q's device.  Returns out (total_q, Hq, D) contiguous and
+// lse (Hq, total_q).  max_seqlen_k is not taken: the kernel has no use for it.
+std::vector<torch::Tensor> flash_attention_v2_varlen(torch::Tensor q, torch::Tensor k, torch::Tensor v,
+                                                     torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
+                                                     int64_t max_seqlen_q, bool is_causal, float softmax_scale) {
+  return varlen_fwd(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, softmax_scale, q.scalar_type(),
+                    nullptr);
+}
+
+// FP8 variable-length batch (tfa_attn_varlen_fp8_fwd): q, k, v as flash_attention_v2_varlen but float8_e4m3fn, with the
+// per-tensor scales their codes stand for; both products run on e4m3 tensor cores.  out_dtype (bfloat16 / float16) is
+// the output's.  Returns out (total_q, Hq, D) contiguous and lse (Hq, total_q).
+std::vector<torch::Tensor> flash_attention_v2_varlen_fp8(torch::Tensor q, torch::Tensor k, torch::Tensor v,
+                                                         torch::Tensor cu_seqlens_q, torch::Tensor cu_seqlens_k,
+                                                         int64_t max_seqlen_q, double q_scale, double k_scale,
+                                                         double v_scale, bool is_causal, float softmax_scale,
+                                                         at::ScalarType out_dtype) {
+  const tfa_qkv_quant_args qa{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
+                              static_cast<float>(v_scale)};
+  return varlen_fwd(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, is_causal, softmax_scale, out_dtype, &qa);
 }
 
 namespace {

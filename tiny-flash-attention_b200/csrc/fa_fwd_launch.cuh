@@ -4,8 +4,8 @@
 //
 // tfa_varlen_kvcache.cu explicitly instantiates launch_forward<kVarlenCache>, tfa_kvcache_fp8.cu launch_forward<
 // kCacheFp8> and launch_forward<kVarlenCacheFp8>, tfa_fp8_fwd.cu launch_forward<kDenseFp8> and tfa_varlen_fp8.cu
-// launch_forward<kVarlenFp8>, and tfa_api.cu declares those instantiations `extern template`, so that each mode's 32
-// kernels are compiled in that unit only (the comment there says why).
+// launch_forward<kVarlenFp8>; the end of this header declares those instantiations `extern template`, so that each
+// mode's 32 kernels are compiled in that unit only.
 #pragma once
 #include "fa_fwd_sm90.cuh"
 
@@ -51,5 +51,18 @@ cudaError_t launch_forward(int D, bool causal, bool bf16, bool f32, const CUtens
   if (D == 64) return launch_forward_d<64, MODE>(causal, bf16, f32, tq, tk, tv, p, nblocks, persist, stream);
   return launch_forward_d<128, MODE>(causal, bf16, f32, tq, tk, tv, p, nblocks, persist, stream);
 }
+
+// The modes compiled in translation units of their own: the device compiler optimises a unit as one module, and new
+// kernels instantiated next to the forward can change the generated code of the existing instantiations.  Kept apart,
+// those are exactly what they were without these modes.
+#define TFA_LAUNCH_ELSEWHERE(MODE_)                                                                                 \
+  extern template cudaError_t launch_forward<MODE_>(int, bool, bool, bool, const CUtensorMap&, const CUtensorMap&, \
+                                                    const CUtensorMap&, const FwdParams&, int, bool, cudaStream_t)
+TFA_LAUNCH_ELSEWHERE(kVarlenCache);       // tfa_varlen_kvcache.cu
+TFA_LAUNCH_ELSEWHERE(kCacheFp8);          // tfa_kvcache_fp8.cu
+TFA_LAUNCH_ELSEWHERE(kVarlenCacheFp8);    // tfa_kvcache_fp8.cu
+TFA_LAUNCH_ELSEWHERE(kDenseFp8);          // tfa_fp8_fwd.cu
+TFA_LAUNCH_ELSEWHERE(kVarlenFp8);         // tfa_varlen_fp8.cu
+#undef TFA_LAUNCH_ELSEWHERE
 
 }  // namespace tfa

@@ -764,6 +764,15 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       __syncwarp();
       if (lane == 0) mbar_arrive(bar);
     };
+    // The rings tile j's K and V arrive on; ent counts the entries of earlier items.  16-bit operands: one ring for
+    // both, K_j at entry ent + 2j and V_j at ent + 2j + 1 of kv_full / kv_empty[NSTAGE].  DF8: a ring each, both at
+    // entry ent + j, K_j on k_full / k_empty[NK] and V^T_j on vt_full / vt_empty[NVT].
+    constexpr int KV_ENTS = DF8 ? 1 : 2;                               // entries per tile
+    constexpr uint32_t NKR = DF8 ? F8::NK : NSTAGE, NVR = DF8 ? F8::NVT : NSTAGE;
+    uint64_t* const kr_full = DF8 ? k_full : kv_full;
+    uint64_t* const kr_empty = DF8 ? k_empty : kv_empty;
+    uint64_t* const vr_full = DF8 ? vt_full : kv_full;
+    uint64_t* const vr_empty = DF8 ? vt_empty : kv_empty;
     // cache: the slots of a page past the sequence's keys may hold anything; varlen: the rows past the sequence's keys
     // are the next sequence's, Inf and NaN included.  P = 0 does not cancel 0 * Inf or 0 * NaN in the PV product.  So
     // before PV reads the tile holding key Sk - 1 (only an item's last tile can: every earlier one lies below
@@ -870,73 +879,18 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     };
 
     // An item without tiles waits on no barrier: its rows get O = 0 and LSE = +inf (a split-KV partial: LSE = -inf).
-    if (DF8 && n > 0) {
-      // kDenseFp8: K_j on k_full[(ent + j) % NK], V^T_j on vt_full[(ent + j) % NVT]; ent counts earlier items' tiles
-      mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
-      ++qcnt;
-      {
-        const uint32_t kslot = ent % F8::NK;
-        mbar_wait(&k_full[kslot], (ent / F8::NK) & 1, p.dbg, SITE_MMA_K, ent);
-        wgmma_fence();
-        issue_S(s, kslot);
-        wgmma_wait<0>();
-        reg_fence(s);
-        release(&k_empty[kslot]);
-        if (n == 1) release(q_empty);
-        bool rs;
-        float a0, a1;
-        softmax(0, rs, a0, a1);
-        pack_P();
-      }
-      for (int j = 1; j < n; ++j) {
-        const uint32_t ek = ent + j, ev = ent + j - 1;
-        const uint32_t kslot = ek % F8::NK, vslot = ev % F8::NVT;
-        mbar_wait(&k_full[kslot], (ek / F8::NK) & 1, p.dbg, SITE_MMA_K, ek);
-        wgmma_fence();
-        issue_S(s, kslot);
-        mbar_wait(&vt_full[vslot], (ev / F8::NVT) & 1, p.dbg, SITE_MMA_V, ev);
-        issue_PV(o, pf, vslot, j > 1);
-        wgmma_wait<1>();                               // S_j done
-        reg_fence(s);
-        release(&k_empty[kslot]);
-        if (j == n - 1) release(q_empty);
-        bool rs;
-        float a_lo, a_hi;
-        softmax(j, rs, a_lo, a_hi);
-        wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
-        reg_fence(o);
-        release(&vt_empty[vslot]);
-        if (rs) {
-#pragma unroll
-          for (int i = 0; i < D / 8; ++i) {
-            o[4 * i + 0] *= a_lo; o[4 * i + 1] *= a_lo;
-            o[4 * i + 2] *= a_hi; o[4 * i + 3] *= a_hi;
-          }
-        }
-        pack_P();
-      }
-      {
-        const uint32_t ev = ent + n - 1, vslot = ev % F8::NVT;
-        mbar_wait(&vt_full[vslot], (ev / F8::NVT) & 1, p.dbg, SITE_MMA_V, ev);
-        wgmma_fence();
-        issue_PV(o, pf, vslot, n > 1);
-        wgmma_wait<0>();
-        reg_fence(o);
-        release(&vt_empty[vslot]);
-      }
-      ent += n;
-    } else if (n > 0) {
+    if (n > 0) {
       mbar_wait(q_full, qcnt & 1, p.dbg, SITE_MMA_Q, qcnt);
       ++qcnt;
       // ---- KV tile 0 ----
       {
-        const uint32_t kslot = ent % NSTAGE;
-        mbar_wait(&kv_full[kslot], (ent / NSTAGE) & 1, p.dbg, SITE_MMA_K, ent);
+        const uint32_t kslot = ent % NKR;
+        mbar_wait(&kr_full[kslot], (ent / NKR) & 1, p.dbg, SITE_MMA_K, ent);
         wgmma_fence();
         issue_S(s, kslot);
         wgmma_wait<0>();
         reg_fence(s);
-        release(&kv_empty[kslot]);
+        release(&kr_empty[kslot]);
         if (n == 1) release(q_empty);
         bool rs;
         float a0, a1;
@@ -945,23 +899,23 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
       // ---- KV tiles 1 .. n-1: S_j and PV_{j-1} in flight together ----
       for (int j = 1; j < n; ++j) {
-        const uint32_t ek = ent + 2 * j, ev = ent + 2 * j - 1;
-        const uint32_t kslot = ek % NSTAGE, vslot = ev % NSTAGE;
-        mbar_wait(&kv_full[kslot], (ek / NSTAGE) & 1, p.dbg, SITE_MMA_K, ek);
+        const uint32_t ek = ent + KV_ENTS * j, ev = ent + KV_ENTS * j - 1;
+        const uint32_t kslot = ek % NKR, vslot = ev % NVR;
+        mbar_wait(&kr_full[kslot], (ek / NKR) & 1, p.dbg, SITE_MMA_K, ek);
         wgmma_fence();
         issue_S(s, kslot);
-        mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        mbar_wait(&vr_full[vslot], (ev / NVR) & 1, p.dbg, SITE_MMA_V, ev);
         issue_PV(o, pf, vslot, j > 1);
         wgmma_wait<1>();                               // S_j done
         reg_fence(s);
-        release(&kv_empty[kslot]);
+        release(&kr_empty[kslot]);
         if (j == n - 1) release(q_empty);
         bool rs;
         float a_lo, a_hi;
         softmax(j, rs, a_lo, a_hi);
         wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
         reg_fence(o);
-        release(&kv_empty[vslot]);
+        release(&vr_empty[vslot]);
         if (rs) {
 #pragma unroll
           for (int i = 0; i < D / 8; ++i) {
@@ -972,16 +926,16 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         pack_P();
       }
       {
-        const uint32_t ev = ent + 2 * n - 1, vslot = ev % NSTAGE;
-        mbar_wait(&kv_full[vslot], (ev / NSTAGE) & 1, p.dbg, SITE_MMA_V, ev);
+        const uint32_t ev = ent + KV_ENTS * n - 1, vslot = ev % NVR;
+        mbar_wait(&vr_full[vslot], (ev / NVR) & 1, p.dbg, SITE_MMA_V, ev);
         zero_v_tail(vslot, n - 1);
         wgmma_fence();
         issue_PV(o, pf, vslot, n > 1);
         wgmma_wait<0>();
         reg_fence(o);
-        release(&kv_empty[vslot]);
+        release(&vr_empty[vslot]);
       }
-      ent += 2 * n;
+      ent += KV_ENTS * n;
     }
 
     // ---------------------------- epilogue ----------------------------

@@ -26,30 +26,6 @@
 // tfa_append.cu: the append's launch, compiled apart from the forward kernels
 int tfa_internal_launch_append(const tfa::AppendKernelParams& p, const tfa::KvQuant* qs, int D, bool bf16, bool rotary,
                                bool interleaved, cudaStream_t stream);
-// tfa_varlen_kvcache.cu: the variable-length cache forward, compiled apart from the other forward kernels
-extern template cudaError_t tfa::launch_forward<tfa::kVarlenCache>(int D, bool causal, bool bf16, bool f32,
-                                                                   const CUtensorMap& tq, const CUtensorMap& tk,
-                                                                   const CUtensorMap& tv, const tfa::FwdParams& p,
-                                                                   int nblocks, bool persist, cudaStream_t stream);
-// tfa_kvcache_fp8.cu: the FP8-cache forwards, compiled apart from the other forward kernels
-extern template cudaError_t tfa::launch_forward<tfa::kCacheFp8>(int D, bool causal, bool bf16, bool f32,
-                                                                const CUtensorMap& tq, const CUtensorMap& tk,
-                                                                const CUtensorMap& tv, const tfa::FwdParams& p,
-                                                                int nblocks, bool persist, cudaStream_t stream);
-extern template cudaError_t tfa::launch_forward<tfa::kVarlenCacheFp8>(int D, bool causal, bool bf16, bool f32,
-                                                                      const CUtensorMap& tq, const CUtensorMap& tk,
-                                                                      const CUtensorMap& tv, const tfa::FwdParams& p,
-                                                                      int nblocks, bool persist, cudaStream_t stream);
-// tfa_fp8_fwd.cu: the FP8 attention forward, compiled apart from the other forward kernels
-extern template cudaError_t tfa::launch_forward<tfa::kDenseFp8>(int D, bool causal, bool bf16, bool f32,
-                                                                const CUtensorMap& tq, const CUtensorMap& tk,
-                                                                const CUtensorMap& tv, const tfa::FwdParams& p,
-                                                                int nblocks, bool persist, cudaStream_t stream);
-// tfa_varlen_fp8.cu: the FP8 variable-length attention forward, compiled apart from the other forward kernels
-extern template cudaError_t tfa::launch_forward<tfa::kVarlenFp8>(int D, bool causal, bool bf16, bool f32,
-                                                                 const CUtensorMap& tq, const CUtensorMap& tk,
-                                                                 const CUtensorMap& tv, const tfa::FwdParams& p,
-                                                                 int nblocks, bool persist, cudaStream_t stream);
 
 namespace {
 
@@ -395,9 +371,18 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   return (a.D == 64) ? launch_combine<64>(cp, bf16, f32, a.stream) : launch_combine<128>(cp, bf16, f32, a.stream);
 }
 
+// The effective softmax scale s' of an FP8 call, as the caller rounds it from softmax_scale and the quantization scales,
+// must stay a normal fp32 number (or 0 with softmax_scale = 0): an overflow, or an underflow that would silently turn
+// the call into uniform attention, is TFA_EINVAL_SCALE.
+int validate_fp8_scale(float softmax_scale, float s) {
+  if (!scale_in_range(s)) return TFA_EINVAL_SCALE;
+  if (softmax_scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
+  return 0;
+}
+
 // The FP8-attention arguments of a call whose 16-bit checks passed: the element type, the scales and q / k / v strides
 // that keep every 1-byte TMA row and box 16-byte aligned.  Sets a.scale to s' = fp32(fp32(softmax_scale * q_scale) *
-// k_scale), which must stay a normal fp32 number (or 0 with softmax_scale = 0), as validate_quant's s'.
+// k_scale).
 int validate_qkv_quant(const tfa_qkv_quant_args& q, Problem& a) {
   if (q.qkv_dtype != TFA_FP8_E4M3) return TFA_EINVAL_QKVQUANT;
   for (const float x : {q.q_scale, q.k_scale, q.v_scale})
@@ -406,40 +391,17 @@ int validate_qkv_quant(const tfa_qkv_quant_args& q, Problem& a) {
     return TFA_EINVAL_QKVQUANT;
   const float qs = a.scale * q.q_scale;
   const float s = qs * q.k_scale;
-  if (!scale_in_range(s)) return TFA_EINVAL_SCALE;
-  if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
+  if (int rc = validate_fp8_scale(a.scale, s)) return rc;
   a.scale = s;
   return 0;
 }
 
-// The dense problem of tfa_attn_fwd() on e4m3 q / k / v: its checks in its order, then the quantization's, then the
-// kDenseFp8 forward over 8-bit swizzled Q / K maps and the raw V map the converter transposes.
-int fp8_impl(Problem a, const tfa_qkv_quant_args& quant) {
+// The dense forward.  `quant` nullptr: 16-bit q / k / v, optionally with the fused exchange (n_extra > 0).  Otherwise
+// e4m3 ones, checked after the 16-bit checks, for the kDenseFp8 forward.
+int fwd_impl(Problem a, const tfa_qkv_quant_args* quant, void* const* extra_dst = nullptr, int n_extra = 0) {
   int rc = validate(a);
   if (rc) return rc;
-  if ((rc = validate_qkv_quant(quant, a))) return rc;
-  if (!arch_ok()) return TFA_EARCH;
-  init_dbg();
-
-  SplitPlan plan;
-  if ((rc = plan_splits(a, plan))) return rc;
-
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, TFA_FP8_E4M3, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, true))) return rc;
-  if ((rc = make_tmap(&tk, a.k, TFA_FP8_E4M3, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss, true))) return rc;
-  if ((rc = make_tmap(&tv, a.v, TFA_FP8_E4M3, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-
-  FwdParams p{};
-  p.Sk = a.Sk;
-  p.causal_off = a.causal ? a.Sk - a.Sq : 0;
-  p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
-  p.v_scale = quant.v_scale;
-  return run_forward<tfa::kDenseFp8>(a, p, a.Sq, tq, tk, tv, plan);
-}
-
-int fwd_impl(const Problem& a, void* const* extra_dst = nullptr, int n_extra = 0) {
-  int rc = validate(a);
-  if (rc) return rc;
+  if (quant && (rc = validate_qkv_quant(*quant, a))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
   const bool causal = a.causal != 0, f32 = a.out_fp32 != 0;
@@ -456,18 +418,22 @@ int fwd_impl(const Problem& a, void* const* extra_dst = nullptr, int n_extra = 0
   SplitPlan plan;
   if ((rc = plan_splits(a, plan))) return rc;
 
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
-  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-
   FwdParams p{};
   p.Sk = a.Sk;
   p.causal_off = causal ? a.Sk - a.Sq : 0;             // < 0: the first Sq - Sk rows see no key
   p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
   for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
   p.n_extra_dst = n_extra;
-  return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan);
+
+  // FP8: 8-bit swizzled Q / K maps the wgmma reads in place, the raw V map the converter transposes, and V's scale
+  const int dt = quant ? TFA_FP8_E4M3 : a.dtype;
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, dt, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, quant != nullptr))) return rc;
+  if ((rc = make_tmap(&tk, a.k, dt, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss, quant != nullptr))) return rc;
+  if ((rc = make_tmap(&tv, a.v, dt, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+  if (!quant) return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan);
+  p.v_scale = quant->v_scale;
+  return run_forward<tfa::kDenseFp8>(a, p, a.Sq, tq, tk, tv, plan);
 }
 
 Problem from_fwd_args(const tfa_fwd_args& a) {
@@ -509,60 +475,44 @@ Problem from_varlen_args(const tfa_attn_varlen_args& a) {
   return q;
 }
 
-int varlen_impl(const tfa_attn_varlen_args& va) {
-  const Problem a = from_varlen_args(va);
-  int rc = validate(a);
-  if (rc) return rc;
-  if (!va.cu_seqlens_q || !va.cu_seqlens_k ||
-      ((reinterpret_cast<uintptr_t>(va.cu_seqlens_q) | reinterpret_cast<uintptr_t>(va.cu_seqlens_k)) & 3u))
-    return TFA_EINVAL_SEQLENS;
+// cu_seqlens_q of a packed query batch, a non-null 4-byte aligned pointer, and max_seqlen_q in [1, total_q].
+template <typename Args>
+int validate_seqlens_q(const Args& va) {
+  if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
   if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
-  if (!arch_ok()) return TFA_EARCH;
-  init_dbg();
-
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
-  if ((rc = make_tmap(&tk, a.k, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
-  if ((rc = make_tmap(&tv, a.v, a.dtype, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
-
-  FwdParams p{};
-  p.cu_q = va.cu_seqlens_q;
-  p.cu_k = va.cu_seqlens_k;
-  p.total_q = a.Sq;
-  p.total_k = a.Sk;
-  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once.  One
-  // split holds every KV tile of any sequence.
-  return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+  return 0;
 }
 
-// The variable-length problem of tfa_attn_varlen_fwd() on e4m3 q / k / v: its checks in its order, then the
-// quantization's, then the kVarlenFp8 forward over the packed tensors as one batch entry of 8-bit swizzled Q / K maps
-// and the raw V map the converter transposes.
-int varlen_fp8_impl(const tfa_attn_varlen_args& va, const tfa_qkv_quant_args& quant) {
+// The variable-length forward over the packed tensors as one batch entry.  `quant` as fwd_impl, for the kVarlenFp8
+// forward.
+int varlen_impl(const tfa_attn_varlen_args& va, const tfa_qkv_quant_args* quant) {
   Problem a = from_varlen_args(va);
   int rc = validate(a);
   if (rc) return rc;
-  if (!va.cu_seqlens_q || !va.cu_seqlens_k ||
-      ((reinterpret_cast<uintptr_t>(va.cu_seqlens_q) | reinterpret_cast<uintptr_t>(va.cu_seqlens_k)) & 3u))
-    return TFA_EINVAL_SEQLENS;
-  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
-  if ((rc = validate_qkv_quant(quant, a))) return rc;
+  if ((rc = validate_seqlens_q(va))) return rc;
+  if (!va.cu_seqlens_k || (reinterpret_cast<uintptr_t>(va.cu_seqlens_k) & 3u)) return TFA_EINVAL_SEQLENS;
+  if (quant && (rc = validate_qkv_quant(*quant, a))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, TFA_FP8_E4M3, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, true))) return rc;
-  if ((rc = make_tmap(&tk, a.k, TFA_FP8_E4M3, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss, true))) return rc;
-  if ((rc = make_tmap(&tv, a.v, TFA_FP8_E4M3, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
 
   FwdParams p{};
   p.cu_q = va.cu_seqlens_q;
   p.cu_k = va.cu_seqlens_k;
   p.total_q = a.Sq;
   p.total_k = a.Sk;
-  p.v_scale = quant.v_scale;
-  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
-  return run_forward<tfa::kVarlenFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+
+  // FP8: as fwd_impl
+  const int dt = quant ? TFA_FP8_E4M3 : a.dtype;
+  CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, dt, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, quant != nullptr))) return rc;
+  if ((rc = make_tmap(&tk, a.k, dt, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss, quant != nullptr))) return rc;
+  if ((rc = make_tmap(&tv, a.v, dt, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
+  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once.  One
+  // split holds every KV tile of any sequence.
+  const SplitPlan one{1, 0x7fffffff};
+  if (!quant) return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, one);
+  p.v_scale = quant->v_scale;
+  return run_forward<tfa::kVarlenFp8>(a, p, va.max_seqlen_q, tq, tk, tv, one);
 }
 
 // The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
@@ -650,17 +600,14 @@ int validate_rotary(const tfa_attn_kvcache_args& ka, const Problem& a, const tfa
 
 // The FP8-cache arguments of a cache call whose other arguments passed: the element type, the scales, and cache
 // strides that keep every 1-byte TMA row and box 16-byte aligned.  Sets a.scale to the effective softmax scale
-// s' = fp32(softmax_scale * k_scale), and `qs` to the scales.  s' must stay a normal fp32 number (or 0 with
-// softmax_scale = 0): an overflow, or an underflow that would silently turn the call into uniform attention, is
-// TFA_EINVAL_SCALE.
+// s' = fp32(softmax_scale * k_scale), and `qs` to the scales.
 int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
   if (q.cache_dtype != TFA_FP8_E4M3) return TFA_EINVAL_KVQUANT;
   if (!(q.k_scale > 0.0f) || !std::isfinite(q.k_scale) || !(q.v_scale > 0.0f) || !std::isfinite(q.v_scale))
     return TFA_EINVAL_KVQUANT;
   if ((a.ksb % 16) || (a.ksh % 16) || (a.kss % 16)) return TFA_EINVAL_KVQUANT;
   const float s = a.scale * q.k_scale;
-  if (!scale_in_range(s)) return TFA_EINVAL_SCALE;
-  if (a.scale > 0.0f && !(s >= FLT_MIN)) return TFA_EINVAL_SCALE;
+  if (int rc = validate_fp8_scale(a.scale, s)) return rc;
   a.scale = s;
   qs.k_scale = q.k_scale;
   qs.v_scale = q.v_scale;
@@ -742,8 +689,7 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_kv_qua
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
-  if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
-  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
+  if ((rc = validate_seqlens_q(va))) return rc;
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (!arch_ok()) return TFA_EARCH;
@@ -800,17 +746,17 @@ int tfa_abi_version(void) { return TFA_ABI_VERSION; }
 
 int tfa_fwd_ex(const tfa_fwd_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return fwd_impl(from_fwd_args(*args));
+  return fwd_impl(from_fwd_args(*args), nullptr);
 }
 
 int tfa_attn_fwd(const tfa_attn_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return fwd_impl(from_attn_args(*args));
+  return fwd_impl(from_attn_args(*args), nullptr);
 }
 
 int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return varlen_impl(*args);
+  return varlen_impl(*args, nullptr);
 }
 
 int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
@@ -841,12 +787,12 @@ int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, co
 
 int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return fp8_impl(from_attn_args(*args), *quant);
+  return fwd_impl(from_attn_args(*args), quant);
 }
 
 int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return varlen_fp8_impl(*args, *quant);
+  return varlen_impl(*args, quant);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -864,7 +810,7 @@ size_t tfa_attn_workspace_bytes(const tfa_attn_args* args, int num_splits) {
 int tfa_fwd_multi(const tfa_fwd_args* args, void* const* extra_out, int n_extra) {
   if (!args) return TFA_EINVAL_PTR;
   if (n_extra < 0) return TFA_EINVAL_SHAPE;
-  return fwd_impl(from_fwd_args(*args), extra_out, n_extra);
+  return fwd_impl(from_fwd_args(*args), nullptr, extra_out, n_extra);
 }
 
 int tfa_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int S, int D, int dtype,
@@ -881,7 +827,7 @@ int tfa_fwd(const void* q, const void* k, const void* v, void* out, float* lse, 
   a.softmax_scale = softmax_scale;
   a.out_fp32 = 0;
   a.stream = cuda_stream;
-  return fwd_impl(from_fwd_args(a));
+  return fwd_impl(from_fwd_args(a), nullptr);
 }
 
 int tfa_fwd_host(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int S, int D,

@@ -1,6 +1,6 @@
 // tfa_fp8_fwd.cu -- instantiates the FP8 attention forward (kDenseFp8 of fa_fwd_sm90.cuh: Q, K and V in e4m3, both
-// products on 8-bit wgmma) and its launch (fa_fwd_launch.cuh) for tfa_api.cu, which declares this instantiation
-// `extern template`: 2 head dims x causal x output dtype x fp32 output x 2 schedules = 32 kernels.
+// products on 8-bit wgmma) and its launch (fa_fwd_launch.cuh, which declares this instantiation `extern template`):
+// 2 head dims x causal x output dtype x fp32 output x 2 schedules = 32 kernels.
 //
 // A translation unit of its own, as tfa_kvcache_fp8.cu, so that the existing instantiations are compiled exactly as
 // they were without this mode.

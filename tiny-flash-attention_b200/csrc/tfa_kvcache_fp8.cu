@@ -1,5 +1,5 @@
 // tfa_kvcache_fp8.cu -- instantiates the FP8-cache forwards (kCacheFp8, kVarlenCacheFp8 of fa_fwd_sm90.cuh) and their
-// launch (fa_fwd_launch.cuh) for tfa_api.cu, which declares these instantiations `extern template`.
+// launch (fa_fwd_launch.cuh, which declares these instantiations `extern template`).
 //
 // A translation unit of its own, as tfa_varlen_kvcache.cu: the device compiler optimises a translation unit as one
 // module, and new kernels instantiated next to the forward can change the generated code of the existing

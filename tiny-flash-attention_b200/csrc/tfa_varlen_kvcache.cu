@@ -1,5 +1,5 @@
-// tfa_varlen_kvcache.cu -- instantiates the kVarlenCache forward (fa_fwd_sm90.cuh) and its launch (fa_fwd_launch.cuh)
-// for tfa_api.cu, which declares this instantiation `extern template`.
+// tfa_varlen_kvcache.cu -- instantiates the kVarlenCache forward (fa_fwd_sm90.cuh) and its launch (fa_fwd_launch.cuh,
+// which declares this instantiation `extern template`).
 //
 // A translation unit of its own, as tfa_append.cu: the device compiler optimises a translation unit as one module,
 // and new kernels instantiated next to the forward can change the generated code of the existing instantiations.
