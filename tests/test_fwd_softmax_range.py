@@ -13,7 +13,9 @@ of very different magnitude one after another.  FP8 inputs are planted in float,
 reference is built from the codes.
 
 Emulation (`emulate`).  The kernel's online softmax per row, tile by tile from the item's first key, with the split
-boundaries of tfa_attn_num_splits: fp32 m and l, m set on tile 0 (-FLT_MAX / c while a row has no key), the rescale
+boundaries of tfa_attn_num_splits: fp32 m and l, l in the kernel's own order (each thread of a row's quad sums its
+16 pairs of a tile into a fresh partial, adds it into l with Kahan's compensated add, and the quad is summed by two
+xor-shuffles at the end; mutation running_l is the earlier order, one fp32 add per pair into l), m set on tile 0 (-FLT_MAX / c while a row has no key), the rescale
 decision `(mx - m) c > 8` with alpha = 2^((m - mx) c), P rounded to 16 bits or e4m3, every split through an fp32 LSE
 and the combine's formula.  It shows that each GPU workload's pattern drives what it is named for (coverage), that the budget
 covers it (soundness), and that the checker rejects a wrong rescale (six mutations).
@@ -49,7 +51,7 @@ import pytest
 import torch
 
 import test_fwd_fp8 as F8
-from test_fwd_float64_reference import OUT_EMIN, OUT_P, U_P, guarded, reference
+from test_fwd_float64_reference import L_SUM, OUT_EMIN, OUT_P, U_P, guarded, lse_bound, reference
 from test_kvcache_fp8 import FP8, bits, quantize
 from test_kvcache_rotary import positions, rope, rope_tables
 from test_varlen import offsets
@@ -195,7 +197,8 @@ def emulate(s, vis, v, scale, rnd, splits=None, mutation=None):
     for (k0, k1) in splits:
         m = np.zeros((H, R), np.float32)
         m_old = m.copy()
-        l = np.zeros((H, R), np.float32)
+        l = np.zeros((H, R, 4), np.float32)      # per thread of the row's quad: l and its Kahan compensation
+        lc = np.zeros((H, R, 4), np.float32)
         o = np.zeros((H, R, v.shape[2]))
         for t0 in range(k0, k1, BN):
             st = s[:, :, t0:min(t0 + BN, k1)]
@@ -214,7 +217,8 @@ def emulate(s, vis, v, scale, rnd, splits=None, mutation=None):
                 m_old = np.where(n, m, m_old)
                 m = np.where(n, mx, m)
                 if mutation != "no_l_rescale":
-                    l = (l * alpha).astype(np.float32)
+                    l = (l * alpha[..., None]).astype(np.float32)
+                    lc = (lc * alpha[..., None]).astype(np.float32)
                 if mutation == "swap_halves":        # alpha of row r applied to row r ^ 8
                     idx = np.arange(R)
                     idx[:R // 16 * 16] ^= 8
@@ -226,8 +230,26 @@ def emulate(s, vis, v, scale, rnd, splits=None, mutation=None):
             p = np.where(np.isnan(p), 0.0, p)
             tr.max_p = max(tr.max_p, float(p.max()) if p.size else 0.0)
             tr.small_p += int(((p > 0) & (p < small)).sum())
-            l = (l + p.astype(np.float64).sum(-1)).astype(np.float32)
+            # thread tq of a row's quad holds the tile's columns 8 i + 2 tq + e (i < 16, e < 2) and adds them in pairs
+            pad = np.zeros((H, R, BN), np.float32)
+            pad[..., :p.shape[-1]] = p
+            pairs = pad.reshape(H, R, 16, 4, 2)
+            pairs = (pairs[..., 0] + pairs[..., 1]).astype(np.float32)          # (H, R, i, tq)
+            if mutation == "running_l":          # the pairs straight into l, one fp32 add per pair
+                for i in range(16):
+                    l = (l + pairs[..., i, :]).astype(np.float32)
+            else:                                # a fresh tile partial, then Kahan's compensated add into l
+                t = pairs[..., 0, :]
+                for i in range(1, 16):
+                    t = (t + pairs[..., i, :]).astype(np.float32)
+                y = (t - lc).astype(np.float32)
+                u = (l + y).astype(np.float32)
+                lc = ((u - l).astype(np.float32) - y).astype(np.float32)
+                l = u
             o = o + np.einsum("hrk,hkd->hrd", _round_p(p, rnd), v[:, t0:min(t0 + BN, k1)])
+        l = (l - lc).astype(np.float32)
+        l = (l + l[..., [1, 0, 3, 2]]).astype(np.float32)                      # the two xor-shuffles of the quad
+        l = (l + l[..., [2, 3, 0, 1]]).astype(np.float32)[..., 0]
         if mutation == "no_reset":               # item h starts from item h - 1's l and O (a persistent CTA's)
             l, o = l.copy(), o.copy()
             l[1:] += l[:-1].copy()
@@ -264,21 +286,21 @@ def full_reference(sq, causal, scale, fp8, ks=1.0, vs=1.0):
     q, k, v = sq.q[None], sq.k[None], sq.v[None]
     if fp8:
         return F8.fp8_reference(q, k, v, causal, scale, 1.0, 1.0)
-    o, lse, a, sub = reference(q, k, v, causal, scale)
+    o, lse, a, sub, pv16 = reference(q, k, v, causal, scale)
     Hq, Hkv = q.shape[1], k.shape[1]
     kk = k[:, torch.arange(Hq) // (Hq // Hkv)]
     Sq, Sk = q.shape[2], k.shape[2]
     vis = (torch.arange(Sk)[None] <= torch.arange(Sq)[:, None] + Sk - Sq) if causal else torch.ones(Sq, Sk).bool()
     eta = ((q.abs().cpu() @ kk.abs().cpu().transpose(-1, -2)) * (scale * EPS_S)).masked_fill(~vis, 0.0).amax(-1)
-    return o, lse, a, sub, eta.to(q.device)
+    return o, lse, a, sub, eta.to(q.device), pv16
 
 
 def budget(ref, kind, out16, fp8, split):
-    o_ref, l_ref, a, extra, eta = ref
+    o_ref, l_ref, a, extra, eta = ref[:5]
     if fp8:
-        b = extra + torch.expm1(2 * eta)[..., None] * a + 2.0 ** -14 * a + 1e-6
+        b = extra + torch.expm1(2 * eta)[..., None] * a + 2.0 ** -14 * a + L_SUM * a + 1e-6
     else:
-        b = U_P[kind] * a + 2.0 ** -14 * a + 1e-6 + torch.expm1(2 * eta)[..., None] * a
+        b = U_P[kind] * a + 2.0 ** -14 * a + L_SUM * a + ref[5] + 1e-6 + torch.expm1(2 * eta)[..., None] * a
         if kind == "fp16":
             b = b + 2.0 ** -25 * extra
     if split:
@@ -301,7 +323,7 @@ def check(out, lse, ref, kind, fp8, split):
     b = budget(ref, kind, out.dtype != torch.float32, fp8, split)
     ratio = torch.nan_to_num((o - o_ref).abs() / b, nan=math.inf).masked_fill(keyless[..., None], 0.0)
     lerr = torch.nan_to_num((l - l_ref).abs(), nan=math.inf).masked_fill(keyless, 0.0)
-    lb = ref[4] + 1e-4 + 2e-6 * l_ref.abs().masked_fill(keyless, 0.0)
+    lb = ref[4] + lse_bound(l_ref.masked_fill(keyless, 0.0))
     r, le = float(ratio.max()) if ratio.numel() else 0.0, float(lerr.max()) if lerr.numel() else 0.0
     if r > 1.0:
         at = np.unravel_index(int(ratio.argmax()), tuple(ratio.shape))
@@ -756,6 +778,30 @@ def test_checker_rejects_wrong_rescale(name, mutation):
     assert not ok, f"{name}: {mutation} passes (ratio {ratio:.3f})"
 
 
+@pytest.mark.parametrize("Sk", [131072, 262144])
+def test_row_sum_order_keeps_lse_bound_on_a_constant_tail(Sk):
+    """One sink key and Sk - 1 keys at the same logit delta below it (repeated tokens, padding without rotary, FP8
+    keys that share a code): summed as one fp32 add per key pair into a running l, l drifts with the tile count past
+    the LSE bound 1e-4 + 2e-6 |LSE| (mutation running_l); the kernel's tile partials with a compensated add into l stay
+    far inside it at every delta."""
+    deltas = np.array([0.5, 1.0, 3.0, 6.0])
+    scale = 1.0 / LOG2E
+    s = np.zeros((1, len(deltas), Sk))
+    s[0, :, 1:] = -deltas[:, None] / scale
+    vis = np.ones((len(deltas), Sk), bool)
+    v = np.ones((1, Sk, 1))
+    lse_ref = np.log1p((Sk - 1) * np.exp(-deltas))
+    bound = 1e-4 + 2e-6 * np.abs(lse_ref)
+    err = {}
+    for mut in (None, "running_l"):
+        _, lse, _ = emulate(s, vis, v, scale, "bf16", mutation=mut)
+        err[mut] = np.abs(lse[0] - lse_ref)
+    print(f"\n[row sum] Sk {Sk}: |dLSE| per delta {deltas.tolist()}: tile partial + Kahan "
+          f"{err[None].tolist()}, running l {err['running_l'].tolist()}, bound {bound.tolist()}")
+    assert (err[None] <= bound / 16).all(), err[None]
+    assert (err["running_l"] > bound).any(), err["running_l"]
+
+
 # ------------------------------------------------------------------ CPU: the scale range --------------------------------
 
 def largest_scale():
@@ -1020,7 +1066,7 @@ def test_keyless_rows_exact_at_large_scales(tfa, monkeypatch, scale):
         keyless = 0
         for i, (out, lse, sq) in enumerate(r["seqs"]):
             fp8 = bool(w.kw.get("fp8"))
-            o_ref, l_ref, a, sub = reference(sq.q[None], sq.k[None], sq.v[None], True, s)
+            o_ref, l_ref, a, sub, pv16 = reference(sq.q[None], sq.k[None], sq.v[None], True, s)
             kl = torch.isinf(l_ref)
             keyless += int(kl.sum())
             o, l = out.double().cpu(), lse.double().cpu()
@@ -1029,7 +1075,7 @@ def test_keyless_rows_exact_at_large_scales(tfa, monkeypatch, scale):
                              f"(nan {int(torch.isnan(o[kl]).sum())})")
                 continue
             ref = (o_ref, l_ref, a, F8.fp8_reference(sq.q[None], sq.k[None], sq.v[None], True, s, 1.0, 1.0)[3]
-                   if fp8 else sub, torch.zeros_like(l_ref))
+                   if fp8 else sub, torch.zeros_like(l_ref), pv16)
             ok, ra, le, msg = check(out.cpu(), lse.cpu(), ref, w.kw["kind"], fp8,
                                     split_ranges(w, sq.k.shape[1]) is not None)
             if not ok:

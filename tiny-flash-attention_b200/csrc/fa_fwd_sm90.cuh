@@ -802,6 +802,11 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     uint32_t pf[DF8 ? 16 : 32];   // P as the A operand: 8 k-steps x 4 registers of 16-bit pairs (e4m3: 4 x 4 of e4m3x4)
     float m_lo = 0.f, m_hi = 0.f;     // reference max the exponentials are taken against (raw score units)
     float l_lo = 0.f, l_hi = 0.f;     // this thread's part of the running sum of exp2((s - m) * c)
+    // Kahan compensation of l: minus the low-order part the adds into l have lost.  Each tile's 32 values are summed
+    // into a fresh partial that is then added with compensation, so l's rounding error stays a few ulps at any key
+    // count (a plain running sum drifts with the number of tiles, past the LSE bound by 128K equal keys).
+    float lc_lo = 0.f, lc_hi = 0.f;
+    float tp_lo = 0.f, tp_hi = 0.f;   // the last tile's partial, added into l while the next wgmmas run
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
 
@@ -847,20 +852,23 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           rescale = true;
           if (n_lo) { a_lo = ex2_approx((m_lo - mx_lo) * c); m_lo = mx_lo; }
           if (n_hi) { a_hi = ex2_approx((m_hi - mx_hi) * c); m_hi = mx_hi; }
-          l_lo *= a_lo;
-          l_hi *= a_hi;
+          l_lo *= a_lo; lc_lo *= a_lo;
+          l_hi *= a_hi; lc_hi *= a_hi;
         }
       }
       const float nm_lo = -m_lo * c, nm_hi = -m_hi * c;
+      float t_lo = 0.f, t_hi = 0.f;               // this tile's part of l; l sums fp32 P, before the 16-bit rounding
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         s[4 * i + 0] = ex2_approx(fmaf(s[4 * i + 0], c, nm_lo));
         s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], c, nm_lo));
         s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], c, nm_hi));
         s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], c, nm_hi));
-        l_lo += s[4 * i + 0] + s[4 * i + 1];      // l sums fp32 P, before the 16-bit rounding
-        l_hi += s[4 * i + 2] + s[4 * i + 3];
+        t_lo += s[4 * i + 0] + s[4 * i + 1];
+        t_hi += s[4 * i + 2] + s[4 * i + 3];
       }
+      tp_lo = t_lo;
+      tp_hi = t_hi;
     };
     // P (fp32 accumulator layout) -> A-operand registers: k-step kk = column groups 2kk, 2kk+1
     // kDenseFp8: P <= 2^8 < 448 (the lazy rescale's bound) is in e4m3 range
@@ -906,6 +914,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         issue_S(s, kslot);
         mbar_wait(&vr_full[vslot], (ev / NVR) & 1, p.dbg, SITE_MMA_V, ev);
         issue_PV(o, pf, vslot, j > 1);
+        kahan_add(l_lo, lc_lo, tp_lo);                 // tile j - 1's partial, before softmax(j) may rescale l
+        kahan_add(l_hi, lc_hi, tp_hi);
         wgmma_wait<1>();                               // S_j done
         reg_fence(s);
         release(&kr_empty[kslot]);
@@ -931,6 +941,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         zero_v_tail(vslot, n - 1);
         wgmma_fence();
         issue_PV(o, pf, vslot, n > 1);
+        kahan_add(l_lo, lc_lo, tp_lo);
+        kahan_add(l_hi, lc_hi, tp_hi);
         wgmma_wait<0>();
         reg_fence(o);
         release(&vr_empty[vslot]);
@@ -939,6 +951,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
 
     // ---------------------------- epilogue ----------------------------
+    l_lo -= lc_lo;
+    l_hi -= lc_hi;
 #pragma unroll
     for (int d = 1; d <= 2; d <<= 1) {
       l_lo += __shfl_xor_sync(0xffffffffu, l_lo, d);

@@ -290,6 +290,14 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// Kahan's compensated add of x into sum; comp holds minus the low-order part lost so far (the total is sum - comp).
+// The _rn intrinsics keep the four adds as written: the compiler neither reassociates nor fuses them.
+__device__ __forceinline__ void kahan_add(float& sum, float& comp, float x) {
+  const float y = __fsub_rn(x, comp);
+  const float t = __fadd_rn(sum, y);
+  comp = __fsub_rn(__fsub_rn(t, sum), y);
+  sum = t;
+}
 // pack two fp32 -> one 32-bit word of 16-bit floats; `lo` lands in bits [0,16)
 template <bool IS_BF16>
 __device__ __forceinline__ uint32_t pack_16x2(float lo, float hi) {
