@@ -280,7 +280,8 @@ typedef struct tfa_rotary_args {
 int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary);
 
 /* ---- a variable-length batch of queries against a (paged) KV cache: the mixed prefill / decode step of a
- * continuous-batching loop (flash-attn's flash_attn_varlen_func with block_table and seqused_k) ----
+ * continuous-batching loop (flash-attn's flash_attn_varlen_func with block_table and seqused_k; with rotary see
+ * tfa_attn_varlen_kvcache_rotary_fwd below) ----
  * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
  * tfa_attn_varlen_kvcache_fwd.  Queries as tfa_attn_varlen_fwd(), keys and values as tfa_attn_kvcache_fwd().
  *
@@ -368,6 +369,37 @@ typedef struct tfa_kv_quant_args {
 int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary /* NULL: none */,
                              const tfa_kv_quant_args* quant);
 int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant);
+
+/* ---- the variable-length KV-cache call with rotary position embedding, on a 16-bit or an FP8 cache ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect it by the exported symbol
+ * tfa_attn_varlen_kvcache_rotary_fwd.  tfa_attn_varlen_kvcache_fwd() (with `quant`: tfa_attn_varlen_kvcache_fp8_fwd())
+ * with, before the attention, the packed q rows and k_new rotated at each sequence's cache positions in the append's
+ * launch, as tfa_attn_kvcache_rotary_fwd() does for the dense-query call: rot(q) goes to q_rot, which the attention
+ * reads in place of q, and rot(k_new) with the unrotated v_new goes into the cache (quantized into an FP8 one as
+ * tfa_attn_kvcache_fp8_fwd() with rotary does).  The caller's q and k_new are not modified.
+ *
+ *   cos, sin, seqlen_ro, rotary_dim, interleaved : as tfa_attn_kvcache_rotary_fwd() (seqlen_ro >= capacity).
+ *   q_rot      : (total_q, Hq, D) contiguous DEVICE scratch in q's dtype, 16-byte aligned; it must not overlap any
+ *              other argument.  After the call, rows cu[b] + i, i < n_b, hold rot(q) for every sequence b; other rows
+ *              are unspecified and do not influence any result.
+ *   lengths    : those of tfa_attn_varlen_kvcache_fwd() with k_new: n_b = min(Sq_b, max_seqlen_q) on the clamped
+ *              offsets, L_b = clamp(cache_seqlens[b], 0, max(capacity - n_b, 0)).
+ *   positions  : appended key i < min(n_b, capacity) of sequence b is rotated at L_b + i (the slot it is stored in);
+ *              query row i < n_b at L_b + i when causal, at L_b for every row otherwise; every position is clamped to
+ *              seqlen_ro - 1.  With n_b <= capacity, sequence b is rotated exactly as tfa_attn_kvcache_rotary_fwd()
+ *              rotates one sequence with Sq = Snew = n_b.
+ *   quant      : NULL for a 16-bit cache; otherwise the FP8 (e4m3) cache's tfa_kv_quant_args, as
+ *              tfa_attn_varlen_kvcache_fp8_fwd().
+ * k_new / v_new are required (TFA_EINVAL_ROTARY otherwise).  out and lse are those of tfa_attn_varlen_kvcache_fwd().
+ * Every argument is checked before any device work, in this order: the cache arguments (TFA_EINVAL_KVCACHE), the
+ * shapes, strides and scale, cu_seqlens_q / max_seqlen_q (TFA_EINVAL_SEQLENS), the rotary arguments
+ * (TFA_EINVAL_ROTARY), with `quant` the FP8 ones (TFA_EINVAL_KVQUANT, then TFA_EINVAL_SCALE for s'), then the device
+ * (TFA_EARCH).  A NULL args or rotary is TFA_EINVAL_PTR.  Launches: 2 (the rotary append, the attention).  The host
+ * never reads cu_seqlens_q, cache_seqlens or block_table: the call can be captured in a CUDA graph and replayed with
+ * new contents of the same total_q.  Whatever cu_seqlens_q holds, no store leaves q_rot and no cos / sin read leaves
+ * the table. */
+int tfa_attn_varlen_kvcache_rotary_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
+                                       const tfa_kv_quant_args* quant /* NULL: 16-bit cache */);
 
 /* ---- attention on FP8 (e4m3) q, k and v with per-tensor scales, both products on FP8 tensor cores (FlashAttention-3's
  * descale_q / descale_k / descale_v) ----

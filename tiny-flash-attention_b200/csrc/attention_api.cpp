@@ -498,11 +498,11 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache(torch::Tensor q, torch::Te
 
 namespace {
 
-// The rotary arguments of a cache call (c checked): the tfa_rotary_args but q_rot.  Throws before any device work.
-tfa_rotary_args check_rotary(const KvcacheCall& c, const torch::Tensor& rotary_cos, const torch::Tensor& rotary_sin,
-                             bool rotary_interleaved) {
-  const torch::Tensor& q = c.q;
-  TORCH_CHECK(c.snew > 0, "rotary needs k_new and v_new: it rotates the appended keys");
+// The rotary arguments of either cache call (its other arguments checked), which reads of the call q, the head dim D,
+// the capacity and whether it appends: the tfa_rotary_args but q_rot.  Throws before any device work.
+tfa_rotary_args check_rotary(const torch::Tensor& q, int64_t D, int64_t capacity, bool append,
+                             const torch::Tensor& rotary_cos, const torch::Tensor& rotary_sin, bool rotary_interleaved) {
+  TORCH_CHECK(append, "rotary needs k_new and v_new: it rotates the appended keys");
   TORCH_CHECK(rotary_cos.device() == q.device() && rotary_sin.device() == q.device(),
               "rotary_cos and rotary_sin must be on q's device");
   TORCH_CHECK(rotary_cos.scalar_type() == q.scalar_type() && rotary_sin.scalar_type() == q.scalar_type(),
@@ -511,13 +511,13 @@ tfa_rotary_args check_rotary(const KvcacheCall& c, const torch::Tensor& rotary_c
               "rotary_cos and rotary_sin must both be (seqlen_ro, rotary_dim / 2)");
   TORCH_CHECK(rotary_cos.is_contiguous() && rotary_sin.is_contiguous(), "rotary_cos and rotary_sin must be contiguous");
   const int64_t seqlen_ro = rotary_cos.size(0), rotary_dim = 2 * rotary_cos.size(1);
-  TORCH_CHECK(rotary_dim >= 16 && rotary_dim <= c.D && rotary_dim % 16 == 0,
+  TORCH_CHECK(rotary_dim >= 16 && rotary_dim <= D && rotary_dim % 16 == 0,
               fmt_msg("rotary_dim (2 * rotary_cos.size(1) = %lld) must be a multiple of 16 in [16, head_dim = %lld]",
-                      static_cast<long long>(rotary_dim), static_cast<long long>(c.D)));
+                      static_cast<long long>(rotary_dim), static_cast<long long>(D)));
   TORCH_CHECK(seqlen_ro < (1LL << 31), "rotary_cos and rotary_sin are too large");
-  TORCH_CHECK(seqlen_ro >= c.mbps * c.page,
+  TORCH_CHECK(seqlen_ro >= capacity,
               fmt_msg("rotary_cos / rotary_sin need a row per cache position: seqlen_ro = %lld < capacity = %lld",
-                      static_cast<long long>(seqlen_ro), static_cast<long long>(c.mbps * c.page)));
+                      static_cast<long long>(seqlen_ro), static_cast<long long>(capacity)));
   tfa_rotary_args r;
   r.cos = rotary_cos.data_ptr(); r.sin = rotary_sin.data_ptr();
   r.seqlen_ro = static_cast<int32_t>(seqlen_ro); r.rotary_dim = static_cast<int32_t>(rotary_dim);
@@ -549,7 +549,7 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_rotary(
     torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved, bool is_causal, float softmax_scale,
     int64_t num_splits) {
   KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits);
-  tfa_rotary_args r = check_rotary(c, rotary_cos, rotary_sin, rotary_interleaved);
+  tfa_rotary_args r = check_rotary(c.q, c.D, c.mbps * c.page, c.snew > 0, rotary_cos, rotary_sin, rotary_interleaved);
   return kvcache_fwd(c, is_causal, softmax_scale, num_splits, &r, nullptr);
 }
 
@@ -565,7 +565,8 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
   const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
   TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
   tfa_rotary_args r;
-  if (rotary_cos.has_value()) r = check_rotary(c, *rotary_cos, *rotary_sin, rotary_interleaved);
+  if (rotary_cos.has_value())
+    r = check_rotary(c.q, c.D, c.mbps * c.page, c.snew > 0, *rotary_cos, *rotary_sin, rotary_interleaved);
   return kvcache_fwd(c, is_causal, softmax_scale, num_splits, rotary_cos.has_value() ? &r : nullptr, &qa);
 }
 
@@ -576,12 +577,15 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
 // query rows) before the attention.  Returns out (total_q, Hq, D) and lse (Hq, total_q).  No split-KV.
 namespace {
 
-// flash_attention_v2_varlen_kvcache, or with `quant` its FP8-cache form.
+// flash_attention_v2_varlen_kvcache, or with `quant` its FP8-cache form; with rotary_cos / rotary_sin, q and k_new
+// are rotated first (tfa_attn_varlen_kvcache_rotary_fwd) through a q_rot allocated here.
 std::vector<torch::Tensor> varlen_kvcache(
     const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
     const torch::Tensor& cu_seqlens_q, int64_t max_seqlen_q, const torch::Tensor& cache_seqlens,
     const std::optional<torch::Tensor>& block_table, const std::optional<torch::Tensor>& k_new,
-    const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant) {
+    const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant,
+    const std::optional<torch::Tensor>& rotary_cos = std::nullopt,
+    const std::optional<torch::Tensor>& rotary_sin = std::nullopt, bool rotary_interleaved = false) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
@@ -609,8 +613,12 @@ std::vector<torch::Tensor> varlen_kvcache(
   TORCH_CHECK(total_q < (1LL << 31) && B < (1LL << 31) && nblk < (1LL << 31) && page < (1LL << 31) &&
                   mbps < (1LL << 31),
               "tensors too large");
+  TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
+  tfa_rotary_args r;
+  if (rotary_cos.has_value())
+    r = check_rotary(q, D, mbps * page, k_new.has_value(), *rotary_cos, *rotary_sin, rotary_interleaved);
 
-  torch::Tensor out, lse;
+  torch::Tensor out, lse, q_rot;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
@@ -639,7 +647,13 @@ std::vector<torch::Tensor> varlen_kvcache(
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    rc = quant ? tfa_attn_varlen_kvcache_fp8_fwd(&a, quant) : tfa_attn_varlen_kvcache_fwd(&a);
+    if (rotary_cos.has_value()) {
+      q_rot = torch::empty({total_q, Hq, D}, q.options().memory_format(at::MemoryFormat::Contiguous));
+      r.q_rot = q_rot.data_ptr();
+      rc = tfa_attn_varlen_kvcache_rotary_fwd(&a, &r, quant);
+    } else {
+      rc = quant ? tfa_attn_varlen_kvcache_fp8_fwd(&a, quant) : tfa_attn_varlen_kvcache_fwd(&a);
+    }
   }
   raise_on_error(rc);
   return {out, lse};
@@ -655,15 +669,28 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
                         is_causal, softmax_scale, nullptr);
 }
 
+// The same with rotary position embedding: q and k_new are rotated at each sequence's cache positions
+// (tfa_attn_varlen_kvcache_rotary_fwd in include/tfa_b200.h) before the attention; the caller's q and k_new are not
+// modified.  rotary_cos / rotary_sin as flash_attention_v2_kvcache_rotary; k_new / v_new are required.
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_rotary(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved,
+    bool is_causal, float softmax_scale) {
+  return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
+                        is_causal, softmax_scale, nullptr, rotary_cos, rotary_sin, rotary_interleaved);
+}
+
 // The same against an FP8 cache (float8_e4m3fn k_cache / v_cache with per-tensor k_scale / v_scale), as
-// flash_attention_v2_kvcache_fp8.
+// flash_attention_v2_kvcache_fp8, with optional rotary as flash_attention_v2_varlen_kvcache_rotary.
 std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_fp8(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
-    std::optional<torch::Tensor> v_new, double k_scale, double v_scale, bool is_causal, float softmax_scale) {
+    std::optional<torch::Tensor> v_new, double k_scale, double v_scale, bool is_causal, float softmax_scale,
+    std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin, bool rotary_interleaved) {
   const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
-                        is_causal, softmax_scale, &qa);
+                        is_causal, softmax_scale, &qa, rotary_cos, rotary_sin, rotary_interleaved);
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -707,7 +734,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_varlen_kvcache_fp8", &flash_attention_v2_varlen_kvcache_fp8,
         "a packed variable-length batch of queries against an FP8 (float8_e4m3fn) cache with per-tensor scales: (q, "
         "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, k_scale, v_scale, "
-        "is_causal, scale)");
+        "is_causal, scale), optional rotary",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
+        py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("k_scale"),
+        py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("rotary_cos") = py::none(),
+        py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
+  m.def("flash_attention_v2_varlen_kvcache_rotary", &flash_attention_v2_varlen_kvcache_rotary,
+        "the variable-length KV-cache call with q and k_new rotated (RoPE) at each sequence's cache positions: (q, "
+        "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, rotary_cos, "
+        "rotary_sin, rotary_interleaved, is_causal, scale)");
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

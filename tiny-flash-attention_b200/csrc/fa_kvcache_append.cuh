@@ -1,7 +1,7 @@
 // fa_kvcache_append.cuh -- the KV-cache append of both cache calls, launched from tfa_append.cu before the forward
 // reads the cache: kvcache_append_kernel writes k_new / v_new into the (paged) cache, with two compile-time switches.
-//   * ROTARY (dense-query call only): q and k_new are rotated (RoPE) at their cache positions on the way, and rot(q)
-//     goes to a scratch buffer the forward reads in place of q.
+//   * ROTARY: q and k_new are rotated (RoPE) at their cache positions on the way, and rot(q) goes to a scratch buffer
+//     the forward reads in place of q.
 //   * FP8: the cache is e4m3 with per-tensor scales; k_new / v_new (rot(k_new) with ROTARY) are quantized on the way.
 #pragma once
 #include "ptx_sm90.cuh"
@@ -33,10 +33,26 @@ struct AppendParams {
   long long chunks;               // B * snew * Hkv * D / 8
 };
 
-// Chunk c < p.chunks of the append: 16-byte chunk `sub` of appended token i of sequence b at head h, read at element
-// src of k_new / v_new and written at element dst of the caches, or dropped (dst < 0).
+// The rows of sequence b: the dense-query call's n = snew rows of its own; the variable-length call's packed rows
+// [q0, q0 + n) with n = min(Sq_b, snew), taken with the forward's clamps (decode_item), so that whatever cu_seqlens
+// holds no row outside [0, total_q) is read or written.  n is also the count of keys the sequence appends.
+struct SeqRows {
+  int q0, n;
+};
+__device__ __forceinline__ SeqRows seq_rows(const AppendParams& p, int b) {
+  SeqRows s{0, p.snew};
+  if (p.cu_q) {
+    s.q0 = min(max(__ldg(p.cu_q + b), 0), p.total_q);
+    const int q1 = min(max(__ldg(p.cu_q + b + 1), 0), p.total_q);
+    s.n = min(max(q1 - s.q0, 0), p.snew);
+  }
+  return s;
+}
+
+// Chunk c < p.chunks of the append: 16-byte chunk `sub` of appended token i of sequence b (which appends n keys) at
+// head h, read at element src of k_new / v_new and written at element dst of the caches, or dropped (dst < 0).
 struct AppendChunk {
-  int b, i, h, sub;
+  int b, i, h, sub, n;
   long long src, dst;
 };
 template <int D>
@@ -49,16 +65,11 @@ __device__ __forceinline__ AppendChunk append_chunk(const AppendParams& p, long 
   r /= p.Hkv;
   a.i = static_cast<int>(r % p.snew);
   a.b = static_cast<int>(r / p.snew);
-  int q0 = 0, n = p.snew;
-  if (p.cu_q) {
-    // the forward's clamps (decode_item): whatever cu_seqlens holds, no row outside [0, total_q) is read
-    q0 = min(max(__ldg(p.cu_q + a.b), 0), p.total_q);
-    const int q1 = min(max(__ldg(p.cu_q + a.b + 1), 0), p.total_q);
-    n = min(max(q1 - q0, 0), p.snew);
-  }
-  a.dst = append_offset(__ldg(p.cache_seqlens + a.b), p.block_table, p.bt_stride, a.b, a.i, a.h, p.page, p.capacity, n,
-                        p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
-  a.src = a.b * p.n_sb + (q0 + a.i) * p.n_ss + a.h * p.n_sh;
+  const SeqRows s = seq_rows(p, a.b);
+  a.n = s.n;
+  a.dst = append_offset(__ldg(p.cache_seqlens + a.b), p.block_table, p.bt_stride, a.b, a.i, a.h, p.page, p.capacity,
+                        s.n, p.num_blocks, p.c_sb, p.c_ss, p.c_sh);
+  a.src = a.b * p.n_sb + (s.q0 + a.i) * p.n_ss + a.h * p.n_sh;
   return a;
 }
 
@@ -70,6 +81,18 @@ __device__ __forceinline__ AppendChunk append_chunk(const AppendParams& p, long 
 __host__ __device__ __forceinline__ int rotary_pos(int cache_len, int i, bool causal, bool is_query, int seqlen_ro) {
   const int pos = (is_query && !causal) ? cache_len : cache_len + i;
   return min(pos, seqlen_ro - 1);
+}
+// The position rule of both cache calls: query row or appended key i of a sequence that appends n keys, with
+// raw = cache_seqlens[b], sits at rotary_pos() of the clamped cached length L_b that cache_lens() gives for those n
+// keys -- the length append_offset() stores the keys at and decode_item() attends from.  The dense-query call has
+// n = Snew <= capacity, where L_b is cache_len(raw, capacity, Snew); the variable-length call has n = n_b, which may
+// exceed the capacity.  n must be the sequence's own count: with max_seqlen_q in its place, a short sequence near the
+// capacity would be rotated at positions other than the slots its keys are stored in.
+__host__ __device__ __forceinline__ int seq_rotary_pos(int raw, int capacity, int n, int i, bool causal, bool is_query,
+                                                       int seqlen_ro) {
+  int L, K;
+  cache_lens(raw, capacity, n, L, K);
+  return rotary_pos(L, i, causal, is_query, seqlen_ro);
 }
 
 // fp32 arithmetic with one IEEE rounding each, written as PTX so that nvcc can neither contract a product and a sum
@@ -144,16 +167,19 @@ __device__ __forceinline__ uint4 rotate_chunk(const uint16_t* row, int sub, cons
 }
 
 // The parameter block of kvcache_append_kernel: the append, and the rotated queries of a ROTARY launch.  Without
-// ROTARY only `ap` is read and q_chunks is 0.  With it, chunks [0, q_chunks) write rot(q) into the contiguous
-// (B, Sq, Hq, D) buffer q_rot, and the remaining ap.chunks ones write rot(k_new) and v_new (unrotated) into the cache,
-// through append_chunk().  Positions: rotary_pos().  A NeoX chunk also reads its partner chunk, and every rotated chunk
-// 16 bytes each of cos and sin.  Algorithmic bytes of the rotated queries: 2 * B*Sq*Hq*D * 2 (q in, q_rot out), plus
-// the cos/sin rows.
+// ROTARY only `ap` is read and q_chunks is 0.  With it, chunks [0, q_chunks) write rot(q) into q_rot, and the remaining
+// ap.chunks ones write rot(k_new) and v_new (unrotated) into the cache, through append_chunk().  The query chunks cover
+// Sq rows of every sequence, as the key chunks cover snew: the dense-query call's Sq rows of (B, Sq, Hq, D) q, written
+// to the contiguous (B, Sq, Hq, D) q_rot; or, packed (ap.cu_q set, Sq = snew = max_seqlen_q), rows q0_b + i of
+// (total_q, Hq, D) q for i < n_b (seq_rows()), written to the same rows of the contiguous (total_q, Hq, D) q_rot -- a
+// chunk with i >= n_b returns.  Positions: seq_rotary_pos().  A NeoX chunk also reads its partner chunk, and every
+// rotated chunk 16 bytes each of cos and sin.  Algorithmic bytes of the rotated queries: 2 * (query rows)*Hq*D * 2
+// (q in, q_rot out), plus the cos/sin rows.
 struct AppendKernelParams {
   AppendParams ap;                // the append; ap.chunks = B * snew * Hkv * D / 8
   const void* q;
-  void* q_rot;                    // (B, Sq, Hq, D) contiguous
-  long long q_sb, q_ss, q_sh;     // element strides of q
+  void* q_rot;                    // (B, Sq, Hq, D) contiguous; packed: (total_q, Hq, D)
+  long long q_sb, q_ss, q_sh;     // element strides of q (q_sb = 0 when packed)
   const void* cos;                // (seqlen_ro, rotary_dim / 2) contiguous, q's dtype
   const void* sin;
   int Sq, Hq, rotary_dim, seqlen_ro, causal;
@@ -208,13 +234,15 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendKernelP
       r /= p.Hq;
       const int i = static_cast<int>(r % p.Sq);
       const int b = static_cast<int>(r / p.Sq);
-      const int len = cache_len(__ldg(a.cache_seqlens + b), a.capacity, a.snew);
-      const long long ro =
-          static_cast<long long>(rotary_pos(len, i, p.causal != 0, true, p.seqlen_ro)) * (p.rotary_dim / 2);
-      const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + i * p.q_ss + h * p.q_sh;
+      const SeqRows s = seq_rows(a, b);
+      if (a.cu_q && i >= s.n) return;          // packed: past the sequence's rows
+      const long long ro = static_cast<long long>(seq_rotary_pos(__ldg(a.cache_seqlens + b), a.capacity, s.n, i,
+                                                                 p.causal != 0, true, p.seqlen_ro)) *
+                           (p.rotary_dim / 2);
+      const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + (s.q0 + i) * p.q_ss + h * p.q_sh;
       const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_tab + ro, sin_tab + ro, p.rotary_dim);
-      reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + ((static_cast<long long>(b) * p.Sq + i) * p.Hq + h) * D)
-          [sub] = y;
+      const long long out_row = a.cu_q ? static_cast<long long>(s.q0) + i : static_cast<long long>(b) * p.Sq + i;
+      reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + (out_row * p.Hq + h) * D)[sub] = y;
       return;
     }
     c -= p.q_chunks;
@@ -224,9 +252,9 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendKernelP
   if (k.dst < 0) return;
   uint4 kx, vx;
   if constexpr (ROTARY) {
-    const int len = cache_len(__ldg(a.cache_seqlens + k.b), a.capacity, a.snew);
-    const long long ro =
-        static_cast<long long>(rotary_pos(len, k.i, p.causal != 0, false, p.seqlen_ro)) * (p.rotary_dim / 2);
+    const long long ro = static_cast<long long>(seq_rotary_pos(__ldg(a.cache_seqlens + k.b), a.capacity, k.n, k.i,
+                                                               p.causal != 0, false, p.seqlen_ro)) *
+                         (p.rotary_dim / 2);
     kx = rotate_chunk<IS_BF16, INTERLEAVED>(static_cast<const uint16_t*>(a.k_new) + k.src, k.sub, cos_tab + ro,
                                             sin_tab + ro, p.rotary_dim);
     vx = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(a.v_new) + k.src) + k.sub);

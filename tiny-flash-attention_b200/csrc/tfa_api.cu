@@ -586,8 +586,9 @@ int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtens
   return 0;
 }
 
-// The rotary arguments of a cache call whose cache arguments passed (capacity = a.Sk).
-int validate_rotary(const tfa_attn_kvcache_args& ka, const Problem& a, const tfa_rotary_args& ra) {
+// The rotary arguments of either cache call whose cache arguments passed (capacity = a.Sk).
+template <typename Args>
+int validate_rotary(const Args& ka, const Problem& a, const tfa_rotary_args& ra) {
   if (!ra.cos || !ra.sin || !ra.q_rot ||
       ((reinterpret_cast<uintptr_t>(ra.cos) | reinterpret_cast<uintptr_t>(ra.sin) |
         reinterpret_cast<uintptr_t>(ra.q_rot)) & 15u))
@@ -683,27 +684,45 @@ Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
   return q;
 }
 
-// `quant` as kvcache_impl.
-int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_kv_quant_args* quant) {
+// `ra` and `quant` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and the forward
+// reads its queries from ra->q_rot.
+int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* ra,
+                        const tfa_kv_quant_args* quant) {
   Problem a = from_varlen_kvcache_args(va);
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if ((rc = validate_seqlens_q(va))) return rc;
+  if (ra && (rc = validate_rotary(va, a, *ra))) return rc;
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
 
+  tfa::AppendKernelParams rp{};         // without rotary only rp.ap is used
+  if (ra) {
+    // the query chunks cover max_seqlen_q rows of every sequence, as the key chunks do (the append returns past n_b)
+    rp.q = a.q; rp.q_rot = ra->q_rot;
+    rp.q_sb = 0; rp.q_ss = a.qss; rp.q_sh = a.qsh;
+    rp.cos = ra->cos; rp.sin = ra->sin;
+    rp.Sq = va.max_seqlen_q; rp.Hq = a.Hq; rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
+    rp.causal = a.causal != 0 ? 1 : 0;
+    rp.q_chunks = static_cast<long long>(a.B) * va.max_seqlen_q * a.Hq * (a.D / 8);
+    // the forward reads rot(q), contiguous (total_q, Hq, D); out and lse are unchanged (ol)
+    a.q = ra->q_rot;
+    a.qss = static_cast<long long>(a.Hq) * a.D;
+    a.qsh = a.D;
+  }
+
   CUtensorMap tq, tk, tv;
-  tfa::AppendKernelParams rp{};         // no rotary: only rp.ap is used
   FwdParams p{};
   if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
   if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
-  if (va.k_new) {
+  if (va.k_new) {                       // rotary needs k_new (validate_rotary): every rotary call appends
     rp.ap.cu_q = va.cu_seqlens_q;
     rp.ap.total_q = a.Sq;
-    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, false, false, a.stream);
+    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
+                                    ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
 
@@ -771,7 +790,13 @@ int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rot
 
 int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, nullptr);
+  return varlen_kvcache_impl(*args, nullptr, nullptr);
+}
+
+int tfa_attn_varlen_kvcache_rotary_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
+                                       const tfa_kv_quant_args* quant) {
+  if (!args || !rotary) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args, rotary, quant);
 }
 
 int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary,
@@ -782,7 +807,7 @@ int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary
 
 int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, quant);
+  return varlen_kvcache_impl(*args, nullptr, quant);
 }
 
 int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant) {
@@ -956,6 +981,11 @@ long long tfa_internal_varlen_append_offset(int raw, const int* block_table, lon
 // development aid (not in the public header): the rotary position rule of fa_kvcache_append.cuh on the host
 int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {
   return tfa::rotary_pos(cache_len, i, causal != 0, is_query != 0, seqlen_ro);
+}
+// development aid (not in the public header): the position rule of both cache calls (seq_rotary_pos) on the host --
+// query row or appended key i of a sequence with raw = cache_seqlens[b] that appends n keys
+int tfa_internal_seq_rotary_pos(int raw, int capacity, int n, int i, int causal, int is_query, int seqlen_ro) {
+  return tfa::seq_rotary_pos(raw, capacity, n, i, causal != 0, is_query != 0, seqlen_ro);
 }
 // development aid (not in the public header): kDenseFp8's key order of P (fa_fwd_sm90.cuh) on the host -- pi of a
 // 32-key block's A column, the accumulator element the packer puts into byte x of A register r, and the key the

@@ -154,6 +154,9 @@ def lib():
         L.tfa_attn_kvcache_fp8_fwd.restype = ci
         L.tfa_attn_varlen_kvcache_fp8_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(KvQuantArgs)]
         L.tfa_attn_varlen_kvcache_fp8_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_rotary_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(RotaryArgs),
+                                                         ctypes.POINTER(KvQuantArgs)]
+        L.tfa_attn_varlen_kvcache_rotary_fwd.restype = ci
         L.tfa_attn_fp8_fwd.argtypes = [ctypes.POINTER(AttnArgs), ctypes.POINTER(QkvQuantArgs)]
         L.tfa_attn_fp8_fwd.restype = ci
         L.tfa_attn_varlen_fp8_fwd.argtypes = [ctypes.POINTER(VarlenArgs), ctypes.POINTER(QkvQuantArgs)]
@@ -347,6 +350,22 @@ def _quant(k_cache, k_scale, v_scale):
     return KvQuantArgs(TFA_FP8_E4M3, float(k_scale), float(v_scale))
 
 
+def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream):
+    """The RotaryArgs of a cache call with q (its q_rot: a contiguous tensor of q's shape and dtype, or a buffer
+    allocated here and kept alive as the split workspace is), or None without rotary_cos."""
+    import torch
+    if rotary_cos is None:
+        return None
+    assert rotary_sin is not None and rotary_cos.dim() == 2 and rotary_cos.shape == rotary_sin.shape
+    assert rotary_cos.is_contiguous() and rotary_sin.is_contiguous()
+    if q_rot is None:
+        q_rot = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+        _WORKSPACES[("q_rot", q.device.index, int(stream))] = q_rot
+    assert q_rot.shape == q.shape and q_rot.dtype == q.dtype and q_rot.is_contiguous()
+    return RotaryArgs(rotary_cos.data_ptr(), rotary_sin.data_ptr(), rotary_cos.shape[0], 2 * rotary_cos.shape[1],
+                      int(bool(rotary_interleaved)), q_rot.data_ptr())
+
+
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
                      scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
                      rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None, k_scale=1.0, v_scale=1.0):
@@ -384,16 +403,7 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
     n = _split_workspace(dense, a, q.device, st)
-    r = None
-    if rotary_cos is not None:
-        assert rotary_sin is not None and rotary_cos.dim() == 2 and rotary_cos.shape == rotary_sin.shape
-        assert rotary_cos.is_contiguous() and rotary_sin.is_contiguous()
-        if q_rot is None:
-            q_rot = torch.empty((B, Sq, Hq, D), dtype=q.dtype, device=q.device)
-            _WORKSPACES[("q_rot", q.device.index, int(st))] = q_rot      # kept alive as the split workspace is
-        assert q_rot.shape == q.shape and q_rot.dtype == q.dtype and q_rot.is_contiguous()
-        r = RotaryArgs(rotary_cos.data_ptr(), rotary_sin.data_ptr(), rotary_cos.shape[0], 2 * rotary_cos.shape[1],
-                       int(bool(rotary_interleaved)), q_rot.data_ptr())
+    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
     if quant is not None:
         check(lib().tfa_attn_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
                                              ctypes.byref(quant)))
@@ -408,13 +418,16 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
 
 def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
                             v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None,
-                            k_scale=1.0, v_scale=1.0):
+                            k_scale=1.0, v_scale=1.0, rotary_cos=None, rotary_sin=None, rotary_interleaved=False,
+                            q_rot=None):
     """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
     (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
     and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
     sharing cu_q, appended in place.  torch.float8_e4m3fn caches go through tfa_attn_varlen_kvcache_fp8_fwd() with
-    the per-tensor k_scale / v_scale.  Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given
-    to write into caller-owned buffers."""
+    the per-tensor k_scale / v_scale.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and
+    k_new first, through tfa_attn_varlen_kvcache_rotary_fwd() (with `quant` for an FP8 cache).  The rotated queries go
+    to `q_rot`, a contiguous (total_q, Hq, D) tensor of q's dtype, or to a buffer allocated here.  Returns out
+    (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
     assert k_cache.stride() == v_cache.stride() and q.stride(2) == 1 and k_cache.stride(3) == 1
@@ -435,7 +448,11 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
                           D, total_q, int(max_seqlen_q), nblk, page, mbps, q.stride(0), q.stride(1),
                           k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1], _dtype_code(q),
                           int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
-    if quant is not None:
+    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
+    if r is not None:
+        check(lib().tfa_attn_varlen_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r),
+                                                       ctypes.byref(quant) if quant is not None else None))
+    elif quant is not None:
         check(lib().tfa_attn_varlen_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(quant)))
     else:
         check(lib().tfa_attn_varlen_kvcache_fwd(ctypes.byref(a)))
