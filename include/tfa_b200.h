@@ -446,6 +446,41 @@ int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant)
  * captured in a CUDA graph and replayed with new cu_seqlens contents of the same totals. */
 int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant);
 
+/* ---- e4m3 queries against an FP8 (e4m3) KV cache, both products on FP8 tensor cores (FlashAttention-3's
+ * flash_attn_with_kvcache on fp8 tensors with descale_q / descale_k / descale_v) ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect them by the exported symbols
+ * tfa_attn_kvcache_qkv8_fwd and tfa_attn_varlen_kvcache_qkv8_fwd.  The problems of tfa_attn_kvcache_fwd() and
+ * tfa_attn_varlen_kvcache_fwd(), unchanged -- lengths and the capacity clamp, the block table, dropped tokens, key-less
+ * rows out = 0 / lse = +inf, slots past K_b holding any byte (NaN codes 0x7f / 0xff included) without changing the
+ * result, nothing read back to the host (CUDA-graph capture), split-KV for the dense-query call only (num_splits /
+ * workspace sized as for tfa_attn_kvcache_fwd()) -- with q and the caches holding one byte per element, and the
+ * arithmetic of tfa_attn_fp8_fwd().  tfa_attn_kvcache_fp8_fwd() widens every cache tile to q's 16-bit type; these calls
+ * read q and K in place and only transpose V, so nothing is widened.
+ *
+ *   q        : e4m3 codes (torch.float8_e4m3fn) in the 16-bit call's layout: (B, Sq, Hq, D) for the dense-query call,
+ *              packed (total_q, Hq, D) for the varlen one.  Strides are in elements, so in bytes, and must be multiples
+ *              of 16.
+ *   k_cache, v_cache : e4m3 codes, laid out as for tfa_attn_kvcache_fp8_fwd() (strides multiples of 16).
+ *   dtype    : the OUTPUT dtype, TFA_BF16 or TFA_FP16 (or fp32 with out_fp32), which is also the dtype of k_new / v_new.
+ *   out      : dense-query call: q's element strides, as tfa_attn_fp8_fwd(); varlen call: (total_q, Hq, D) contiguous.
+ *              lse as the 16-bit cache calls.
+ *   scales   : `quant` as tfa_attn_fp8_fwd(): a code x8 stands for q_scale * x8 in Q, k_scale * x8 in K, v_scale * x8 in
+ *              V.  s' = fp32(fp32(softmax_scale * q_scale) * k_scale), P rounded to e4m3, O multiplied by v_scale.
+ *   append   : k_new / v_new are quantized into the cache with k_scale / v_scale exactly as tfa_attn_kvcache_fp8_fwd()
+ *              quantizes them: the pools come out bit-identical to that call's.
+ *   result   : each sequence's out and lse are bit-identical to tfa_attn_fp8_fwd() (num_splits = 1) on that sequence
+ *              alone, with its q rows, its first K_b cached keys and values gathered into contiguous tensors, the same
+ *              scales, causal flag and output dtype (a sequence with K_b = 0 gets out = 0 / lse = +inf).
+ *   rotary   : not supported: q arrives quantized, so a RoPE caller rotates before it quantizes, or keeps
+ *              tfa_attn_kvcache_fp8_fwd() with `rotary`.
+ * Every check runs before any device work, in this order: the cache arguments (TFA_EINVAL_KVCACHE), the shapes,
+ * strides, dtype and scale of the 16-bit call, (varlen) cu_seqlens_q / max_seqlen_q (TFA_EINVAL_SEQLENS), the
+ * quantization (TFA_EINVAL_QKVQUANT for qkv_dtype, the scales, and q or cache strides that are not multiples of 16;
+ * then TFA_EINVAL_SCALE for s'), then the device (TFA_EARCH).  A NULL args or quant is TFA_EINVAL_PTR.  Launches: 1,
+ * + 1 with k_new, + 1 with split-KV. */
+int tfa_attn_kvcache_qkv8_fwd(const tfa_attn_kvcache_args* args, const tfa_qkv_quant_args* quant);
+int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_qkv_quant_args* quant);
+
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on
  * `n_streams` internal streams so H2D, compute and D2H overlap, copies out, and

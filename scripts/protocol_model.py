@@ -572,6 +572,16 @@ def random_fp8_cache_items(rng, varlen):
     return items, empty, vtail, rng.choice([2, 4])
 
 
+def random_qkv8_cache_items(rng, varlen):
+    """kCacheQkv8 (or kVarlenCacheQkv8 when `varlen`): the items of its cache mode as random_cache_items /
+    random_varlen_cache_items draw them -- items skipped by every role, items without tiles whose rows are still written,
+    items whose last tile has keys past K_b (the converter writes their V^T entries as zeros in the same stores, so the
+    barriers see them as any other tile) -- and ring depths as random_dense_fp8.  Returns (items, empty, vtail, depths)."""
+    depths = rng.choice([(4, 3, 4), (8, 4, 8), (1, 1, 1), (2, 3, 1), (3, 1, 2)])
+    items, empty, vtail = random_varlen_cache_items(rng) if varlen else random_cache_items(rng)
+    return items, empty, vtail, depths
+
+
 def main():
     trials = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
     for trial in range(trials):
@@ -592,6 +602,10 @@ def main():
         rngv = random.Random(3000003 + trial)             # kVarlenFp8, on a generator of its own
         items, empty, depths = random_varlen_fp8(rngv)
         DenseFp8Sim(items, *depths, rngv, empty).run()
+        rngc = random.Random(4000003 + trial)             # kCacheQkv8 / kVarlenCacheQkv8, on a generator of their own
+        for varlen in (False, True):
+            items, empty, _, depths = random_qkv8_cache_items(rngc, varlen)
+            DenseFp8Sim(items, *depths, rngc, empty).run()
     print(f"{trials} trials: no violation")
 
 

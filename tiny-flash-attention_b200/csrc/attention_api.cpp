@@ -338,15 +338,18 @@ struct CacheShape {
 // The arguments both cache entry points share, for a q of B sequences: the caches, cache_seqlens, block_table and the
 // pairing, device and dtype of k_new / v_new.  Each entry point checks the shapes of its q and k_new itself.  Throws
 // on a bad argument, before any device work.  `fp8`: the caches are float8_e4m3fn (the FP8 entry points), else q's
-// dtype.
+// dtype.  `qkv8_out` (with `fp8`): q is float8_e4m3fn too (the e4m3-query entry points), and k_new / v_new have the
+// output dtype *qkv8_out, bfloat16 or float16.
 CacheShape check_cache(const torch::Tensor& q, int64_t B, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
                        const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
                        const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
-                       bool fp8 = false) {
+                       bool fp8 = false, std::optional<at::ScalarType> qkv8_out = std::nullopt) {
   TFA_CHECK_CUDA(k_cache);
   TFA_CHECK_CUDA(v_cache);
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "k_cache, v_cache must have 4 dimensions");
-  if (fp8) {
+  if (fp8 && qkv8_out) {
+    check_dtype_device(q, k_cache, v_cache, "q, k_cache, v_cache", qkv8_out);
+  } else if (fp8) {
     TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be float16 or bfloat16");
     TORCH_CHECK(k_cache.scalar_type() == at::kFloat8_e4m3fn && v_cache.scalar_type() == at::kFloat8_e4m3fn,
                 "k_cache and v_cache must be float8_e4m3fn for the FP8 cache calls");
@@ -378,9 +381,11 @@ CacheShape check_cache(const torch::Tensor& q, int64_t B, const torch::Tensor& k
   TORCH_CHECK(k_new.has_value() == v_new.has_value(), "k_new and v_new must be given together");
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
-    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == q.scalar_type() &&
-                    vn.scalar_type() == q.scalar_type(),
-                "k_new and v_new must be on q's device with q's dtype");
+    const at::ScalarType nt = qkv8_out ? *qkv8_out : q.scalar_type();
+    TORCH_CHECK(kn.device() == q.device() && vn.device() == q.device() && kn.scalar_type() == nt &&
+                    vn.scalar_type() == nt,
+                qkv8_out ? "k_new and v_new must be on q's device with dtype out_dtype"
+                         : "k_new and v_new must be on q's device with q's dtype");
   }
   return c;
 }
@@ -396,10 +401,12 @@ struct KvcacheCall {
 KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
                           const torch::Tensor& cache_seqlens, const std::optional<torch::Tensor>& block_table,
                           const std::optional<torch::Tensor>& k_new, const std::optional<torch::Tensor>& v_new,
-                          int64_t num_splits, bool fp8 = false) {
+                          int64_t num_splits, bool fp8 = false,
+                          std::optional<at::ScalarType> qkv8_out = std::nullopt) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 4, "q must have 4 dimensions (B, Sq, Hq, D)");
-  const CacheShape cs = check_cache(q, q.size(0), k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, fp8);
+  const CacheShape cs =
+      check_cache(q, q.size(0), k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, fp8, qkv8_out);
   KvcacheCall c{q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new};
   c.B = q.size(0); c.Sq = q.size(1); c.Hq = q.size(2); c.D = q.size(3);
   c.nblk = cs.nblk; c.page = cs.page; c.Hkv = cs.Hkv; c.mbps = cs.mbps; c.bts = cs.bts;
@@ -422,17 +429,20 @@ KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, 
 
 // The dense-query cache call once every argument passed: allocates out (q's strides; a non-dense q is replaced by its
 // contiguous copy first), lse, the split-KV workspace and, with rotary (`r`), q_rot, and runs the call.  `quant`
-// nullptr: a 16-bit cache.
+// nullptr: a 16-bit cache.  `qkv8` (with `r` and `quant` nullptr): e4m3 q against an e4m3 cache, out in `out_dtype`.
 std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float softmax_scale, int64_t num_splits,
-                                       tfa_rotary_args* r, const tfa_kv_quant_args* quant) {
+                                       tfa_rotary_args* r, const tfa_kv_quant_args* quant,
+                                       const tfa_qkv_quant_args* qkv8 = nullptr,
+                                       at::ScalarType out_dtype = at::kBFloat16) {
   torch::Tensor out, lse, ws, q_rot;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(c.q.device());
-    out = torch::empty_like(c.q);
+    const at::ScalarType odt = qkv8 ? out_dtype : c.q.scalar_type();
+    out = torch::empty_like(c.q, c.q.options().dtype(odt));
     if (out.strides() != c.q.strides()) {     // out takes q's strides: give a non-dense q out's dense ones
       c.q = c.q.contiguous();
-      out = torch::empty_like(c.q);
+      out = torch::empty_like(c.q, c.q.options().dtype(odt));
     }
     lse = torch::empty({c.B, c.Hq, c.Sq}, c.q.options().dtype(at::kFloat));
     tfa_attn_kvcache_args a;
@@ -454,7 +464,7 @@ std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float sof
     if (c.snew) {
       a.new_stride_b = c.k_new->stride(0); a.new_stride_s = c.k_new->stride(1); a.new_stride_h = c.k_new->stride(2);
     }
-    a.dtype = c.q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.dtype = odt == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
     a.is_causal = is_causal ? 1 : 0;
     a.softmax_scale = softmax_scale;
     a.num_splits = static_cast<int32_t>(num_splits);
@@ -472,9 +482,10 @@ std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float sof
       q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
       r->q_rot = q_rot.data_ptr();
     }
-    rc = quant ? tfa_attn_kvcache_fp8_fwd(&a, r, quant)
-         : r   ? tfa_attn_kvcache_rotary_fwd(&a, r)
-               : tfa_attn_kvcache_fwd(&a);
+    rc = qkv8  ? tfa_attn_kvcache_qkv8_fwd(&a, qkv8)
+         : quant ? tfa_attn_kvcache_fp8_fwd(&a, r, quant)
+         : r     ? tfa_attn_kvcache_rotary_fwd(&a, r)
+                 : tfa_attn_kvcache_fwd(&a);
   }
   raise_on_error(rc);
   return {out, lse};
@@ -585,7 +596,8 @@ std::vector<torch::Tensor> varlen_kvcache(
     const std::optional<torch::Tensor>& block_table, const std::optional<torch::Tensor>& k_new,
     const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant,
     const std::optional<torch::Tensor>& rotary_cos = std::nullopt,
-    const std::optional<torch::Tensor>& rotary_sin = std::nullopt, bool rotary_interleaved = false) {
+    const std::optional<torch::Tensor>& rotary_sin = std::nullopt, bool rotary_interleaved = false,
+    const tfa_qkv_quant_args* qkv8 = nullptr, at::ScalarType out_dtype = at::kBFloat16) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
@@ -595,7 +607,9 @@ std::vector<torch::Tensor> varlen_kvcache(
                                                  static_cast<long long>(cu_seqlens_q.numel())));
   const int64_t total_q = q.size(0), Hq = q.size(1), D = q.size(2);
   const int64_t B = cu_seqlens_q.numel() - 1;
-  const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, quant != nullptr);
+  const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new,
+                                    quant != nullptr || qkv8 != nullptr,
+                                    qkv8 ? std::optional<at::ScalarType>(out_dtype) : std::nullopt);
   const int64_t nblk = cs.nblk, page = cs.page, Hkv = cs.Hkv, mbps = cs.mbps, bts = cs.bts;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
@@ -622,7 +636,8 @@ std::vector<torch::Tensor> varlen_kvcache(
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
-    out = torch::empty({total_q, Hq, D}, q.options());
+    const at::ScalarType odt = qkv8 ? out_dtype : q.scalar_type();
+    out = torch::empty({total_q, Hq, D}, q.options().dtype(odt));
     lse = torch::empty({Hq, total_q}, q.options().dtype(at::kFloat));
     tfa_attn_varlen_kvcache_args a;
     std::memset(&a, 0, sizeof(a));
@@ -642,12 +657,14 @@ std::vector<torch::Tensor> varlen_kvcache(
     a.cache_stride_block = k_cache.stride(0); a.cache_stride_s = k_cache.stride(1); a.cache_stride_h = k_cache.stride(2);
     a.block_table_stride = bts;
     if (k_new.has_value()) { a.new_stride_s = k_new->stride(0); a.new_stride_h = k_new->stride(1); }
-    a.dtype = q.scalar_type() == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
+    a.dtype = odt == at::kBFloat16 ? TFA_BF16 : TFA_FP16;
     a.is_causal = is_causal ? 1 : 0;
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    if (rotary_cos.has_value()) {
+    if (qkv8) {
+      rc = tfa_attn_varlen_kvcache_qkv8_fwd(&a, qkv8);
+    } else if (rotary_cos.has_value()) {
       q_rot = torch::empty({total_q, Hq, D}, q.options().memory_format(at::MemoryFormat::Contiguous));
       r.q_rot = q_rot.data_ptr();
       rc = tfa_attn_varlen_kvcache_rotary_fwd(&a, &r, quant);
@@ -691,6 +708,47 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_fp8(
   const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
                         is_causal, softmax_scale, &qa, rotary_cos, rotary_sin, rotary_interleaved);
+}
+
+namespace {
+
+// The per-tensor scales of an e4m3-query cache call; throws before any device work.
+tfa_qkv_quant_args check_qkv8_quant(double q_scale, double k_scale, double v_scale) {
+  TORCH_CHECK(std::isfinite(q_scale) && q_scale > 0 && std::isfinite(k_scale) && k_scale > 0 &&
+                  std::isfinite(v_scale) && v_scale > 0,
+              "q_scale, k_scale and v_scale must be finite and > 0");
+  return tfa_qkv_quant_args{TFA_FP8_E4M3, static_cast<float>(q_scale), static_cast<float>(k_scale),
+                            static_cast<float>(v_scale)};
+}
+
+}  // namespace
+
+// e4m3 queries against an FP8 cache (tfa_attn_kvcache_qkv8_fwd in include/tfa_b200.h): q (B, Sq, Hq, D), k_cache /
+// v_cache as flash_attention_v2_kvcache_fp8, all float8_e4m3fn with the per-tensor scales their codes stand for; both
+// products run on e4m3 tensor cores.  k_new / v_new (out_dtype) are quantized into the cache.  out_dtype (bfloat16 /
+// float16) is the output's; out takes q's strides.  No rotary: rotate q before quantizing it.
+std::vector<torch::Tensor> flash_attention_v2_kvcache_qkv8(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
+    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
+    double q_scale, double k_scale, double v_scale, bool is_causal, float softmax_scale, int64_t num_splits,
+    at::ScalarType out_dtype) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits, true,
+                                out_dtype);
+  const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
+  return kvcache_fwd(c, is_causal, softmax_scale, num_splits, nullptr, nullptr, &qa, out_dtype);
+}
+
+// The packed variable-length form: q (total_q, Hq, D) float8_e4m3fn with cu_seqlens_q as
+// flash_attention_v2_varlen_kvcache; the rest as flash_attention_v2_kvcache_qkv8.  Returns out (total_q, Hq, D) in
+// out_dtype and lse (Hq, total_q).  No split-KV.
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_qkv8(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, double q_scale, double k_scale, double v_scale, bool is_causal,
+    float softmax_scale, at::ScalarType out_dtype) {
+  const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
+  return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
+                        is_causal, softmax_scale, nullptr, std::nullopt, std::nullopt, false, &qa, out_dtype);
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -743,6 +801,18 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "the variable-length KV-cache call with q and k_new rotated (RoPE) at each sequence's cache positions: (q, "
         "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, rotary_cos, "
         "rotary_sin, rotary_interleaved, is_causal, scale)");
+  m.def("flash_attention_v2_kvcache_qkv8", &flash_attention_v2_kvcache_qkv8,
+        "float8_e4m3fn q against an FP8 (float8_e4m3fn) cache with per-tensor scales, both products on e4m3 tensor "
+        "cores, k_new / v_new (out_dtype) quantized on append -> [out (out_dtype), lse]",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("block_table"),
+        py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"), py::arg("k_scale"), py::arg("v_scale"),
+        py::arg("is_causal"), py::arg("softmax_scale"), py::arg("num_splits"), py::arg("out_dtype"));
+  m.def("flash_attention_v2_varlen_kvcache_qkv8", &flash_attention_v2_varlen_kvcache_qkv8,
+        "a packed variable-length batch of float8_e4m3fn queries against an FP8 (float8_e4m3fn) cache, both products "
+        "on e4m3 tensor cores -> [out (out_dtype), lse]",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
+        py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"),
+        py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"));
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

@@ -4,8 +4,9 @@
 //
 // tfa_varlen_kvcache.cu explicitly instantiates launch_forward<kVarlenCache>, tfa_kvcache_fp8.cu launch_forward<
 // kCacheFp8> and launch_forward<kVarlenCacheFp8>, tfa_fp8_fwd.cu launch_forward<kDenseFp8> and tfa_varlen_fp8.cu
-// launch_forward<kVarlenFp8>; the end of this header declares those instantiations `extern template`, so that each
-// mode's 32 kernels are compiled in that unit only.
+// launch_forward<kVarlenFp8>, tfa_kvcache_qkv8.cu launch_forward<kCacheQkv8> and launch_forward<kVarlenCacheQkv8>; the
+// end of this header declares those instantiations `extern template`, so that each mode's 32 kernels are compiled in
+// that unit only.
 #pragma once
 #include "fa_fwd_sm90.cuh"
 
@@ -63,6 +64,8 @@ TFA_LAUNCH_ELSEWHERE(kCacheFp8);          // tfa_kvcache_fp8.cu
 TFA_LAUNCH_ELSEWHERE(kVarlenCacheFp8);    // tfa_kvcache_fp8.cu
 TFA_LAUNCH_ELSEWHERE(kDenseFp8);          // tfa_fp8_fwd.cu
 TFA_LAUNCH_ELSEWHERE(kVarlenFp8);         // tfa_varlen_fp8.cu
+TFA_LAUNCH_ELSEWHERE(kCacheQkv8);         // tfa_kvcache_qkv8.cu
+TFA_LAUNCH_ELSEWHERE(kVarlenCacheQkv8);   // tfa_kvcache_qkv8.cu
 #undef TFA_LAUNCH_ELSEWHERE
 
 }  // namespace tfa

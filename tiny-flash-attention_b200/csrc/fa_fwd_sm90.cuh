@@ -39,22 +39,28 @@
 // ring of their own, and producer warps 1-3 (the converter) widen each into the 16-bit K/V ring slot the softmax
 // warpgroups read, exactly, in the layout TMA gives a 16-bit tile; their code does not change.  kDenseFp8 and
 // kVarlenFp8 are kDense and kVarlen with Q, K and V in e4m3 and both products on 8-bit wgmma (qkv8_mode()).
+// kCacheQkv8 and kVarlenCacheQkv8 are kCache and kVarlenCache on that datapath: e4m3 queries against the e4m3 cache,
+// K read in place from its pages and V transposed by the converter, nothing widened.
 #pragma once
 #include "ptx_sm90.cuh"
 
 namespace tfa {
 
 enum : int {
-  kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5, kDenseFp8 = 6, kVarlenFp8 = 7
+  kDense = 0, kVarlen = 1, kCache = 2, kVarlenCache = 3, kCacheFp8 = 4, kVarlenCacheFp8 = 5, kDenseFp8 = 6, kVarlenFp8 = 7,
+  kCacheQkv8 = 8, kVarlenCacheQkv8 = 9
 };
 // The problem an FP8-cache mode solves is that of its 16-bit mode: they differ only in how K/V reach the ring.
 __host__ __device__ constexpr bool fp8_mode(int mode) { return mode == kCacheFp8 || mode == kVarlenCacheFp8; }
-// kDenseFp8 / kVarlenFp8 solve the dense / varlen problem with Q, K and V in e4m3 and both products on 8-bit wgmma
-// (fp8_mode() is false for them: that predicate means "widen K/V to 16 bits").
-__host__ __device__ constexpr bool qkv8_mode(int mode) { return mode == kDenseFp8 || mode == kVarlenFp8; }
+// kDenseFp8 / kVarlenFp8 / kCacheQkv8 / kVarlenCacheQkv8 solve the dense / varlen / cache / varlen-cache problem with Q,
+// K and V in e4m3 and both products on 8-bit wgmma (fp8_mode() is false for them: that predicate means "widen K/V to
+// 16 bits").
+__host__ __device__ constexpr bool qkv8_mode(int mode) {
+  return mode == kDenseFp8 || mode == kVarlenFp8 || mode == kCacheQkv8 || mode == kVarlenCacheQkv8;
+}
 __host__ __device__ constexpr int base_mode(int mode) {
   return mode == kCacheFp8 ? kCache : mode == kVarlenCacheFp8 ? kVarlenCache : mode == kDenseFp8 ? kDense
-       : mode == kVarlenFp8 ? kVarlen : mode;
+       : mode == kVarlenFp8 ? kVarlen : mode == kCacheQkv8 ? kCache : mode == kVarlenCacheQkv8 ? kVarlenCache : mode;
 }
 
 // ---- kDenseFp8: P as the 8-bit A operand without shuffles ----
@@ -221,7 +227,7 @@ struct Fp8Cfg {
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB of shared memory a block may use");
   static constexpr int CONVERTER_WARPS = 3;   // producer warps 1..3
 };
-// Shared-memory plan of kDenseFp8 and kVarlenFp8: Q (128 rows x D bytes), the 16-bit O staging of FwdCfg, then three rings of
+// Shared-memory plan of the qkv8_mode() modes: Q (128 rows x D bytes), the 16-bit O staging of FwdCfg, then three rings of
 // 128 x D-byte tiles -- K (filled by TMA, SWIZZLE_128B at D = 128, SWIZZLE_64B at D = 64), raw V (unswizzled, as TMA
 // loads it) and V^T (D rows x 128 keys, SWIZZLE_128B, written by the converter) -- then the barriers: q_full, q_empty,
 // k_full / k_empty[NK], raw_full / raw_empty[NRAW], vt_full / vt_empty[NVT].  Each ring has its own barriers, so each
@@ -285,7 +291,8 @@ __device__ __forceinline__ uint4 widen_e4m3x8(uint2 r) {
 // V^T row -- x columns [4 dc, 4 dc + 4) of the raw tile at `raw` (128 keys x D bytes, row-major) into the V^T slot at
 // `dst` (D rows x 128 keys, positions in fp8_vt_key order, SWIZZLE_128B).  Consecutive units take two chunks x 16
 // columns per warp: its loads hit two rows per bank, its stores (8 lanes: four chunks x two rows) distinct bank groups.
-// TAIL (kVarlenFp8): keys >= `valid` are written as zeros -- in a packed tile they are the next sequence's, any byte.
+// TAIL (kVarlenFp8, and the cache modes): keys >= `valid` are written as zeros -- in a packed tile they are the next
+// sequence's, in a cache page the slots past the sequence's keys: any byte either way.
 template <int D, bool TAIL = false>
 __device__ __forceinline__ void vt_convert_unit(uint32_t raw, uint32_t dst, int u, int valid = 128) {
   constexpr int DC = D / 4;
@@ -544,8 +551,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       if (warp > 0) {
         // ---- the converter (warps 1..3): raw V tile (128 keys x D bytes) -> V^T slot (D rows x 128 keys, keys in
         // fp8_vt_key order, SWIZZLE_128B), walking the TMA lane's tiles.  Dense: keys past Sk arrive as TMA's zero fill.
-        // Packed: they are the next sequence's keys, any byte, NaN codes included (P = 0 does not cancel 0 * NaN), so
-        // they are written as zeros, which also makes a sequence's result that of the dense call on it alone. ----
+        // Packed: they are the next sequence's keys, any byte, NaN codes included (P = 0 does not cancel 0 * NaN); cache:
+        // the page's slots past K_b, any byte too.  So they are written as zeros, which also makes a sequence's result
+        // that of the dense call on it alone.  K needs nothing: the edge mask overwrites those scores, NaN or not. ----
         const int ct = threadIdx.x - 32;                          // 0 .. 95
         uint32_t tile = 0;
         for (int item = first; item < p.total_items; item += stride) {
@@ -557,7 +565,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             mbar_wait(&vt_empty[vslot], ((tile / F8::NVT) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             const uint32_t raw = smem_u32(sRaw8) + rslot * F8::TILE8;
             const uint32_t dst = smem_u32(sVt) + vslot * F8::TILE8;
-            if constexpr (QPACK) {
+            if constexpr (QPACK || PAGED) {
               const int valid = w.Sk - (w.jb + j) * C::BN;
 #pragma unroll 1
               for (int u = ct; u < 2 * D; u += 32 * F8::CONVERTER_WARPS) vt_convert_unit<D, true>(raw, dst, u, valid);
@@ -583,9 +591,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           if (qcnt > 0) mbar_wait(q_empty, (qcnt - 1) & 1, p.dbg, SITE_LOAD_Q, qcnt);
           ++qcnt;
           mbar_arrive_expect_tx(q_full, F8::Q_BYTES);
-          // packed (kVarlenFp8): the tensors are one batch entry, the sequence starts at row q0 / k0.  Rows a box takes
-          // in past the sequence's end are never stored (queries) or get -inf from the edge mask (keys; their V^T
-          // entries the converter writes as zeros)
+          // packed (kVarlenFp8, kVarlenCacheQkv8): the tensors are one batch entry, the sequence starts at row q0 / k0.
+          // Rows a box takes in past the sequence's end are never stored (queries) or get -inf from the edge mask (keys;
+          // their V^T entries the converter writes as zeros)
           int qy = w.row0, k0 = 0, wz = w.bidx;
           if constexpr (QPACK) {
             qy += w.q0;
@@ -594,14 +602,17 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           }
           tma_load_4d(sQ, &tmQ, q_full, 0, qy, w.hidx, wz);
           for (int j = 0; j < w.n; ++j, ++tile) {
-            const int ky = k0 + (w.jb + j) * C::BN;
+            // cache: the tile's 128 keys lie in one page (page % 128 == 0, or one page per sequence), K and V at the
+            // same (row, block)
+            int ky = k0 + (w.jb + j) * C::BN, kw = wz;
+            if constexpr (PAGED) page_lookup(p.block_table, p.bt_stride, w.bidx, ky, p.page, kw, ky);
             const uint32_t kslot = tile % F8::NK, rslot = tile % F8::NRAW;
             mbar_wait(&k_empty[kslot], ((tile / F8::NK) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             mbar_arrive_expect_tx(&k_full[kslot], F8::TILE8);
-            tma_load_4d(sK8 + kslot * F8::TILE8, &tmK, &k_full[kslot], 0, ky, w.hkv, wz);
+            tma_load_4d(sK8 + kslot * F8::TILE8, &tmK, &k_full[kslot], 0, ky, w.hkv, kw);
             mbar_wait(&raw8_empty[rslot], ((tile / F8::NRAW) & 1) ^ 1, p.dbg, SITE_LOAD_EMPTY, tile);
             mbar_arrive_expect_tx(&raw8_full[rslot], F8::TILE8);
-            tma_load_4d(sRaw8 + rslot * F8::TILE8, &tmV, &raw8_full[rslot], 0, ky, w.hkv, wz);
+            tma_load_4d(sRaw8 + rslot * F8::TILE8, &tmV, &raw8_full[rslot], 0, ky, w.hkv, kw);
           }
         }
       }
@@ -780,7 +791,7 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     // (whole 128-byte swizzle rows of each slab, so the swizzle does not matter).  Both warpgroups write the same
     // zeros; the slot is released only after both have read it.  Between the kv_full wait and the release, so the
     // producer cannot refill the slot under the stores (scripts/protocol_model.py).  Dense: the rows past Sk are TMA's
-    // zero fill.  FP8 cache and kVarlenFp8: the converter wrote those rows as zeros already.
+    // zero fill.  FP8 cache, kVarlenFp8 and the e4m3-query cache modes: the converter wrote those rows as zeros already.
     auto zero_v_tail = [&](uint32_t vslot, int jt) {
       if constexpr ((PAGED || M == kVarlen) && !FP8 && !DF8) {
         const int valid = Sk - (w.jb + jt) * C::BN;          // warpgroup-uniform

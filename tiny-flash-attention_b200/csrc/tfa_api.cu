@@ -172,7 +172,7 @@ long long fwd_grid(long long nitems, int variant) {
 }
 
 // One forward kernel launch over `nitems` work items of problem mode MODE (tfa::kDense / kVarlen / kCache /
-// kVarlenCache / kCacheFp8 / kVarlenCacheFp8 / kDenseFp8 / kVarlenFp8).
+// kVarlenCache / kCacheFp8 / kVarlenCacheFp8 / kDenseFp8 / kVarlenFp8 / kCacheQkv8 / kVarlenCacheQkv8).
 template <int MODE>
 int launch_fwd(int D, bool causal, bool bf16, bool f32, const CUtensorMap& tq, const CUtensorMap& tk,
                const CUtensorMap& tv, FwdParams p, long long nitems, int variant, cudaStream_t stream) {
@@ -564,12 +564,14 @@ int validate_cache(const Args& ka) {
 // The cache side of a cache call whose arguments passed (a = its Problem, capacity = a.Sk): the K/V tensor maps over
 // the pages, the append of `n` rows per sequence (ap.chunks = 0 without k_new; the caller sets its k_new layout fields
 // n_sb / cu_q / total_q) and the cache fields of the forward but snew.
-// `cache_dtype`: a.dtype, or TFA_FP8_E4M3 for an FP8 cache.
+// `cache_dtype`: a.dtype, or TFA_FP8_E4M3 for an FP8 cache.  `k_operand8`: the FP8 cache's K map is the 8-bit wgmma
+// operand the e4m3-query modes read in place (make_tmap's operand8); V's stays the raw map the converter reads.
 template <typename Args>
 int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtensorMap& tv, tfa::AppendParams& ap,
-                FwdParams& p, int cache_dtype) {
+                FwdParams& p, int cache_dtype, bool k_operand8 = false) {
   const int page = ka.block_table ? ka.page_block_size : a.Sk;
-  if (int rc = make_tmap(&tk, a.k, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
+  if (int rc = make_tmap(&tk, a.k, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss, k_operand8))
+    return rc;
   if (int rc = make_tmap(&tv, a.v, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
   ap = tfa::AppendParams{};
   ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
@@ -617,8 +619,11 @@ int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
 
 // `ra` nullptr: the plain cache forward.  Otherwise the append also rotates q and k_new, and the forward reads its
 // queries from ra->q_rot.  `quant` nullptr: a 16-bit cache; otherwise an FP8 one, into which the append quantizes and
-// which the kCacheFp8 forward reads.
-int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant) {
+// which the kCacheFp8 forward reads.  `qkv8` (with `ra` and `quant` nullptr): e4m3 q against an FP8 cache, a.dtype the
+// output's and k_new's; the append quantizes as for `quant` and the kCacheQkv8 forward reads q and the cache on 8-bit
+// wgmma.
+int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant,
+                 const tfa_qkv_quant_args* qkv8 = nullptr) {
   Problem a = from_kvcache_args(ka);
   int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
@@ -626,6 +631,10 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
   if (ra && (rc = validate_rotary(ka, a, *ra))) return rc;
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
+  if (qkv8) {
+    if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
+    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale};
+  }
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
   const int snew = ka.k_new ? ka.Snew : 0;
@@ -648,18 +657,26 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
     a.qsb = a.qss * a.Sq;
   }
 
+  // qkv8: the 8-bit swizzled Q and K maps the wgmma reads in place, as fwd_impl builds them
+  const bool fp8_cache = quant || qkv8;
   CUtensorMap tq, tk, tv;
   FwdParams p{};
-  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(ka, a, snew, tk, tv, rp.ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
+  if ((rc = make_tmap(&tq, a.q, qkv8 ? TFA_FP8_E4M3 : a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss,
+                      qkv8 != nullptr)))
+    return rc;
+  if ((rc = setup_cache(ka, a, snew, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype, qkv8 != nullptr))) return rc;
   rp.ap.n_sb = ka.new_stride_b;
   if (snew > 0) {                       // rotary needs k_new (validate_rotary): every rotary call appends
-    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
+    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
                                     ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
 
   p.snew = snew;
+  if (qkv8) {
+    p.v_scale = qs.v_scale;
+    return run_forward<tfa::kCacheQkv8>(a, p, a.Sq, tq, tk, tv, plan);
+  }
   if (quant) {
     p.v_scale = qs.v_scale;
     return run_forward<tfa::kCacheFp8>(a, p, a.Sq, tq, tk, tv, plan);
@@ -684,10 +701,10 @@ Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
   return q;
 }
 
-// `ra` and `quant` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and the forward
-// reads its queries from ra->q_rot.
+// `ra`, `quant` and `qkv8` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and the
+// forward reads its queries from ra->q_rot.
 int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* ra,
-                        const tfa_kv_quant_args* quant) {
+                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr) {
   Problem a = from_varlen_kvcache_args(va);
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
@@ -696,6 +713,10 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
   if (ra && (rc = validate_rotary(va, a, *ra))) return rc;
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
+  if (qkv8) {
+    if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
+    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale};
+  }
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
 
@@ -714,14 +735,18 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
     a.qsh = a.D;
   }
 
+  const bool fp8_cache = quant || qkv8;
   CUtensorMap tq, tk, tv;
   FwdParams p{};
-  if ((rc = make_tmap(&tq, a.q, a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss))) return rc;
-  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, quant ? TFA_FP8_E4M3 : a.dtype))) return rc;
+  if ((rc = make_tmap(&tq, a.q, qkv8 ? TFA_FP8_E4M3 : a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, qkv8 != nullptr)))
+    return rc;
+  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype,
+                        qkv8 != nullptr)))
+    return rc;
   if (va.k_new) {                       // rotary needs k_new (validate_rotary): every rotary call appends
     rp.ap.cu_q = va.cu_seqlens_q;
     rp.ap.total_q = a.Sq;
-    rc = tfa_internal_launch_append(rp, quant ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
+    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
                                     ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
@@ -730,6 +755,10 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
   p.total_q = a.Sq;
   p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
   // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
+  if (qkv8) {
+    p.v_scale = qs.v_scale;
+    return run_forward<tfa::kVarlenCacheQkv8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+  }
   if (quant) {
     p.v_scale = qs.v_scale;
     return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
@@ -818,6 +847,16 @@ int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant)
 int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
   return varlen_impl(*args, quant);
+}
+
+int tfa_attn_kvcache_qkv8_fwd(const tfa_attn_kvcache_args* args, const tfa_qkv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return kvcache_impl(*args, nullptr, nullptr, quant);
+}
+
+int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_qkv_quant_args* quant) {
+  if (!args || !quant) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args, nullptr, nullptr, quant);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {

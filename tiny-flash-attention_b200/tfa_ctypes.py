@@ -161,6 +161,10 @@ def lib():
         L.tfa_attn_fp8_fwd.restype = ci
         L.tfa_attn_varlen_fp8_fwd.argtypes = [ctypes.POINTER(VarlenArgs), ctypes.POINTER(QkvQuantArgs)]
         L.tfa_attn_varlen_fp8_fwd.restype = ci
+        L.tfa_attn_kvcache_qkv8_fwd.argtypes = [ctypes.POINTER(KvcacheArgs), ctypes.POINTER(QkvQuantArgs)]
+        L.tfa_attn_kvcache_qkv8_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_qkv8_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(QkvQuantArgs)]
+        L.tfa_attn_varlen_kvcache_qkv8_fwd.restype = ci
         L.tfa_selftest_wgmma_fp8.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp]
         L.tfa_selftest_wgmma_fp8.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
@@ -350,6 +354,33 @@ def _quant(k_cache, k_scale, v_scale):
     return KvQuantArgs(TFA_FP8_E4M3, float(k_scale), float(v_scale))
 
 
+def _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype):
+    """What a cache call takes of its element types and scales: (tfa_kv_quant_args or None, tfa_qkv_quant_args or None,
+    the output dtype).  A float8_e4m3fn q needs a float8_e4m3fn cache (the e4m3-query calls, out in out_dtype, k_new in
+    out_dtype) and takes no rotary; a 16-bit q takes a cache of its own dtype or an FP8 one, and no q_scale / out_dtype."""
+    import torch
+    if q.dtype != torch.float8_e4m3fn:
+        if q_scale != 1.0 or out_dtype not in (None, q.dtype):
+            raise ValueError(f"q_scale / out_dtype apply to a float8_e4m3fn q only; q is {q.dtype}")
+        return _quant(k_cache, k_scale, v_scale), None, q.dtype
+    if k_cache.dtype != torch.float8_e4m3fn:
+        raise TypeError(f"a float8_e4m3fn q needs a float8_e4m3fn cache, got {k_cache.dtype}")
+    if rotary_cos is not None:
+        raise ValueError("a float8_e4m3fn q takes no rotary: rotate q before quantizing it, or pass a 16-bit q")
+    qkv8, odt = _qkv_quant(q, q_scale, k_scale, v_scale, out_dtype)
+    if k_new is not None and k_new.dtype != odt:
+        raise TypeError(f"k_new / v_new must have out_dtype {odt} with a float8_e4m3fn q, got {k_new.dtype}")
+    return None, qkv8, odt
+
+
+def _cache_dtype_code(q, qkv8, odt):
+    """args->dtype of a cache call: q's, or with a float8_e4m3fn q (qkv8) the output's."""
+    import torch
+    if qkv8 is None:
+        return _dtype_code(q)
+    return TFA_BF16 if odt == torch.bfloat16 else TFA_FP16
+
+
 def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream):
     """The RotaryArgs of a cache call with q (its q_rot: a contiguous tensor of q's shape and dtype, or a buffer
     allocated here and kept alive as the split workspace is), or None without rotary_cos."""
@@ -368,7 +399,8 @@ def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream):
 
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
                      scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
-                     rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None, k_scale=1.0, v_scale=1.0):
+                     rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None, k_scale=1.0, v_scale=1.0,
+                     q_scale=1.0, out_dtype=None):
     """Attention against a KV cache through tfa_attn_kvcache_fwd(): q (B, Sq, Hq, D) with unit head_dim stride;
     k_cache / v_cache (num_blocks, page, Hkv, D) with a block_table (B, max_blocks_per_seq) int32, or (B, capacity,
     Hkv, D) with block_table None; cache_seqlens (B,) int32; optional k_new / v_new (B, Snew, Hkv, D) appended in
@@ -376,7 +408,9 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and k_new first, through
     tfa_attn_kvcache_rotary_fwd().  The rotated queries go to `q_rot`, a contiguous (B, Sq, Hq, D) tensor of q's dtype
     that holds them after the call, or to a buffer allocated here.
-    torch.float8_e4m3fn caches go through tfa_attn_kvcache_fp8_fwd() with the per-tensor k_scale / v_scale.
+    torch.float8_e4m3fn caches go through tfa_attn_kvcache_fp8_fwd() with the per-tensor k_scale / v_scale.  A
+    torch.float8_e4m3fn q with them goes through tfa_attn_kvcache_qkv8_fwd() with q_scale too, the output (and k_new /
+    v_new) in out_dtype (bfloat16 or float16), without rotary.
     Returns out (q's shape and strides) and lse (B, Hq, Sq)."""
     import torch
     assert q.is_cuda and q.dim() == 4 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -384,27 +418,29 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     assert cache_seqlens.dtype == torch.int32
     B, Sq, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    quant = _quant(k_cache, k_scale, v_scale)
+    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 3)
     snew = k_new.shape[1] if k_new is not None else 0
     if scale is None:
         scale = D ** -0.5
     if out is None:
-        out = torch.empty_strided(q.shape, q.stride(), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+        out = torch.empty_strided(q.shape, q.stride(), dtype=torch.float32 if out_fp32 else odt, device=q.device)
     if lse is None:
         lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=q.device)
     st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
     a = KvcacheArgs(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), nptr, vptr, out.data_ptr(), lse.data_ptr(),
                     cache_seqlens.data_ptr(), bt_ptr, B, Hq, Hkv, Sq, D, nblk, page, mbps, snew,
                     q.stride(0), q.stride(1), q.stride(2), k_cache.stride(0), k_cache.stride(1), k_cache.stride(2),
-                    bts, ns[0], ns[1], ns[2], _dtype_code(q), int(bool(is_causal)), float(scale),
+                    bts, ns[0], ns[1], ns[2], _cache_dtype_code(q, qkv8, odt), int(bool(is_causal)), float(scale),
                     int(bool(out_fp32)), int(num_splits), None, 0, st)
     # the split count and workspace of the dense problem with Sk = capacity
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
     n = _split_workspace(dense, a, q.device, st)
     r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
-    if quant is not None:
+    if qkv8 is not None:
+        check(lib().tfa_attn_kvcache_qkv8_fwd(ctypes.byref(a), ctypes.byref(qkv8)))
+    elif quant is not None:
         check(lib().tfa_attn_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
                                              ctypes.byref(quant)))
     elif r is None:
@@ -419,37 +455,41 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
 def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
                             v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None,
                             k_scale=1.0, v_scale=1.0, rotary_cos=None, rotary_sin=None, rotary_interleaved=False,
-                            q_rot=None):
+                            q_rot=None, q_scale=1.0, out_dtype=None):
     """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
     (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
     and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
     sharing cu_q, appended in place.  torch.float8_e4m3fn caches go through tfa_attn_varlen_kvcache_fp8_fwd() with
     the per-tensor k_scale / v_scale.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and
     k_new first, through tfa_attn_varlen_kvcache_rotary_fwd() (with `quant` for an FP8 cache).  The rotated queries go
-    to `q_rot`, a contiguous (total_q, Hq, D) tensor of q's dtype, or to a buffer allocated here.  Returns out
-    (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given to write into caller-owned buffers."""
+    to `q_rot`, a contiguous (total_q, Hq, D) tensor of q's dtype, or to a buffer allocated here.  A
+    torch.float8_e4m3fn q with an FP8 cache goes through tfa_attn_varlen_kvcache_qkv8_fwd() as attn_kvcache_fwd's.
+    Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
     assert k_cache.stride() == v_cache.stride() and q.stride(2) == 1 and k_cache.stride(3) == 1
     assert cu_q.dtype == torch.int32 and cu_q.numel() >= 2 and cache_seqlens.dtype == torch.int32
     total_q, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    quant = _quant(k_cache, k_scale, v_scale)
+    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 2)
     if scale is None:
         scale = D ** -0.5
     if out is None:
-        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else q.dtype, device=q.device)
+        out = torch.empty((total_q, Hq, D), dtype=torch.float32 if out_fp32 else odt, device=q.device)
     if lse is None:
         lse = torch.empty((Hq, total_q), dtype=torch.float32, device=q.device)
     st = stream if stream is not None else torch.cuda.current_stream(q.device).cuda_stream
     a = VarlenKvcacheArgs(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), nptr, vptr, out.data_ptr(),
                           lse.data_ptr(), cu_q.data_ptr(), cache_seqlens.data_ptr(), bt_ptr, cu_q.numel() - 1, Hq, Hkv,
                           D, total_q, int(max_seqlen_q), nblk, page, mbps, q.stride(0), q.stride(1),
-                          k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1], _dtype_code(q),
+                          k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1],
+                          _cache_dtype_code(q, qkv8, odt),
                           int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
     r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
-    if r is not None:
+    if qkv8 is not None:
+        check(lib().tfa_attn_varlen_kvcache_qkv8_fwd(ctypes.byref(a), ctypes.byref(qkv8)))
+    elif r is not None:
         check(lib().tfa_attn_varlen_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r),
                                                        ctypes.byref(quant) if quant is not None else None))
     elif quant is not None:
