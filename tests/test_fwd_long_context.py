@@ -22,7 +22,8 @@ Cache workloads.  The cache-decode pool holds more than 2^31 elements and its bl
 sequence 0's last pages, the appended row among them, sit past element 2^31: the kernel's and the append's 64-bit
 offsets are exercised.  FP8 pools are quantized as a caller would, with per-tensor scales from the data; one FP8
 decode run rotates q and the appended keys (rotary_dim 64, NeoX) at positions near 256K: q_rot must equal the eager
-fp32 rotation bit for bit, and the appended row the quantized rotated key.  The varlen-cache workload (kVarlenCache,
+fp32 rotation bit for bit, and the appended row the quantized rotated key.  Its twin qkv8_cache_decode builds the same
+pools and quantizes q too (kCacheQkv8: both products on FP8 wgmma, checked against the FP8 budget).  The varlen-cache workload (kVarlenCache,
 which has no split-KV) runs a 2048-row prefill chunk on a 128K cache and decode rows on caches near 200K, appending
 every query row's key first.
 
@@ -195,6 +196,8 @@ def workloads():
             W(f"fp8_cache_decode_{pat}", "cache", pat, s + 5,
               dict(lens=CACHE_LENS, Hq=32, Hkv=8, D=128, kind="fp16", page=256, ns=(0,), kvfp8=True,
                    rotary=(64, False) if i == 0 else None)),
+            W(f"qkv8_cache_decode_{pat}", "cache", pat, s + 5,        # the same pools, e4m3 q on FP8 wgmma
+              dict(lens=CACHE_LENS, Hq=32, Hkv=8, D=128, kind="fp16", page=256, ns=(0,), kvfp8=True, qkv8=True)),
             W(f"fp8_dense_{pat}", "dense", pat, s + 6,
               dict(B=1, Hq=4, Hkv=2, Sq=256, Sk=131072, D=128, kind="bf16", causal=False, ns=1, fp8=True),
               ("kv head h % Hkv",) if i == 1 else ()),
@@ -361,7 +364,9 @@ def _run_cache(tfa, w, check):
     assert int(table[0, lens[0] // page]) * page * Hkv * D >= 2 ** 31, "sequence 0's appended row below element 2^31"
     fp8 = kw.get("kvfp8", False)
     tab = table.cuda()
-    q = make_q(w.pattern, (B, 1, Hq, D), g).to(dt)
+    q = make_q(w.pattern, (B, 1, Hq, D), g)
+    q, qs = fp8_of(q) if kw.get("qkv8") else (q.to(dt), 1.0)
+    qkw = dict(q_scale=qs, out_dtype=dt) if kw.get("qkv8") else {}
     kn, vn = make_kv(w.pattern, B, Hkv, D, g, 1)
     kn, vn = kn[:, None].to(dt), vn[:, None].to(dt)
     kp, vp, ks, vs = _make_pools(w, lens, Hkv, D, page, tab, nblk, dt, fp8, (kn, vn))
@@ -381,7 +386,7 @@ def _run_cache(tfa, w, check):
         lb, lse = guarded((B, Hq, 1), torch.float32)
         q_rot = torch.full_like(q, float("nan")) if rot else None
         _, _, n = tfa.attn_kvcache_fwd(q, kp, vp, sl, tab, kn, vn, is_causal=True, scale=scale, num_splits=ns, out=out,
-                                       lse=lse, return_splits=True, k_scale=ks, v_scale=vs,
+                                       lse=lse, return_splits=True, k_scale=ks, v_scale=vs, **qkw,
                                        **(dict(rot, q_rot=q_rot) if rot else {}))
         variant = tfa.lib().tfa_internal_last_variant()
         torch.cuda.synchronize()
@@ -396,7 +401,7 @@ def _run_cache(tfa, w, check):
         run = dict(ns=ns, splits=n, digest=digest(out, lse, *([q_rot] if rot else [])), variant=variant)
         if check:
             verdict, neg = Verdict(), {}
-            f8 = (1.0, ks, vs) if fp8 else None
+            f8 = (qs, ks, vs) if fp8 else None
             for b, L in enumerate(lens):
                 kk, vv = _seq_kv(kp, vp, tab, page, b, L + 1)
                 args = (qa[b].permute(1, 0, 2), kk, vv, out[b].permute(1, 0, 2), lse[b])

@@ -540,7 +540,27 @@ def _gather(pool, table, b, K):
     return gather(pool, table, b, K)
 
 
-# name, pool layout, fp8 (k_scale, v_scale) or None, Sq, snew, num_splits, rotary (rotary_dim, interleaved) or None
+def quantize_q(q, fp8):
+    """q for the call: 16-bit as given, or with fp8 = (q_scale, k_scale, v_scale) e4m3 codes as a caller quantizes."""
+    return (q.float() / fp8[0]).clamp(-448, 448).to(FP8) if fp8 is not None and len(fp8) == 3 else q
+
+
+def check_seq(q, k, v, out, lse, causal, scale, fp8, kind):
+    """(ok, message) of one sequence against the float64 reference: the FP8 budget for e4m3 q (fp8 of length 3),
+    the 16-bit one otherwise (and for a sequence without keys, whose rows must be exactly 0 / +inf)."""
+    ks, vs = fp8[-2:] if fp8 else (1.0, 1.0)
+    if fp8 is not None and len(fp8) == 3:
+        qd = deq(q, fp8[0])
+        if k.shape[2]:
+            ok, _, _, msg = fp8_compare(out, lse, fp8_reference(qd, k, v, causal, scale, ks, vs), kind)
+            return ok, msg
+        q = qd
+    verdict = compare(out, lse, reference(q, k, v, causal, scale, ks, vs), kind)
+    return verdict.ok, verdict.msg
+
+
+# name, pool layout, FP8 scales or None, Sq, snew, num_splits, rotary (rotary_dim, interleaved) or None.  FP8 scales
+# (k_scale, v_scale): an FP8 cache with a 16-bit q; (q_scale, k_scale, v_scale): e4m3 q codes too (kCacheQkv8)
 CACHE = [
     ("stacked", "stacked", None, 1, 1, 1, None),
     ("stacked_splits", "stacked", None, 4, 4, 3, None),
@@ -550,14 +570,17 @@ CACHE = [
     ("fp8_interleaved", "interleaved", (0.0311, 0.0089), 4, 4, 1, None),
     ("rotary_decode", "interleaved", None, 1, 1, 3, (64, False)),
     ("fp8_rotary_decode", "stacked", (0.0213, 0.0117), 1, 1, 1, (128, True)),
+    ("qkv8_stacked", "stacked", (0.0213, 0.0171, 0.0117), 1, 1, 3, None),
+    ("qkv8_interleaved", "interleaved", (0.0213, 0.0311, 0.0089), 4, 4, 1, None),
 ]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,pool,fp8,Sq,snew,ns,rotary", CACHE, ids=[c[0] for c in CACHE])
 def test_cache_poisoned_layouts(tfa, name, pool, fp8, Sq, snew, ns, rotary):
-    """tfa_attn_kvcache_fwd (16-bit and FP8 pools, rotary): q a view of a head-padded buffer, out at q's strides inside
-    poison, k_new / v_new interleaved views, the pools as above."""
+    """tfa_attn_kvcache_fwd (16-bit and FP8 pools, rotary, e4m3 q): q a view of a head-padded buffer (for e4m3 q its
+    strides are multiples of 16 bytes), out at q's element strides inside poison, k_new / v_new interleaved views, the
+    pools as above."""
     lens = [0, 1, 127, 128, 129, 300, 255, 511]
     Hq, Hkv, page = 8, 2, 128
     D = 64 if (fp8 is None) == (ns == 1) else 128
@@ -575,7 +598,9 @@ def test_cache_poisoned_layouts(tfa, name, pool, fp8, Sq, snew, ns, rotary):
     g = torch.Generator().manual_seed(71)
     kn, vn = ((torch.empty(B, snew, Hkv, D).normal_(0, 0.5, generator=g).to(dt).cuda() for _ in range(2)) if snew
               else (None, None))
-    ks, vs = fp8 or (1.0, 1.0)
+    q = quantize_q(q, fp8)
+    ks, vs = fp8[-2:] if fp8 else (1.0, 1.0)
+    qkw = dict(q_scale=fp8[0], out_dtype=dt) if len(fp8 or ()) == 3 else {}
     scale = D ** -0.5
     rot, rot_p = {}, {}
     if rotary:
@@ -584,7 +609,7 @@ def test_cache_poisoned_layouts(tfa, name, pool, fp8, Sq, snew, ns, rotary):
         rot = dict(rotary_cos=cos, rotary_sin=sin, rotary_interleaved=il, q_rot=torch.empty_like(q))
     k1, v1 = kp.clone(), vp.clone()
     out, lse = tfa.attn_kvcache_fwd(q, k1, v1, sl, table, kn, vn, is_causal=causal, scale=scale, num_splits=ns,
-                                    k_scale=ks, v_scale=vs, **rot)
+                                    k_scale=ks, v_scale=vs, **rot, **qkw)
     torch.cuda.synchronize()
     # the poisoned run
     which = len(name)
@@ -607,7 +632,7 @@ def test_cache_poisoned_layouts(tfa, name, pool, fp8, Sq, snew, ns, rotary):
         rot_p = dict(rot, q_rot=pr.view)
     assert pout.view.stride() == pq.view.stride()
     tfa.attn_kvcache_fwd(pq.view, pools.views[0], pools.views[1], sl, table, kn2, vn2, is_causal=causal, scale=scale,
-                         num_splits=ns, out=pout.view, lse=plse.view, k_scale=ks, v_scale=vs, **rot_p)
+                         num_splits=ns, out=pout.view, lse=plse.view, k_scale=ks, v_scale=vs, **rot_p, **qkw)
     torch.cuda.synchronize()
     pq.assert_kept("q", whole=True)
     if pn is not None:
@@ -624,20 +649,20 @@ def test_cache_poisoned_layouts(tfa, name, pool, fp8, Sq, snew, ns, rotary):
         qa = rot["q_rot"]
     fails = []
     for b, K in enumerate(Ks):
-        ref = reference(qa[b:b + 1].permute(0, 2, 1, 3), _gather(k1, table, b, K), _gather(v1, table, b, K), causal,
-                        scale, ks, vs)
-        verdict = compare(out[b:b + 1].permute(0, 2, 1, 3), lse[b:b + 1], ref, kind)
-        if not verdict.ok:
-            fails.append(f"sequence {b} (K {K}): {verdict.msg}")
+        ok, msg = check_seq(qa[b:b + 1].permute(0, 2, 1, 3), _gather(k1, table, b, K), _gather(v1, table, b, K),
+                            out[b:b + 1].permute(0, 2, 1, 3), lse[b:b + 1], causal, scale, fp8, kind)
+        if not ok:
+            fails.append(f"sequence {b} (K {K}): {msg}")
     assert not fails, "; ".join(fails)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("pool", ["stacked", "interleaved"])
-@pytest.mark.parametrize("fp8", [None, (0.0371, 0.0093)])
+@pytest.mark.parametrize("fp8", [None, (0.0371, 0.0093), (0.0213, 0.0371, 0.0093)])
 def test_varlen_cache_poisoned_layouts(tfa, pool, fp8):
-    """tfa_attn_varlen_kvcache_fwd: one mixed batch of prefill chunks and one-token decodes with an append, packed q a
-    view of a head-padded buffer, k_new / v_new interleaved views, out and lse between poison guards."""
+    """tfa_attn_varlen_kvcache_fwd (16-bit and FP8 pools, e4m3 q): one mixed batch of prefill chunks and one-token
+    decodes with an append, packed q a view of a head-padded buffer, k_new / v_new interleaved views, out and lse
+    between poison guards."""
     import numpy as np
     sq = [129, 1, 1, 300, 0, 1, 64, 1]
     lens = [0, 1, 127, 128, 300, 255, 513, 383]
@@ -656,16 +681,18 @@ def test_varlen_cache_poisoned_layouts(tfa, pool, fp8):
     g = torch.Generator().manual_seed(81)
     mk = lambda *s: torch.empty(s).normal_(0.0, 0.5, generator=g).to(dt).cuda()
     q, kn, vn = mk(total, Hq, D), mk(total, Hkv, D), mk(total, Hkv, D)
+    q = quantize_q(q, fp8)
     cu = torch.tensor(np.concatenate([[0], np.cumsum(sq)]), dtype=torch.int32, device="cuda")
-    ks, vs = fp8 or (1.0, 1.0)
+    ks, vs = fp8[-2:] if fp8 else (1.0, 1.0)
+    qkw = dict(q_scale=fp8[0], out_dtype=dt) if len(fp8 or ()) == 3 else {}
     scale = D ** -0.5
     k1, v1 = kp.clone(), vp.clone()
     out, lse = tfa.attn_varlen_kvcache_fwd(q, k1, v1, cu, max(sq), sl, table, kn, vn, is_causal=True, scale=scale,
-                                           k_scale=ks, v_scale=vs)
+                                           k_scale=ks, v_scale=vs, **qkw)
     torch.cuda.synchronize()
-    which = 1 if fp8 else 2
+    which = 2 if fp8 is None else len(fp8) - 1
     pools = CachePools(pool, kp, vp, table, Ls, which)
-    pq = Poisoned(*head_padded(tuple(q.shape)), dt, which, "cuda", q)
+    pq = Poisoned(*head_padded(tuple(q.shape)), q.dtype, which, "cuda", q)
     shape, fns = new_layout(tuple(kn.shape))
     pn = Poisoned(shape, lambda b: b, dt, which + 1, "cuda")
     bits(fns[0](pn.buf)).copy_(bits(kn))
@@ -675,7 +702,7 @@ def test_varlen_cache_poisoned_layouts(tfa, pool, fp8):
     plse = Poisoned(*guarded_layout(tuple(lse.shape)), torch.float32, which + 1, "cuda")
     tfa.attn_varlen_kvcache_fwd(pq.view, pools.views[0], pools.views[1], cu, max(sq), sl, table, fns[0](pn.buf),
                                 fns[1](pn.buf), is_causal=True, scale=scale, out=pout.view, lse=plse.view, k_scale=ks,
-                                v_scale=vs)
+                                v_scale=vs, **qkw)
     torch.cuda.synchronize()
     pq.assert_kept("q", whole=True)
     pn.assert_kept("k_new / v_new", whole=True)
@@ -688,9 +715,8 @@ def test_varlen_cache_poisoned_layouts(tfa, pool, fp8):
     for b, ((r0, r1), K) in enumerate(zip(offsets(sq), Ks)):
         if r1 == r0:
             continue
-        ref = reference(q[r0:r1].permute(1, 0, 2)[None], _gather(k1, table, b, K), _gather(v1, table, b, K), True,
-                        scale, ks, vs)
-        verdict = compare(out[r0:r1].permute(1, 0, 2)[None], lse[:, r0:r1][None], ref, kind)
-        if not verdict.ok:
-            fails.append(f"sequence {b} (Sq {r1 - r0}, K {K}): {verdict.msg}")
+        ok, msg = check_seq(q[r0:r1].permute(1, 0, 2)[None], _gather(k1, table, b, K), _gather(v1, table, b, K),
+                            out[r0:r1].permute(1, 0, 2)[None], lse[:, r0:r1][None], True, scale, fp8, kind)
+        if not ok:
+            fails.append(f"sequence {b} (Sq {r1 - r0}, K {K}): {msg}")
     assert not fails, "; ".join(fails)

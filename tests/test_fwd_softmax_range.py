@@ -410,6 +410,13 @@ def workloads():
         out.append(W(f"fp8_varlen_cache_{pat}", "varlen_cache", pat,
                      dict(sq=sq, lens=_lens_cache(800 + i, len(sq), 256)[:len(sq)], Hq=16 if big else 8, Hkv=4, D=D,
                           kind=kind, page=256, causal=True, append=True, kvfp8="auto")))
+        # e4m3 queries against the FP8 cache: q, k and v quantized, both products on FP8 wgmma
+        out.append(W(f"qkv8_cache_{pat}", "cache", pat, dict(lens=_lens_cache(900 + i, 48 if big else 8, 128),
+                                                             Sq=1, snew=1, Hq=16, Hkv=4, D=D, kind=kind, page=128,
+                                                             causal=True, ns=1 if big else 3, fp8=fp8, kvfp8=fp8)))
+        out.append(W(f"qkv8_varlen_cache_{pat}", "varlen_cache", pat,
+                     dict(sq=sq, lens=_lens_cache(1000 + i, len(sq), 256)[:len(sq)], Hq=16 if big else 8, Hkv=4,
+                          D=D, kind=kind, page=256, causal=True, append=True, fp8=fp8, kvfp8=fp8)))
     return out
 
 
@@ -550,6 +557,8 @@ def _run_cache(tfa, w, seqs, sc, scale):
     D, kind, Hq, Hkv, page = kw["D"], kw["kind"], kw["Hq"], kw["Hkv"], kw["page"]
     dt = _dt(kind)
     kvfp8 = kw.get("kvfp8")
+    qkv8 = bool(kw.get("fp8"))      # e4m3 q codes against the FP8 cache, out in the workload's dtype
+    qkw = dict(q_scale=sc[0], out_dtype=dt) if qkv8 else {}
     varlen = w.mode == "varlen_cache"
     B = len(seqs)
     n_app = [s.q.shape[1] if (varlen and kw["append"]) else (0 if varlen else kw["snew"]) for s, _ in seqs]
@@ -586,7 +595,8 @@ def _run_cache(tfa, w, seqs, sc, scale):
     rotary = kw.get("rotary")
     q_rot = None
     if varlen:
-        q = torch.cat([s.q.permute(1, 0, 2) for s, _ in seqs]).to(dt).cuda()
+        q = (torch.cat([c[0].permute(1, 0, 2) for _, c in seqs]) if qkv8 else
+             torch.cat([s.q.permute(1, 0, 2) for s, _ in seqs]).to(dt)).cuda()
         cu = torch.tensor([0] + np.cumsum(kw["sq"]).tolist(), dtype=torch.int32, device="cuda")
         kn = torch.cat([x[0] for x in new]).cuda() if kw["append"] else None
         vn = torch.cat([x[1] for x in new]).cuda() if kw["append"] else None
@@ -594,13 +604,14 @@ def _run_cache(tfa, w, seqs, sc, scale):
         ob, out = guarded((total, Hq, D), dt)
         lb, lse = guarded((Hq, total), torch.float32)
         tfa.attn_varlen_kvcache_fwd(q, k1, v1, cu, max(kw["sq"]), sl, table.cuda(), kn, vn, is_causal=kw["causal"],
-                                    scale=scale, out=out, lse=lse, k_scale=ks, v_scale=vs)
+                                    scale=scale, out=out, lse=lse, k_scale=ks, v_scale=vs, **qkw)
         items = -(-max(kw["sq"]) // BN) * B * Hq
         per = [(out[a:b].permute(1, 0, 2)[None], lse[:, a:b][None]) for a, b in offsets(kw["sq"])]
         qs = [s.q for s, _ in seqs]
     else:
         Sq, snew = kw["Sq"], kw["snew"]
-        q = torch.stack([s.q.permute(1, 0, 2) for s, _ in seqs]).to(dt).cuda()
+        q = (torch.stack([c[0].permute(1, 0, 2) for _, c in seqs]) if qkv8 else
+             torch.stack([s.q.permute(1, 0, 2) for s, _ in seqs]).to(dt)).cuda()
         kn = torch.stack([x[0] for x in new]).cuda() if snew else None
         vn = torch.stack([x[1] for x in new]).cuda() if snew else None
         rot = {}
@@ -614,7 +625,7 @@ def _run_cache(tfa, w, seqs, sc, scale):
         lb, lse = guarded((B, Hq, Sq), torch.float32)
         _, _, n = tfa.attn_kvcache_fwd(q, k1, v1, sl, table.cuda(), kn, vn, is_causal=kw["causal"], scale=scale,
                                        num_splits=kw.get("ns", 1), out=out, lse=lse, return_splits=True, k_scale=ks,
-                                       v_scale=vs, **rot)
+                                       v_scale=vs, **rot, **qkw)
         items = -(-Sq // BN) * B * Hq * n
         per = [(out[b:b + 1].permute(0, 2, 1, 3), lse[b:b + 1]) for b in range(B)]
         qs = [s.q for s, _ in seqs]
@@ -836,9 +847,10 @@ def _has_gpu():
 
 def test_every_entry_point_takes_the_largest_scale_and_rejects_the_next(tfa):
     """softmax_scale at the largest accepted float passes the scale check, the next float up is TFA_EINVAL_SCALE, in
-    every call; for the FP8 calls the same for s'.  Accepted calls are stopped before any device work by a later
-    argument error (split-KV without a workspace, max_seqlen_q = 0, more than 7 exchange peers), or by TFA_EARCH
-    without an H100; the two FP8 varlen calls have no later check and are taken on the GPU by the boundary test."""
+    every call; for the FP8 calls the same for s', through k_scale and, for the e4m3-query calls, through q_scale.
+    Accepted calls are stopped before any device work by a later argument error (split-KV without a workspace,
+    max_seqlen_q = 0, more than 7 exchange peers), or by TFA_EARCH without an H100; the FP8 varlen calls' s' has no
+    later check, so only a machine without an H100 takes the largest s' here."""
     top, above = largest_scale()
     L = tfa.lib()
     A = 0x100000
@@ -880,6 +892,15 @@ def test_every_entry_point_takes_the_largest_scale_and_rejects_the_next(tfa):
         "tfa_attn_varlen_kvcache_fwd": (lambda s: L.tfa_attn_varlen_kvcache_fwd(by(vcache(s))), (-12,)),
         "tfa_attn_varlen_kvcache_fp8_fwd": (lambda s: L.tfa_attn_varlen_kvcache_fp8_fwd(by(vcache(s)), by(kvq())),
                                             (-12,)),
+        "tfa_attn_varlen_kvcache_rotary_fwd": (lambda s: L.tfa_attn_varlen_kvcache_rotary_fwd(by(vcache(s)), by(rot),
+                                                                                             None), (-12,)),
+        "tfa_attn_kvcache_qkv8_fwd": (lambda s: L.tfa_attn_kvcache_qkv8_fwd(by(cache(s)), by(quant())), (-11, -7)),
+        "tfa_attn_kvcache_qkv8_fwd q_scale s'": (lambda s: L.tfa_attn_kvcache_qkv8_fwd(by(cache(1.0)), by(quant(s))),
+                                                 (-11, -7)),
+        "tfa_attn_kvcache_qkv8_fwd k_scale s'": (
+            lambda s: L.tfa_attn_kvcache_qkv8_fwd(by(cache(1.0)), by(quant(1.0, s))), (-11, -7)),
+        "tfa_attn_varlen_kvcache_qkv8_fwd": (lambda s: L.tfa_attn_varlen_kvcache_qkv8_fwd(by(vcache(s)), by(quant())),
+                                             (-12,)),
         "tfa_fwd_multi": (lambda s: L.tfa_fwd_multi(by(tfa.FwdArgs(A, A, A, A, A, 1, 4, 256, 128, 4 * 256 * 128,
                                                                    256 * 128, 128, 0, 0, s, 0, None)),
                                                     (ctypes.c_void_p * 8)(*([A] * 8)), 8), (-3, -7)),
@@ -889,6 +910,10 @@ def test_every_entry_point_takes_the_largest_scale_and_rejects_the_next(tfa):
             lambda s: L.tfa_attn_varlen_fp8_fwd(by(varlen(1.0, 300)), by(quant(1.0, s))), (-7,))
         calls["tfa_attn_varlen_kvcache_fp8_fwd s'"] = (
             lambda s: L.tfa_attn_varlen_kvcache_fp8_fwd(by(vcache(1.0, 1)), by(kvq(s))), (-7,))
+        calls["tfa_attn_varlen_kvcache_qkv8_fwd q_scale s'"] = (
+            lambda s: L.tfa_attn_varlen_kvcache_qkv8_fwd(by(vcache(1.0, 1)), by(quant(s))), (-7,))
+        calls["tfa_attn_varlen_kvcache_qkv8_fwd k_scale s'"] = (
+            lambda s: L.tfa_attn_varlen_kvcache_qkv8_fwd(by(vcache(1.0, 1)), by(quant(1.0, s))), (-7,))
     for name, (call, accepted) in calls.items():
         assert call(top) in accepted, (name, call(top))
         assert call(above) == -9, (name, call(above))
@@ -897,6 +922,8 @@ def test_every_entry_point_takes_the_largest_scale_and_rejects_the_next(tfa):
     # the two FP8 varlen calls reject s' above the bound before any device work on every machine
     assert L.tfa_attn_varlen_fp8_fwd(by(varlen(1.0, 300)), by(quant(1.0, above))) == -9
     assert L.tfa_attn_varlen_kvcache_fp8_fwd(by(vcache(1.0, 1)), by(kvq(above))) == -9
+    assert L.tfa_attn_varlen_kvcache_qkv8_fwd(by(vcache(1.0, 1)), by(quant(above))) == -9
+    assert L.tfa_attn_varlen_kvcache_qkv8_fwd(by(vcache(1.0, 1)), by(quant(1.0, above))) == -9
     # tfa_fwd and tfa_fwd_host: the next float up is rejected before any device work
     assert L.tfa_fwd(A, A, A, A, A, 1, 4, 256, 128, 0, 0, above, None) == -9
     h = np.zeros(64 * 64, dtype=np.uint16)
