@@ -471,8 +471,9 @@ int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quan
  *   result   : each sequence's out and lse are bit-identical to tfa_attn_fp8_fwd() (num_splits = 1) on that sequence
  *              alone, with its q rows, its first K_b cached keys and values gathered into contiguous tensors, the same
  *              scales, causal flag and output dtype (a sequence with K_b = 0 gets out = 0 / lse = +inf).
- *   rotary   : not supported: q arrives quantized, so a RoPE caller rotates before it quantizes, or keeps
- *              tfa_attn_kvcache_fp8_fwd() with `rotary`.
+ *   rotary   : not supported here: q arrives quantized.  A caller with a 16-bit q -- rotated or not -- takes
+ *              tfa_attn_kvcache_qkv8_q16_fwd() / tfa_attn_varlen_kvcache_qkv8_q16_fwd() below, which rotate and
+ *              quantize q in the append's launch.
  * Every check runs before any device work, in this order: the cache arguments (TFA_EINVAL_KVCACHE), the shapes,
  * strides, dtype and scale of the 16-bit call, (varlen) cu_seqlens_q / max_seqlen_q (TFA_EINVAL_SEQLENS), the
  * quantization (TFA_EINVAL_QKVQUANT for qkv_dtype, the scales, and q or cache strides that are not multiples of 16;
@@ -480,6 +481,43 @@ int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quan
  * + 1 with k_new, + 1 with split-KV. */
 int tfa_attn_kvcache_qkv8_fwd(const tfa_attn_kvcache_args* args, const tfa_qkv_quant_args* quant);
 int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_qkv_quant_args* quant);
+
+/* ---- the e4m3-query cache calls fed from a 16-bit q: rotate (optionally) and quantize q in the append's launch ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect them by the exported symbols
+ * tfa_attn_kvcache_qkv8_q16_fwd and tfa_attn_varlen_kvcache_qkv8_q16_fwd.  With q' = rot(q) rounded to q's dtype as
+ * tfa_attn_kvcache_rotary_fwd() / tfa_attn_varlen_kvcache_rotary_fwd() round it (q' = q when `rotary` is NULL), the
+ * append writes q8 = e4m3_rn_satfinite(q' / q_scale) -- IEEE fp32 division, bit-identical to torch's
+ * (q'.float() / q_scale).clamp(-448, 448).to(torch.float8_e4m3fn) -- into the scratch `q8`, quantizes k_new / v_new
+ * (rot(k_new) with rotary) into the cache, and tfa_attn_kvcache_qkv8_fwd() / tfa_attn_varlen_kvcache_qkv8_fwd() then
+ * run on q8.  The caller's q and k_new are not modified.
+ *
+ *   q        : 16-bit (args->dtype), in the 16-bit cache calls' layout: strides multiples of 8 elements, unit head_dim
+ *              stride.  args->dtype is also the dtype of out (unless out_fp32), k_new / v_new and cos / sin.
+ *   k_cache, v_cache : e4m3 codes, strides multiples of 16 (TFA_EINVAL_QKVQUANT otherwise).
+ *   rotary   : NULL, or as tfa_attn_kvcache_rotary_fwd() / tfa_attn_varlen_kvcache_rotary_fwd() (positions included),
+ *              except that q_rot is not read and may be NULL.  Rotary needs k_new (TFA_EINVAL_ROTARY otherwise);
+ *              quantizing alone does not.
+ *   quant    : the e4m3-query call's tfa_qkv_quant_args: q_scale quantizes q', k_scale / v_scale the cache.
+ *   q8       : contiguous DEVICE scratch of e4m3 codes, 16-byte aligned, not overlapping any other argument: (B, Sq, Hq,
+ *              D) for the dense-query call, (total_q, Hq, D) for the varlen one.  After the call it holds q8: every row
+ *              for the dense-query call, rows cu[b] + i with i < n_b for the varlen one (other rows are unspecified
+ *              and do not influence any result).  The e4m3-query call's stride rule applies to this layout.
+ *   result   : out and lse are bit-identical to tfa_attn_kvcache_qkv8_fwd() / tfa_attn_varlen_kvcache_qkv8_fwd() given
+ *              q8, the same scales and args->dtype; out keeps q's element strides (dense-query call) or is (total_q,
+ *              Hq, D) contiguous (varlen call).  The pools are bit-identical to tfa_attn_kvcache_fp8_fwd()'s /
+ *              tfa_attn_varlen_kvcache_rotary_fwd()'s with the same rotary (tfa_attn_varlen_kvcache_fp8_fwd()'s
+ *              without it).  Lengths, the capacity clamp, dropped tokens, key-less rows, split-KV (dense-query call
+ *              only) and CUDA-graph capture are those of the e4m3-query calls.
+ * Every check runs before any device work, in this order: a NULL args or quant, or a NULL or misaligned q8
+ * (TFA_EINVAL_PTR); the cache arguments (TFA_EINVAL_KVCACHE); the shapes, strides, dtype and scale of the 16-bit call;
+ * (varlen) cu_seqlens_q / max_seqlen_q (TFA_EINVAL_SEQLENS); the rotary arguments but q_rot (TFA_EINVAL_ROTARY); the
+ * quantization (TFA_EINVAL_QKVQUANT, then TFA_EINVAL_SCALE for s'); then the device (TFA_EARCH).  Launches: 2 (the
+ * quantizing append, the attention), + 1 with split-KV, with or without k_new. */
+int tfa_attn_kvcache_qkv8_q16_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary /* NULL: none */,
+                                  const tfa_qkv_quant_args* quant, void* q8);
+int tfa_attn_varlen_kvcache_qkv8_q16_fwd(const tfa_attn_varlen_kvcache_args* args,
+                                         const tfa_rotary_args* rotary /* NULL: none */,
+                                         const tfa_qkv_quant_args* quant, void* q8);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

@@ -429,12 +429,14 @@ KvcacheCall check_kvcache(const torch::Tensor& q, const torch::Tensor& k_cache, 
 
 // The dense-query cache call once every argument passed: allocates out (q's strides; a non-dense q is replaced by its
 // contiguous copy first), lse, the split-KV workspace and, with rotary (`r`), q_rot, and runs the call.  `quant`
-// nullptr: a 16-bit cache.  `qkv8` (with `r` and `quant` nullptr): e4m3 q against an e4m3 cache, out in `out_dtype`.
+// nullptr: a 16-bit cache.  `qkv8` (with `quant` nullptr): e4m3 q against an e4m3 cache, out in `out_dtype`; with
+// `q16` q is 16-bit instead (out_dtype its dtype), and the call quantizes it (rot(q) with `r`) into a q8 scratch
+// allocated here.
 std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float softmax_scale, int64_t num_splits,
                                        tfa_rotary_args* r, const tfa_kv_quant_args* quant,
                                        const tfa_qkv_quant_args* qkv8 = nullptr,
-                                       at::ScalarType out_dtype = at::kBFloat16) {
-  torch::Tensor out, lse, ws, q_rot;
+                                       at::ScalarType out_dtype = at::kBFloat16, bool q16 = false) {
+  torch::Tensor out, lse, ws, q_rot, q8;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(c.q.device());
@@ -478,11 +480,14 @@ std::vector<torch::Tensor> kvcache_fwd(KvcacheCall& c, bool is_causal, float sof
     d.num_splits = a.num_splits;
     ws = split_workspace(d, c.q);
     a.num_splits = d.num_splits; a.workspace = d.workspace; a.workspace_bytes = d.workspace_bytes;
-    if (r) {
+    if (q16) {
+      q8 = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().dtype(at::kFloat8_e4m3fn));
+    } else if (r) {
       q_rot = torch::empty({c.B, c.Sq, c.Hq, c.D}, c.q.options().memory_format(at::MemoryFormat::Contiguous));
       r->q_rot = q_rot.data_ptr();
     }
-    rc = qkv8  ? tfa_attn_kvcache_qkv8_fwd(&a, qkv8)
+    rc = q16   ? tfa_attn_kvcache_qkv8_q16_fwd(&a, r, qkv8, q8.data_ptr())
+         : qkv8  ? tfa_attn_kvcache_qkv8_fwd(&a, qkv8)
          : quant ? tfa_attn_kvcache_fp8_fwd(&a, r, quant)
          : r     ? tfa_attn_kvcache_rotary_fwd(&a, r)
                  : tfa_attn_kvcache_fwd(&a);
@@ -589,7 +594,9 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
 namespace {
 
 // flash_attention_v2_varlen_kvcache, or with `quant` its FP8-cache form; with rotary_cos / rotary_sin, q and k_new
-// are rotated first (tfa_attn_varlen_kvcache_rotary_fwd) through a q_rot allocated here.
+// are rotated first (tfa_attn_varlen_kvcache_rotary_fwd) through a q_rot allocated here.  `qkv8`: the e4m3-query form,
+// on an e4m3 q, or with `q16` on a 16-bit q (out_dtype its dtype) quantized, and rotated with rotary_cos / rotary_sin,
+// into an e4m3 scratch allocated here (tfa_attn_varlen_kvcache_qkv8_q16_fwd).
 std::vector<torch::Tensor> varlen_kvcache(
     const torch::Tensor& q, const torch::Tensor& k_cache, const torch::Tensor& v_cache,
     const torch::Tensor& cu_seqlens_q, int64_t max_seqlen_q, const torch::Tensor& cache_seqlens,
@@ -597,7 +604,7 @@ std::vector<torch::Tensor> varlen_kvcache(
     const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant,
     const std::optional<torch::Tensor>& rotary_cos = std::nullopt,
     const std::optional<torch::Tensor>& rotary_sin = std::nullopt, bool rotary_interleaved = false,
-    const tfa_qkv_quant_args* qkv8 = nullptr, at::ScalarType out_dtype = at::kBFloat16) {
+    const tfa_qkv_quant_args* qkv8 = nullptr, at::ScalarType out_dtype = at::kBFloat16, bool q16 = false) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
@@ -609,7 +616,7 @@ std::vector<torch::Tensor> varlen_kvcache(
   const int64_t B = cu_seqlens_q.numel() - 1;
   const CacheShape cs = check_cache(q, B, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new,
                                     quant != nullptr || qkv8 != nullptr,
-                                    qkv8 ? std::optional<at::ScalarType>(out_dtype) : std::nullopt);
+                                    qkv8 && !q16 ? std::optional<at::ScalarType>(out_dtype) : std::nullopt);
   const int64_t nblk = cs.nblk, page = cs.page, Hkv = cs.Hkv, mbps = cs.mbps, bts = cs.bts;
   if (k_new.has_value()) {
     const torch::Tensor &kn = *k_new, &vn = *v_new;
@@ -632,7 +639,7 @@ std::vector<torch::Tensor> varlen_kvcache(
   if (rotary_cos.has_value())
     r = check_rotary(q, D, mbps * page, k_new.has_value(), *rotary_cos, *rotary_sin, rotary_interleaved);
 
-  torch::Tensor out, lse, q_rot;
+  torch::Tensor out, lse, q_rot, q8;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
@@ -662,7 +669,10 @@ std::vector<torch::Tensor> varlen_kvcache(
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
-    if (qkv8) {
+    if (q16) {
+      q8 = torch::empty({total_q, Hq, D}, q.options().dtype(at::kFloat8_e4m3fn));
+      rc = tfa_attn_varlen_kvcache_qkv8_q16_fwd(&a, rotary_cos.has_value() ? &r : nullptr, qkv8, q8.data_ptr());
+    } else if (qkv8) {
       rc = tfa_attn_varlen_kvcache_qkv8_fwd(&a, qkv8);
     } else if (rotary_cos.has_value()) {
       q_rot = torch::empty({total_q, Hq, D}, q.options().memory_format(at::MemoryFormat::Contiguous));
@@ -751,6 +761,40 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_qkv8(
                         is_causal, softmax_scale, nullptr, std::nullopt, std::nullopt, false, &qa, out_dtype);
 }
 
+// The e4m3-query cache call fed from a 16-bit q (tfa_attn_kvcache_qkv8_q16_fwd in include/tfa_b200.h): q (B, Sq, Hq, D)
+// bfloat16 / float16, rotated with rotary_cos / rotary_sin as flash_attention_v2_kvcache_rotary when given, is quantized
+// with q_scale into an e4m3 scratch in the append's launch; k_cache / v_cache, k_new / v_new (q's dtype) and the scales
+// as flash_attention_v2_kvcache_qkv8.  out (q's dtype) takes q's strides.
+std::vector<torch::Tensor> flash_attention_v2_kvcache_qkv8_q16(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cache_seqlens,
+    std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new, std::optional<torch::Tensor> v_new,
+    double q_scale, double k_scale, double v_scale, bool is_causal, float softmax_scale, int64_t num_splits,
+    std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin, bool rotary_interleaved) {
+  KvcacheCall c = check_kvcache(q, k_cache, v_cache, cache_seqlens, block_table, k_new, v_new, num_splits, true);
+  const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
+  TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
+  tfa_rotary_args r;
+  if (rotary_cos.has_value())
+    r = check_rotary(c.q, c.D, c.mbps * c.page, c.snew > 0, *rotary_cos, *rotary_sin, rotary_interleaved);
+  return kvcache_fwd(c, is_causal, softmax_scale, num_splits, rotary_cos.has_value() ? &r : nullptr, nullptr, &qa,
+                     c.q.scalar_type(), true);
+}
+
+// The packed variable-length form: q (total_q, Hq, D) bfloat16 / float16 with cu_seqlens_q as
+// flash_attention_v2_varlen_kvcache; the rest as flash_attention_v2_kvcache_qkv8_q16.  Returns out (total_q, Hq, D) in
+// q's dtype and lse (Hq, total_q).  No split-KV.
+std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_qkv8_q16(
+    torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
+    torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
+    std::optional<torch::Tensor> v_new, double q_scale, double k_scale, double v_scale, bool is_causal,
+    float softmax_scale, std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin,
+    bool rotary_interleaved) {
+  const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
+  return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
+                        is_causal, softmax_scale, nullptr, rotary_cos, rotary_sin, rotary_interleaved, &qa,
+                        q.scalar_type(), true);
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("flash_attention_v2_cutlass", &flash_attention_v2_cutlass,
         "Flash attention v2 forward, H100-native (sm_90a wgmma/TMA)");
@@ -813,6 +857,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
         py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"),
         py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"));
+  m.def("flash_attention_v2_kvcache_qkv8_q16", &flash_attention_v2_kvcache_qkv8_q16,
+        "bfloat16 / float16 q, optionally rotated (RoPE), quantized to e4m3 in the append's launch and run against an "
+        "FP8 (float8_e4m3fn) cache on e4m3 tensor cores -> [out (q's dtype), lse]",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("block_table"),
+        py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"), py::arg("k_scale"), py::arg("v_scale"),
+        py::arg("is_causal"), py::arg("softmax_scale"), py::arg("num_splits"), py::arg("rotary_cos") = py::none(),
+        py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
+  m.def("flash_attention_v2_varlen_kvcache_qkv8_q16", &flash_attention_v2_varlen_kvcache_qkv8_q16,
+        "a packed variable-length batch of bfloat16 / float16 queries, optionally rotated (RoPE), quantized to e4m3 in "
+        "the append's launch and run against an FP8 (float8_e4m3fn) cache on e4m3 tensor cores -> [out (q's dtype), "
+        "lse]",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
+        py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"),
+        py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"),
+        py::arg("rotary_cos") = py::none(), py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

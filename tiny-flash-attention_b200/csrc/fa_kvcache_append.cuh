@@ -3,6 +3,8 @@
 //   * ROTARY: q and k_new are rotated (RoPE) at their cache positions on the way, and rot(q) goes to a scratch buffer
 //     the forward reads in place of q.
 //   * FP8: the cache is e4m3 with per-tensor scales; k_new / v_new (rot(k_new) with ROTARY) are quantized on the way.
+//   * Q8 (with FP8): q (rot(q) with ROTARY) is quantized to e4m3 on the way too, into a scratch buffer the e4m3-query
+//     forward reads in place of q.
 #pragma once
 #include "ptx_sm90.cuh"
 #include "fa_fwd_sm90.cuh"    // the KV-cache address helpers the append shares with the forward
@@ -166,24 +168,25 @@ __device__ __forceinline__ uint4 rotate_chunk(const uint16_t* row, int sub, cons
                     pack_16x2<IS_BF16>(r[6], r[7]));
 }
 
-// The parameter block of kvcache_append_kernel: the append, and the rotated queries of a ROTARY launch.  Without
-// ROTARY only `ap` is read and q_chunks is 0.  With it, chunks [0, q_chunks) write rot(q) into q_rot, and the remaining
-// ap.chunks ones write rot(k_new) and v_new (unrotated) into the cache, through append_chunk().  The query chunks cover
+// The parameter block of kvcache_append_kernel: the append, and the queries of a ROTARY or Q8 launch.  Without either
+// only `ap` is read and q_chunks is 0.  With them, chunks [0, q_chunks) write rot(q) (ROTARY), e4m3(q / q_scale) (Q8)
+// or e4m3(rot(q) / q_scale) (both) into q_rot, and the remaining ap.chunks ones write rot(k_new) and v_new (unrotated)
+// into the cache, through append_chunk() -- none without k_new, which only a Q8 launch allows.  The query chunks cover
 // Sq rows of every sequence, as the key chunks cover snew: the dense-query call's Sq rows of (B, Sq, Hq, D) q, written
 // to the contiguous (B, Sq, Hq, D) q_rot; or, packed (ap.cu_q set, Sq = snew = max_seqlen_q), rows q0_b + i of
 // (total_q, Hq, D) q for i < n_b (seq_rows()), written to the same rows of the contiguous (total_q, Hq, D) q_rot -- a
 // chunk with i >= n_b returns.  Positions: seq_rotary_pos().  A NeoX chunk also reads its partner chunk, and every
 // rotated chunk 16 bytes each of cos and sin.  Algorithmic bytes of the rotated queries: 2 * (query rows)*Hq*D * 2
-// (q in, q_rot out), plus the cos/sin rows.
+// (q in, q_rot out; 1 byte per element out with Q8), plus the cos/sin rows.
 struct AppendKernelParams {
   AppendParams ap;                // the append; ap.chunks = B * snew * Hkv * D / 8
   const void* q;
-  void* q_rot;                    // (B, Sq, Hq, D) contiguous; packed: (total_q, Hq, D)
+  void* q_rot;                    // (B, Sq, Hq, D) contiguous; packed: (total_q, Hq, D); e4m3 codes with Q8
   long long q_sb, q_ss, q_sh;     // element strides of q (q_sb = 0 when packed)
   const void* cos;                // (seqlen_ro, rotary_dim / 2) contiguous, q's dtype
   const void* sin;
   int Sq, Hq, rotary_dim, seqlen_ro, causal;
-  long long q_chunks;             // B * Sq * Hq * D / 8 with ROTARY, else 0
+  long long q_chunks;             // B * Sq * Hq * D / 8 with ROTARY or Q8, else 0
 };
 
 // ---- FP8 (e4m3) cache: the append quantizes what it would have stored ----
@@ -193,6 +196,7 @@ struct AppendKernelParams {
 // rotary the key is rotated and rounded to q's dtype first, as the 16-bit rotary append stores it.
 struct KvQuant {
   float k_scale, v_scale;
+  float q_scale;                  // read only by a Q8 launch: q8 = e4m3_rn_satfinite(q / q_scale), the same way
 };
 __device__ __forceinline__ float div_rn(float a, float b) {
   float d;
@@ -218,14 +222,16 @@ __device__ __forceinline__ uint2 quantize_chunk(const uint4& x, float scale) {
 }
 
 // One thread per 16-byte chunk of q_chunks + ap.chunks.  IS_BF16 is the dtype of q / k_new / v_new; the copy without
-// ROTARY or FP8 does not depend on it.  `qs` is read only with FP8: 16 bytes of k_new / v_new in, 8 bytes of codes out.
-template <int D, bool IS_BF16, bool ROTARY, bool INTERLEAVED, bool FP8>
+// ROTARY or FP8 does not depend on it.  `qs` is read only with FP8: 16 bytes of k_new / v_new in, 8 bytes of codes out;
+// with Q8 likewise 16 bytes of q (rotated and rounded to q's dtype first with ROTARY) in, 8 bytes of q8 codes out.
+template <int D, bool IS_BF16, bool ROTARY, bool INTERLEAVED, bool FP8, bool Q8 = false>
 __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendKernelParams p, const KvQuant qs) {
+  static_assert(FP8 || !Q8, "an e4m3 q goes with an e4m3 cache");
   long long c = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
   const AppendParams& a = p.ap;
   const uint16_t* cos_tab = static_cast<const uint16_t*>(p.cos);
   const uint16_t* sin_tab = static_cast<const uint16_t*>(p.sin);
-  if constexpr (ROTARY) {
+  if constexpr (ROTARY || Q8) {
     if (c < p.q_chunks) {
       constexpr int CPR = D / 8;               // 16-byte chunks per row
       const int sub = static_cast<int>(c % CPR);
@@ -236,13 +242,22 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const AppendKernelP
       const int b = static_cast<int>(r / p.Sq);
       const SeqRows s = seq_rows(a, b);
       if (a.cu_q && i >= s.n) return;          // packed: past the sequence's rows
-      const long long ro = static_cast<long long>(seq_rotary_pos(__ldg(a.cache_seqlens + b), a.capacity, s.n, i,
-                                                                 p.causal != 0, true, p.seqlen_ro)) *
-                           (p.rotary_dim / 2);
       const uint16_t* row = static_cast<const uint16_t*>(p.q) + b * p.q_sb + (s.q0 + i) * p.q_ss + h * p.q_sh;
-      const uint4 y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_tab + ro, sin_tab + ro, p.rotary_dim);
+      uint4 y;
+      if constexpr (ROTARY) {
+        const long long ro = static_cast<long long>(seq_rotary_pos(__ldg(a.cache_seqlens + b), a.capacity, s.n, i,
+                                                                   p.causal != 0, true, p.seqlen_ro)) *
+                             (p.rotary_dim / 2);
+        y = rotate_chunk<IS_BF16, INTERLEAVED>(row, sub, cos_tab + ro, sin_tab + ro, p.rotary_dim);
+      } else {
+        y = __ldg(reinterpret_cast<const uint4*>(row) + sub);
+      }
       const long long out_row = a.cu_q ? static_cast<long long>(s.q0) + i : static_cast<long long>(b) * p.Sq + i;
-      reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + (out_row * p.Hq + h) * D)[sub] = y;
+      if constexpr (Q8)
+        reinterpret_cast<uint2*>(static_cast<uint8_t*>(p.q_rot) + (out_row * p.Hq + h) * D)[sub] =
+            quantize_chunk<IS_BF16>(y, qs.q_scale);
+      else
+        reinterpret_cast<uint4*>(static_cast<uint16_t*>(p.q_rot) + (out_row * p.Hq + h) * D)[sub] = y;
       return;
     }
     c -= p.q_chunks;

@@ -24,8 +24,8 @@
 #include <cstring>
 
 // tfa_append.cu: the append's launch, compiled apart from the forward kernels
-int tfa_internal_launch_append(const tfa::AppendKernelParams& p, const tfa::KvQuant* qs, int D, bool bf16, bool rotary,
-                               bool interleaved, cudaStream_t stream);
+int tfa_internal_launch_append(const tfa::AppendKernelParams& p, const tfa::KvQuant* qs, bool q8, int D, bool bf16,
+                               bool rotary, bool interleaved, cudaStream_t stream);
 
 namespace {
 
@@ -588,13 +588,13 @@ int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtens
   return 0;
 }
 
-// The rotary arguments of either cache call whose cache arguments passed (capacity = a.Sk).
+// The rotary arguments of either cache call whose cache arguments passed (capacity = a.Sk).  `q_rot` false: the call
+// writes its rotated queries elsewhere (the q8 scratch) and ra.q_rot is not read.
 template <typename Args>
-int validate_rotary(const Args& ka, const Problem& a, const tfa_rotary_args& ra) {
-  if (!ra.cos || !ra.sin || !ra.q_rot ||
-      ((reinterpret_cast<uintptr_t>(ra.cos) | reinterpret_cast<uintptr_t>(ra.sin) |
-        reinterpret_cast<uintptr_t>(ra.q_rot)) & 15u))
+int validate_rotary(const Args& ka, const Problem& a, const tfa_rotary_args& ra, bool q_rot = true) {
+  if (!ra.cos || !ra.sin || ((reinterpret_cast<uintptr_t>(ra.cos) | reinterpret_cast<uintptr_t>(ra.sin)) & 15u))
     return TFA_EINVAL_ROTARY;
+  if (q_rot && (!ra.q_rot || (reinterpret_cast<uintptr_t>(ra.q_rot) & 15u))) return TFA_EINVAL_ROTARY;
   if (ra.rotary_dim < 16 || ra.rotary_dim > a.D || ra.rotary_dim % 16) return TFA_EINVAL_ROTARY;
   if (ra.seqlen_ro < a.Sk) return TFA_EINVAL_ROTARY;      // every key position is below the capacity
   if (!ka.k_new) return TFA_EINVAL_ROTARY;                // as flash-attn: rotary rotates the appended keys
@@ -617,23 +617,47 @@ int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
   return 0;
 }
 
+// The query side of an append that writes the queries the forward reads: rot(q) (`ra`), or with `q8` the e4m3 codes of
+// q or rot(q) into q8.  Sets a.q to that scratch with its contiguous strides: (B, S, Hq, D), or packed (total_q, Hq, D)
+// when `packed` (S = max_seqlen_q rows of every sequence then).  out and lse keep their layout (a.ol).
+void set_query_append(tfa::AppendKernelParams& rp, Problem& a, const tfa_rotary_args* ra, void* q8, int S,
+                      bool packed) {
+  rp.q = a.q; rp.q_rot = q8 ? q8 : ra->q_rot;
+  rp.q_sb = packed ? 0 : a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
+  if (ra) {
+    rp.cos = ra->cos; rp.sin = ra->sin;
+    rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
+  }
+  rp.Sq = S; rp.Hq = a.Hq;
+  rp.causal = a.causal != 0 ? 1 : 0;
+  rp.q_chunks = static_cast<long long>(a.B) * S * a.Hq * (a.D / 8);
+  a.q = rp.q_rot;
+  a.qss = static_cast<long long>(a.Hq) * a.D;
+  a.qsh = a.D;
+  a.qsb = packed ? 0 : a.qss * a.Sq;
+}
+
 // `ra` nullptr: the plain cache forward.  Otherwise the append also rotates q and k_new, and the forward reads its
 // queries from ra->q_rot.  `quant` nullptr: a 16-bit cache; otherwise an FP8 one, into which the append quantizes and
-// which the kCacheFp8 forward reads.  `qkv8` (with `ra` and `quant` nullptr): e4m3 q against an FP8 cache, a.dtype the
-// output's and k_new's; the append quantizes as for `quant` and the kCacheQkv8 forward reads q and the cache on 8-bit
-// wgmma.
+// which the kCacheFp8 forward reads.  `qkv8` (with `quant` nullptr): e4m3 q against an FP8 cache, a.dtype the output's
+// and k_new's; the append quantizes as for `quant` and the kCacheQkv8 forward reads q and the cache on 8-bit wgmma.
+// Without `q8`, q arrives in e4m3 and `ra` is nullptr.  With `q8`, q is 16-bit: the append writes e4m3(q / q_scale)
+// (rot(q) with `ra`, ra->q_rot unused) into the contiguous scratch q8, the forward's q, whose layout the quantization
+// checks see.
 int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant,
-                 const tfa_qkv_quant_args* qkv8 = nullptr) {
+                 const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr) {
   Problem a = from_kvcache_args(ka);
   int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
-  if (ra && (rc = validate_rotary(ka, a, *ra))) return rc;
+  if (ra && (rc = validate_rotary(ka, a, *ra, q8 == nullptr))) return rc;
+  tfa::AppendKernelParams rp{};
+  if (ra || q8) set_query_append(rp, a, ra, q8, a.Sq, false);
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (qkv8) {
     if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
-    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale};
+    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale, qkv8->q_scale};
   }
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
@@ -641,21 +665,6 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
 
   SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
   if ((rc = plan_splits(a, plan))) return rc;
-
-  tfa::AppendKernelParams rp{};
-  if (ra) {
-    rp.q = a.q; rp.q_rot = ra->q_rot;
-    rp.q_sb = a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
-    rp.cos = ra->cos; rp.sin = ra->sin;
-    rp.Sq = a.Sq; rp.Hq = a.Hq; rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
-    rp.causal = a.causal != 0 ? 1 : 0;
-    rp.q_chunks = static_cast<long long>(a.B) * a.Sq * a.Hq * (a.D / 8);
-    // the forward reads rot(q), contiguous (B, Sq, Hq, D); out keeps the caller's q strides (ol)
-    a.q = ra->q_rot;
-    a.qss = static_cast<long long>(a.Hq) * a.D;
-    a.qsh = a.D;
-    a.qsb = a.qss * a.Sq;
-  }
 
   // qkv8: the 8-bit swizzled Q and K maps the wgmma reads in place, as fwd_impl builds them
   const bool fp8_cache = quant || qkv8;
@@ -666,9 +675,10 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
     return rc;
   if ((rc = setup_cache(ka, a, snew, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype, qkv8 != nullptr))) return rc;
   rp.ap.n_sb = ka.new_stride_b;
-  if (snew > 0) {                       // rotary needs k_new (validate_rotary): every rotary call appends
-    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
-                                    ra && ra->interleaved != 0, a.stream);
+  // rotary needs k_new (validate_rotary): every rotary call appends; a quantized q is written even without k_new
+  if (snew > 0 || q8) {
+    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, q8 != nullptr, a.D, a.dtype == TFA_BF16,
+                                    ra != nullptr, ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
 
@@ -701,39 +711,28 @@ Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
   return q;
 }
 
-// `ra`, `quant` and `qkv8` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and the
-// forward reads its queries from ra->q_rot.
+// `ra`, `quant`, `qkv8` and `q8` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and
+// the forward reads its queries from ra->q_rot (from q8 with `q8`).
 int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* ra,
-                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr) {
+                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr) {
   Problem a = from_varlen_kvcache_args(va);
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
   if ((rc = validate_seqlens_q(va))) return rc;
-  if (ra && (rc = validate_rotary(va, a, *ra))) return rc;
+  if (ra && (rc = validate_rotary(va, a, *ra, q8 == nullptr))) return rc;
+  // without rotary or q8 only rp.ap is used; with them the query chunks cover max_seqlen_q rows of every sequence, as
+  // the key chunks do (the append returns past n_b)
+  tfa::AppendKernelParams rp{};
+  if (ra || q8) set_query_append(rp, a, ra, q8, va.max_seqlen_q, true);
   tfa::KvQuant qs{1.0f, 1.0f};
   if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
   if (qkv8) {
     if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
-    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale};
+    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale, qkv8->q_scale};
   }
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
-
-  tfa::AppendKernelParams rp{};         // without rotary only rp.ap is used
-  if (ra) {
-    // the query chunks cover max_seqlen_q rows of every sequence, as the key chunks do (the append returns past n_b)
-    rp.q = a.q; rp.q_rot = ra->q_rot;
-    rp.q_sb = 0; rp.q_ss = a.qss; rp.q_sh = a.qsh;
-    rp.cos = ra->cos; rp.sin = ra->sin;
-    rp.Sq = va.max_seqlen_q; rp.Hq = a.Hq; rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
-    rp.causal = a.causal != 0 ? 1 : 0;
-    rp.q_chunks = static_cast<long long>(a.B) * va.max_seqlen_q * a.Hq * (a.D / 8);
-    // the forward reads rot(q), contiguous (total_q, Hq, D); out and lse are unchanged (ol)
-    a.q = ra->q_rot;
-    a.qss = static_cast<long long>(a.Hq) * a.D;
-    a.qsh = a.D;
-  }
 
   const bool fp8_cache = quant || qkv8;
   CUtensorMap tq, tk, tv;
@@ -743,11 +742,12 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
   if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype,
                         qkv8 != nullptr)))
     return rc;
-  if (va.k_new) {                       // rotary needs k_new (validate_rotary): every rotary call appends
+  // rotary needs k_new (validate_rotary): every rotary call appends; a quantized q is written even without k_new
+  if (va.k_new || q8) {
     rp.ap.cu_q = va.cu_seqlens_q;
     rp.ap.total_q = a.Sq;
-    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, a.D, a.dtype == TFA_BF16, ra != nullptr,
-                                    ra && ra->interleaved != 0, a.stream);
+    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, q8 != nullptr, a.D, a.dtype == TFA_BF16,
+                                    ra != nullptr, ra && ra->interleaved != 0, a.stream);
     if (rc) return rc;
   }
 
@@ -857,6 +857,18 @@ int tfa_attn_kvcache_qkv8_fwd(const tfa_attn_kvcache_args* args, const tfa_qkv_q
 int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
   return varlen_kvcache_impl(*args, nullptr, nullptr, quant);
+}
+
+int tfa_attn_kvcache_qkv8_q16_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary,
+                                  const tfa_qkv_quant_args* quant, void* q8) {
+  if (!args || !quant || !q8 || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
+  return kvcache_impl(*args, rotary, nullptr, quant, q8);
+}
+
+int tfa_attn_varlen_kvcache_qkv8_q16_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
+                                         const tfa_qkv_quant_args* quant, void* q8) {
+  if (!args || !quant || !q8 || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args, rotary, nullptr, quant, q8);
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {

@@ -29,10 +29,14 @@ int launch(void (*kern)(P...), long long chunks, cudaStream_t stream, const P&..
 }
 
 // The dtype and cache-type dispatch of one head dimension and rotary layout.  The 16-bit append without rotary copies
-// bits, so one instantiation serves both dtypes.
+// bits, so one instantiation serves both dtypes.  `q8`: q is quantized too (FP8 cache only).
 template <int D, bool ROTARY, bool INTERLEAVED>
-int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool bf16, cudaStream_t stream) {
+int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool q8, bool bf16, cudaStream_t stream) {
   const long long chunks = p.q_chunks + p.ap.chunks;
+  if (q8)
+    return launch(bf16 ? kvcache_append_kernel<D, true, ROTARY, INTERLEAVED, true, true>
+                       : kvcache_append_kernel<D, false, ROTARY, INTERLEAVED, true, true>,
+                  chunks, stream, p, *qs);
   if (qs)
     return launch(bf16 ? kvcache_append_kernel<D, true, ROTARY, INTERLEAVED, true>
                        : kvcache_append_kernel<D, false, ROTARY, INTERLEAVED, true>,
@@ -46,21 +50,22 @@ int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool bf16, cud
 }
 
 template <int D>
-int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool bf16, bool rotary, bool interleaved,
+int launch_append(const AppendKernelParams& p, const KvQuant* qs, bool q8, bool bf16, bool rotary, bool interleaved,
                   cudaStream_t stream) {
-  if (!rotary) return launch_append<D, false, false>(p, qs, bf16, stream);
-  return interleaved ? launch_append<D, true, true>(p, qs, bf16, stream)
-                     : launch_append<D, true, false>(p, qs, bf16, stream);
+  if (!rotary) return launch_append<D, false, false>(p, qs, q8, bf16, stream);
+  return interleaved ? launch_append<D, true, true>(p, qs, q8, bf16, stream)
+                     : launch_append<D, true, false>(p, qs, q8, bf16, stream);
 }
 
 }  // namespace
 
 // The append of either cache call, over p.q_chunks + p.ap.chunks chunks.  `qs` nullptr: a 16-bit cache; otherwise an
-// FP8 (e4m3) one, into which k_new / v_new (rot(k_new) with rotary) are quantized with its scales.  `rotary`: q and
-// k_new are rotated, with (2j, 2j+1) pairs when `interleaved`.  Returns 0, a cudaError_t, or TFA_EINVAL_SHAPE when the
-// grid does not fit.
-int tfa_internal_launch_append(const AppendKernelParams& p, const KvQuant* qs, int D, bool bf16, bool rotary,
+// FP8 (e4m3) one, into which k_new / v_new (rot(k_new) with rotary) are quantized with its scales.  `q8` (with `qs`):
+// the query chunks write q (rot(q) with rotary) quantized with qs->q_scale into the e4m3 scratch p.q_rot.  `rotary`: q
+// and k_new are rotated, with (2j, 2j+1) pairs when `interleaved`.  Returns 0, a cudaError_t, or TFA_EINVAL_SHAPE when
+// the grid does not fit.
+int tfa_internal_launch_append(const AppendKernelParams& p, const KvQuant* qs, bool q8, int D, bool bf16, bool rotary,
                                bool interleaved, cudaStream_t stream) {
-  return D == 64 ? launch_append<64>(p, qs, bf16, rotary, interleaved, stream)
-                 : launch_append<128>(p, qs, bf16, rotary, interleaved, stream);
+  return D == 64 ? launch_append<64>(p, qs, q8, bf16, rotary, interleaved, stream)
+                 : launch_append<128>(p, qs, q8, bf16, rotary, interleaved, stream);
 }

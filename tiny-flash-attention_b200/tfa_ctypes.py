@@ -165,6 +165,12 @@ def lib():
         L.tfa_attn_kvcache_qkv8_fwd.restype = ci
         L.tfa_attn_varlen_kvcache_qkv8_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(QkvQuantArgs)]
         L.tfa_attn_varlen_kvcache_qkv8_fwd.restype = ci
+        L.tfa_attn_kvcache_qkv8_q16_fwd.argtypes = [ctypes.POINTER(KvcacheArgs), ctypes.POINTER(RotaryArgs),
+                                                    ctypes.POINTER(QkvQuantArgs), vp]
+        L.tfa_attn_kvcache_qkv8_q16_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_qkv8_q16_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs),
+                                                           ctypes.POINTER(RotaryArgs), ctypes.POINTER(QkvQuantArgs), vp]
+        L.tfa_attn_varlen_kvcache_qkv8_q16_fwd.restype = ci
         L.tfa_selftest_wgmma_fp8.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp]
         L.tfa_selftest_wgmma_fp8.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
@@ -354,11 +360,21 @@ def _quant(k_cache, k_scale, v_scale):
     return KvQuantArgs(TFA_FP8_E4M3, float(k_scale), float(v_scale))
 
 
-def _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype):
+def _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype, q8_scale=None):
     """What a cache call takes of its element types and scales: (tfa_kv_quant_args or None, tfa_qkv_quant_args or None,
     the output dtype).  A float8_e4m3fn q needs a float8_e4m3fn cache (the e4m3-query calls, out in out_dtype, k_new in
-    out_dtype) and takes no rotary; a 16-bit q takes a cache of its own dtype or an FP8 one, and no q_scale / out_dtype."""
+    out_dtype) and takes no rotary; a 16-bit q takes a cache of its own dtype or an FP8 one, and no q_scale / out_dtype.
+    q8_scale: a 16-bit q quantized with it for the e4m3-query calls on a float8_e4m3fn cache (out and k_new in q's
+    dtype, rotary allowed)."""
     import torch
+    if q8_scale is not None:
+        if q.dtype == torch.float8_e4m3fn:
+            raise ValueError("q8_scale quantizes a 16-bit q; this q is float8_e4m3fn already (pass q_scale)")
+        if k_cache.dtype != torch.float8_e4m3fn:
+            raise TypeError(f"q8_scale needs a float8_e4m3fn cache, got {k_cache.dtype}")
+        if q_scale != 1.0 or out_dtype not in (None, q.dtype):
+            raise ValueError(f"q_scale / out_dtype apply to a float8_e4m3fn q only; q is {q.dtype}")
+        return None, QkvQuantArgs(TFA_FP8_E4M3, float(q8_scale), float(k_scale), float(v_scale)), q.dtype
     if q.dtype != torch.float8_e4m3fn:
         if q_scale != 1.0 or out_dtype not in (None, q.dtype):
             raise ValueError(f"q_scale / out_dtype apply to a float8_e4m3fn q only; q is {q.dtype}")
@@ -381,14 +397,18 @@ def _cache_dtype_code(q, qkv8, odt):
     return TFA_BF16 if odt == torch.bfloat16 else TFA_FP16
 
 
-def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream):
+def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream, need_q_rot=True):
     """The RotaryArgs of a cache call with q (its q_rot: a contiguous tensor of q's shape and dtype, or a buffer
-    allocated here and kept alive as the split workspace is), or None without rotary_cos."""
+    allocated here and kept alive as the split workspace is; none unless given when not `need_q_rot`), or None without
+    rotary_cos."""
     import torch
     if rotary_cos is None:
         return None
     assert rotary_sin is not None and rotary_cos.dim() == 2 and rotary_cos.shape == rotary_sin.shape
     assert rotary_cos.is_contiguous() and rotary_sin.is_contiguous()
+    if q_rot is None and not need_q_rot:
+        return RotaryArgs(rotary_cos.data_ptr(), rotary_sin.data_ptr(), rotary_cos.shape[0], 2 * rotary_cos.shape[1],
+                          int(bool(rotary_interleaved)), None)
     if q_rot is None:
         q_rot = torch.empty(q.shape, dtype=q.dtype, device=q.device)
         _WORKSPACES[("q_rot", q.device.index, int(stream))] = q_rot
@@ -397,10 +417,21 @@ def _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, stream):
                       int(bool(rotary_interleaved)), q_rot.data_ptr())
 
 
+def _q8_scratch(q, q8, stream):
+    """The e4m3 scratch a 16-bit q is quantized into: `q8`, a contiguous float8_e4m3fn tensor of q's shape, or a buffer
+    allocated here and kept alive as the split workspace is."""
+    import torch
+    if q8 is None:
+        q8 = torch.empty(q.shape, dtype=torch.float8_e4m3fn, device=q.device)
+        _WORKSPACES[("q8", q.device.index, int(stream))] = q8
+    assert q8.shape == q.shape and q8.dtype == torch.float8_e4m3fn and q8.is_contiguous()
+    return q8
+
+
 def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new=None, v_new=None, is_causal=False,
                      scale=None, num_splits=1, out_fp32=False, out=None, lse=None, stream=None, return_splits=False,
                      rotary_cos=None, rotary_sin=None, rotary_interleaved=False, q_rot=None, k_scale=1.0, v_scale=1.0,
-                     q_scale=1.0, out_dtype=None):
+                     q_scale=1.0, out_dtype=None, q8_scale=None, q8=None):
     """Attention against a KV cache through tfa_attn_kvcache_fwd(): q (B, Sq, Hq, D) with unit head_dim stride;
     k_cache / v_cache (num_blocks, page, Hkv, D) with a block_table (B, max_blocks_per_seq) int32, or (B, capacity,
     Hkv, D) with block_table None; cache_seqlens (B,) int32; optional k_new / v_new (B, Snew, Hkv, D) appended in
@@ -410,7 +441,9 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     that holds them after the call, or to a buffer allocated here.
     torch.float8_e4m3fn caches go through tfa_attn_kvcache_fp8_fwd() with the per-tensor k_scale / v_scale.  A
     torch.float8_e4m3fn q with them goes through tfa_attn_kvcache_qkv8_fwd() with q_scale too, the output (and k_new /
-    v_new) in out_dtype (bfloat16 or float16), without rotary.
+    v_new) in out_dtype (bfloat16 or float16), without rotary.  A 16-bit q with them and q8_scale goes through
+    tfa_attn_kvcache_qkv8_q16_fwd(): q (rotated with rotary_cos / rotary_sin) is quantized with q8_scale into `q8`, a
+    contiguous float8_e4m3fn tensor of q's shape that holds the codes after the call, or into a buffer allocated here.
     Returns out (q's shape and strides) and lse (B, Hq, Sq)."""
     import torch
     assert q.is_cuda and q.dim() == 4 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -418,7 +451,7 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     assert cache_seqlens.dtype == torch.int32
     B, Sq, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype)
+    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype, q8_scale)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 3)
     snew = k_new.shape[1] if k_new is not None else 0
     if scale is None:
@@ -437,8 +470,12 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
     dense = AttnArgs(None, None, None, None, None, B, Hq, Hkv, Sq, mbps * page, D, 0, 0, 0, 0, 0, 0, 0,
                      int(bool(is_causal)), 0.0, 0, int(num_splits), None, 0, None)
     n = _split_workspace(dense, a, q.device, st)
-    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
-    if qkv8 is not None:
+    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st, q8_scale is None)
+    if q8_scale is not None:
+        q8 = _q8_scratch(q, q8, st)
+        check(lib().tfa_attn_kvcache_qkv8_q16_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
+                                                  ctypes.byref(qkv8), q8.data_ptr()))
+    elif qkv8 is not None:
         check(lib().tfa_attn_kvcache_qkv8_fwd(ctypes.byref(a), ctypes.byref(qkv8)))
     elif quant is not None:
         check(lib().tfa_attn_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
@@ -455,7 +492,7 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
 def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
                             v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None,
                             k_scale=1.0, v_scale=1.0, rotary_cos=None, rotary_sin=None, rotary_interleaved=False,
-                            q_rot=None, q_scale=1.0, out_dtype=None):
+                            q_rot=None, q_scale=1.0, out_dtype=None, q8_scale=None, q8=None):
     """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
     (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
     and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
@@ -463,7 +500,8 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
     the per-tensor k_scale / v_scale.  rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) in q's dtype: rotate q and
     k_new first, through tfa_attn_varlen_kvcache_rotary_fwd() (with `quant` for an FP8 cache).  The rotated queries go
     to `q_rot`, a contiguous (total_q, Hq, D) tensor of q's dtype, or to a buffer allocated here.  A
-    torch.float8_e4m3fn q with an FP8 cache goes through tfa_attn_varlen_kvcache_qkv8_fwd() as attn_kvcache_fwd's.
+    torch.float8_e4m3fn q with an FP8 cache goes through tfa_attn_varlen_kvcache_qkv8_fwd() as attn_kvcache_fwd's, and
+    a 16-bit q with q8_scale through tfa_attn_varlen_kvcache_qkv8_q16_fwd() (`q8`: (total_q, Hq, D)) as its.
     Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
@@ -471,7 +509,7 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
     assert cu_q.dtype == torch.int32 and cu_q.numel() >= 2 and cache_seqlens.dtype == torch.int32
     total_q, Hq, D = q.shape
     nblk, page, Hkv, _ = k_cache.shape
-    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype)
+    quant, qkv8, odt = _cache_quant(q, k_cache, k_new, rotary_cos, q_scale, k_scale, v_scale, out_dtype, q8_scale)
     (mbps, bts, bt_ptr), nptr, vptr, ns = _cache_args(block_table, k_new, v_new, 2)
     if scale is None:
         scale = D ** -0.5
@@ -486,8 +524,12 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
                           k_cache.stride(0), k_cache.stride(1), k_cache.stride(2), bts, ns[0], ns[1],
                           _cache_dtype_code(q, qkv8, odt),
                           int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
-    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st)
-    if qkv8 is not None:
+    r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st, q8_scale is None)
+    if q8_scale is not None:
+        q8 = _q8_scratch(q, q8, st)
+        check(lib().tfa_attn_varlen_kvcache_qkv8_q16_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
+                                                         ctypes.byref(qkv8), q8.data_ptr()))
+    elif qkv8 is not None:
         check(lib().tfa_attn_varlen_kvcache_qkv8_fwd(ctypes.byref(a), ctypes.byref(qkv8)))
     elif r is not None:
         check(lib().tfa_attn_varlen_kvcache_rotary_fwd(ctypes.byref(a), ctypes.byref(r),
