@@ -42,6 +42,8 @@
 // kCacheQkv8 and kVarlenCacheQkv8 are kCache and kVarlenCache on that datapath: e4m3 queries against the e4m3 cache,
 // K read in place from its pages and V transposed by the converter, nothing widened.
 #pragma once
+#include <type_traits>
+
 #include "ptx_sm90.cuh"
 
 namespace tfa {
@@ -325,16 +327,18 @@ __device__ __forceinline__ void vt_convert_unit(uint32_t raw, uint32_t dst, int 
                  "r"(W[0]), "r"(W[1]), "r"(W[2]), "r"(W[3]) : "memory");
   }
 }
+// One 32-key k-step of P (s16: its 16 fp32 accumulator values) -> its 4 A registers, in fp8_p_key order.
+__device__ __forceinline__ void pack_p_e4m3_kstep(const float* s16, uint32_t* pf4) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    pf4[r] = pack_e4m3x4(s16[fp8_pack_src(r, 0)], s16[fp8_pack_src(r, 1)], s16[fp8_pack_src(r, 2)],
+                         s16[fp8_pack_src(r, 3)]);
+}
 // P (s[64], the fp32 accumulator layout of a 128-key tile) -> the A registers of its 4 k-steps of 32 keys, each
 // thread's own values in fp8_p_key order.
 __device__ __forceinline__ void pack_p_e4m3(const float* s, uint32_t* pf) {
 #pragma unroll
-  for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-      pf[4 * kk + r] = pack_e4m3x4(s[16 * kk + fp8_pack_src(r, 0)], s[16 * kk + fp8_pack_src(r, 1)],
-                                   s[16 * kk + fp8_pack_src(r, 2)], s[16 * kk + fp8_pack_src(r, 3)]);
-  }
+  for (int kk = 0; kk < 4; ++kk) pack_p_e4m3_kstep(s + 16 * kk, pf + 4 * kk);
 }
 
 // watchdog call sites
@@ -725,6 +729,16 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const uint32_t sQ_addr = smem_u32(sQ) + t * 64 * 128;   // this tile's rows inside each slab
   const uint32_t sKV_addr = smem_u32(sKV);
 
+  // Ping-pong: the two warpgroups take turns issuing their wgmmas.  Named barrier 3 + t is warpgroup t's turn:
+  // it syncs on it (128 threads) before issuing and, once issued, arrives (128 threads) on the other's.  Warpgroup 0
+  // goes first.  Both walk the same items with the same tile counts, so every sync meets one arrive; the arrive that
+  // lets warpgroup 0 go first stays pending at the CTA's end.  One warpgroup's whole batch (S_j and PV_{j-1}) thus
+  // reaches the tensor cores before the other's, and each runs its softmax under the other's batch.
+  const uint32_t turn_bar = 3 + t;          // 3 or 4 (ids 1 + t are the warpgroups' own barriers); the other's: ^ 7
+  auto turn_take = [&]() { named_bar_sync(turn_bar, 256); };
+  auto turn_pass = [&]() { named_bar_arrive(turn_bar ^ 7u, 256); };
+  if (t == 1) turn_pass();
+
   uint32_t ent = 0;        // K/V ring entry of K_0 of the current item (same sequence as the producer's)
   uint32_t qcnt = 0;
   for (int item = first; item < p.total_items; item += stride) {
@@ -810,7 +824,9 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
     float s[64];             // S tile: 16 column groups of 8 keys x {row_lo: [0],[1], row_hi: [2],[3]}
     float o[D / 2];          // O tile, same layout over D columns
-    uint32_t pf[DF8 ? 16 : 32];   // P as the A operand: 8 k-steps x 4 registers of 16-bit pairs (e4m3: 4 x 4 of e4m3x4)
+    // P as the A operand: 8 k-steps x 4 registers of 16-bit pairs (e4m3: 4 x 4 of e4m3x4), in two sets: while
+    // PV_{j-1} reads one, the softmax of tile j packs into the other (see the KV loop below)
+    uint32_t pfA[DF8 ? 16 : 32], pfB[DF8 ? 16 : 32];
     float m_lo = 0.f, m_hi = 0.f;     // reference max the exponentials are taken against (raw score units)
     float l_lo = 0.f, l_hi = 0.f;     // this thread's part of the running sum of exp2((s - m) * c)
     // Kahan compensation of l: minus the low-order part the adds into l have lost.  Each tile's 32 values are summed
@@ -821,80 +837,88 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
     for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
 
-    // mask + row max + lazy rescale decision + P = exp2(s*c - m*c) (fp32, in s) + row sums
+    // mask + row max + lazy rescale decision + P = exp2(s*c - m*c) + row sums of the scores sv (= s), P packed into
+    // the A registers pn.  The scores are only read: ptxas moves the PV wait above the first instruction that writes
+    // the S accumulator, and a non-wgmma write to the registers the in-flight PV reads serializes every wgmma (C7513).
+    // So each exponential goes from a temporary into the row sum and straight into pn, the set the in-flight PV does
+    // not read.  A masked score is -inf in the max and in the exponential alike (P = exp2(-inf) = 0), as if it had
+    // been written into s.  tests/test_sass_pv_overlap.py checks the compiled order.
     // returns alpha for (lo, hi) when O must be rescaled (rare), else {1, 1}
-    auto softmax = [&](int j, bool& rescale, float& a_lo, float& a_hi) {
+    auto softmax = [&](int j, const float* sv, bool& rescale, float& a_lo, float& a_hi, uint32_t* pn) {
       const int col0 = (w.jb + j) * C::BN;
       const bool edge = (col0 + C::BN > Sk) || (CAUSAL && col0 + C::BN - 1 > w.row0 + t * 64 + coff);
-      if (edge) {     // tiles crossing the causal diagonal or the end of the keys (warpgroup-uniform)
-        const int lim_lo = (CAUSAL ? min(Sk, row_lo + coff + 1) : Sk) - col0;
-        const int lim_hi = (CAUSAL ? min(Sk, row_hi + coff + 1) : Sk) - col0;
+      const int lim_lo = (CAUSAL ? min(Sk, row_lo + coff + 1) : Sk) - col0;
+      const int lim_hi = (CAUSAL ? min(Sk, row_hi + coff + 1) : Sk) - col0;
+      // EDGE: tiles crossing the causal diagonal or the end of the keys (warpgroup-uniform), one copy of the code each
+      auto tile = [&](auto edge_c) {
+        constexpr bool EDGE = decltype(edge_c)::value;
+        auto sc = [&](int k) {         // score k, masked
+          if constexpr (EDGE) {
+            const int col = 8 * (k >> 2) + 2 * tq + (k & 1);
+            return col >= ((k & 2) ? lim_hi : lim_lo) ? -INFINITY : sv[k];
+          } else {
+            return sv[k];
+          }
+        };
+        float mx_lo = -INFINITY, mx_hi = -INFINITY;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
+          mx_lo = fmaxf(mx_lo, fmaxf(sc(4 * i), sc(4 * i + 1)));
+          mx_hi = fmaxf(mx_hi, fmaxf(sc(4 * i + 2), sc(4 * i + 3)));
+        }
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = 8 * i + 2 * tq + e;
-            if (col >= lim_lo) s[4 * i + e] = -INFINITY;
-            if (col >= lim_hi) s[4 * i + 2 + e] = -INFINITY;
+        for (int d = 1; d <= 2; d <<= 1) {
+          mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, d));
+          mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, d));
+        }
+        a_lo = a_hi = 1.f;
+        rescale = false;
+        if (j == 0) {
+          m_lo = fmaxf(mx_lo, m_none);               // a row that sees no key yet (key-less, or masked in this split)
+          m_hi = fmaxf(mx_hi, m_none);
+        } else {
+          // lazy rescale of l and O: only when the row max moved by more than 2^8 (warp-uniform branch, rare)
+          const bool n_lo = (mx_lo - m_lo) * c > kRescaleThresholdLog2;
+          const bool n_hi = (mx_hi - m_hi) * c > kRescaleThresholdLog2;
+          if (__any_sync(0xffffffffu, n_lo || n_hi)) {
+            rescale = true;
+            if (n_lo) { a_lo = ex2_approx((m_lo - mx_lo) * c); m_lo = mx_lo; }
+            if (n_hi) { a_hi = ex2_approx((m_hi - mx_hi) * c); m_hi = mx_hi; }
+            l_lo *= a_lo; lc_lo *= a_lo;
+            l_hi *= a_hi; lc_hi *= a_hi;
           }
         }
-      }
-      float mx_lo = -INFINITY, mx_hi = -INFINITY;
+        const float nm_lo = -m_lo * c, nm_hi = -m_hi * c;
+        float t_lo = 0.f, t_hi = 0.f;             // this tile's part of l; l sums fp32 P, before the 16-bit rounding
+        // 32 keys at a time (one e4m3 k-step, two 16-bit ones); P -> A registers: 16-bit k-step kk = column groups
+        // 2kk, 2kk+1, so register r of the tile packs P values 2r, 2r+1
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        mx_lo = fmaxf(mx_lo, fmaxf(s[4 * i], s[4 * i + 1]));
-        mx_hi = fmaxf(mx_hi, fmaxf(s[4 * i + 2], s[4 * i + 3]));
-      }
+        for (int kb = 0; kb < 4; ++kb) {
+          float e[16];
 #pragma unroll
-      for (int d = 1; d <= 2; d <<= 1) {
-        mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, d));
-        mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, d));
-      }
-      a_lo = a_hi = 1.f;
-      rescale = false;
-      if (j == 0) {
-        m_lo = fmaxf(mx_lo, m_none);               // a row that sees no key yet (key-less, or masked in this split)
-        m_hi = fmaxf(mx_hi, m_none);
-      } else {
-        // lazy rescale of l and O: only when the row max moved by more than 2^8 (warp-uniform branch, rare)
-        const bool n_lo = (mx_lo - m_lo) * c > kRescaleThresholdLog2;
-        const bool n_hi = (mx_hi - m_hi) * c > kRescaleThresholdLog2;
-        if (__any_sync(0xffffffffu, n_lo || n_hi)) {
-          rescale = true;
-          if (n_lo) { a_lo = ex2_approx((m_lo - mx_lo) * c); m_lo = mx_lo; }
-          if (n_hi) { a_hi = ex2_approx((m_hi - mx_hi) * c); m_hi = mx_hi; }
-          l_lo *= a_lo; lc_lo *= a_lo;
-          l_hi *= a_hi; lc_hi *= a_hi;
+          for (int x = 0; x < 4; ++x) {
+            const int i = 4 * kb + x;
+            e[4 * x + 0] = ex2_approx(fmaf(sc(4 * i + 0), c, nm_lo));
+            e[4 * x + 1] = ex2_approx(fmaf(sc(4 * i + 1), c, nm_lo));
+            e[4 * x + 2] = ex2_approx(fmaf(sc(4 * i + 2), c, nm_hi));
+            e[4 * x + 3] = ex2_approx(fmaf(sc(4 * i + 3), c, nm_hi));
+            t_lo += e[4 * x + 0] + e[4 * x + 1];
+            t_hi += e[4 * x + 2] + e[4 * x + 3];
+          }
+          if constexpr (DF8) {      // P <= 2^8 < 448 (the lazy rescale's bound) is in e4m3 range
+            pack_p_e4m3_kstep(e, pn + 4 * kb);
+          } else {
+#pragma unroll
+            for (int r = 0; r < 8; ++r) pn[8 * kb + r] = pack_16x2<IS_BF16>(e[2 * r], e[2 * r + 1]);
+          }
         }
-      }
-      const float nm_lo = -m_lo * c, nm_hi = -m_hi * c;
-      float t_lo = 0.f, t_hi = 0.f;               // this tile's part of l; l sums fp32 P, before the 16-bit rounding
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        s[4 * i + 0] = ex2_approx(fmaf(s[4 * i + 0], c, nm_lo));
-        s[4 * i + 1] = ex2_approx(fmaf(s[4 * i + 1], c, nm_lo));
-        s[4 * i + 2] = ex2_approx(fmaf(s[4 * i + 2], c, nm_hi));
-        s[4 * i + 3] = ex2_approx(fmaf(s[4 * i + 3], c, nm_hi));
-        t_lo += s[4 * i + 0] + s[4 * i + 1];
-        t_hi += s[4 * i + 2] + s[4 * i + 3];
-      }
-      tp_lo = t_lo;
-      tp_hi = t_hi;
-    };
-    // P (fp32 accumulator layout) -> A-operand registers: k-step kk = column groups 2kk, 2kk+1
-    // kDenseFp8: P <= 2^8 < 448 (the lazy rescale's bound) is in e4m3 range
-    auto pack_P = [&]() {
-      if constexpr (DF8) {
-        pack_p_e4m3(s, pf);
-      } else {
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          pf[4 * kk + 0] = pack_16x2<IS_BF16>(s[8 * kk + 0], s[8 * kk + 1]);
-          pf[4 * kk + 1] = pack_16x2<IS_BF16>(s[8 * kk + 2], s[8 * kk + 3]);
-          pf[4 * kk + 2] = pack_16x2<IS_BF16>(s[8 * kk + 4], s[8 * kk + 5]);
-          pf[4 * kk + 3] = pack_16x2<IS_BF16>(s[8 * kk + 6], s[8 * kk + 7]);
-        }
-      }
+        tp_lo = t_lo;
+        tp_hi = t_hi;
+      };
+      // edge is warpgroup-uniform; the vote lets ptxas see that too.  In a branch it takes for divergent, it injects a
+      // warpgroup.arrive after the writes to pn and serializes every wgmma of the kernel (C7520).
+      if (__any_sync(0xffffffffu, edge)) tile(std::true_type{});
+      else tile(std::false_type{});
     };
 
     // An item without tiles waits on no barrier: its rows get O = 0 and LSE = +inf (a split-KV partial: LSE = -inf).
@@ -905,26 +929,30 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       {
         const uint32_t kslot = ent % NKR;
         mbar_wait(&kr_full[kslot], (ent / NKR) & 1, p.dbg, SITE_MMA_K, ent);
+        turn_take();
         wgmma_fence();
         issue_S(s, kslot);
+        turn_pass();
         wgmma_wait<0>();
         reg_fence(s);
         release(&kr_empty[kslot]);
         if (n == 1) release(q_empty);
         bool rs;
         float a0, a1;
-        softmax(0, rs, a0, a1);
-        pack_P();
+        softmax(0, s, rs, a0, a1, pfA);
       }
-      // ---- KV tiles 1 .. n-1: S_j and PV_{j-1} in flight together ----
-      for (int j = 1; j < n; ++j) {
+      // ---- KV tile j (1 <= j < n): S_j and PV_{j-1} in flight together; PV_{j-1} reads P_{j-1} from pc while the
+      // softmax of tile j runs under it and packs P_j into pn ----
+      auto step = [&](int j, const uint32_t* pc, uint32_t* pn) {
         const uint32_t ek = ent + KV_ENTS * j, ev = ent + KV_ENTS * j - 1;
         const uint32_t kslot = ek % NKR, vslot = ev % NVR;
         mbar_wait(&kr_full[kslot], (ek / NKR) & 1, p.dbg, SITE_MMA_K, ek);
+        turn_take();
         wgmma_fence();
         issue_S(s, kslot);
         mbar_wait(&vr_full[vslot], (ev / NVR) & 1, p.dbg, SITE_MMA_V, ev);
-        issue_PV(o, pf, vslot, j > 1);
+        issue_PV(o, pc, vslot, j > 1);
+        turn_pass();
         kahan_add(l_lo, lc_lo, tp_lo);                 // tile j - 1's partial, before softmax(j) may rescale l
         kahan_add(l_hi, lc_hi, tp_hi);
         wgmma_wait<1>();                               // S_j done
@@ -933,8 +961,8 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         if (j == n - 1) release(q_empty);
         bool rs;
         float a_lo, a_hi;
-        softmax(j, rs, a_lo, a_hi);
-        wgmma_wait<0>();                               // PV_{j-1} done: O and P registers are ours again
+        softmax(j, s, rs, a_lo, a_hi, pn);
+        wgmma_wait<0>();                               // PV_{j-1} done: O is ours again
         reg_fence(o);
         release(&vr_empty[vslot]);
         if (rs) {
@@ -944,19 +972,33 @@ fa_fwd_sm90_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             o[4 * i + 2] *= a_hi; o[4 * i + 3] *= a_hi;
           }
         }
-        pack_P();
-      }
-      {
+      };
+      // ---- the last tile's PV ----
+      auto last_pv = [&](const uint32_t* pc) {
         const uint32_t ev = ent + KV_ENTS * n - 1, vslot = ev % NVR;
         mbar_wait(&vr_full[vslot], (ev / NVR) & 1, p.dbg, SITE_MMA_V, ev);
         zero_v_tail(vslot, n - 1);
+        turn_take();
         wgmma_fence();
-        issue_PV(o, pf, vslot, n > 1);
+        issue_PV(o, pc, vslot, n > 1);
+        turn_pass();
         kahan_add(l_lo, lc_lo, tp_lo);
         kahan_add(l_hi, lc_hi, tp_hi);
         wgmma_wait<0>();
         reg_fence(o);
         release(&vr_empty[vslot]);
+      };
+      // unrolled by two, so that the sets swap roles without a copy: tile j's P is in pfA for even j, pfB for odd j
+      int j = 1;
+      for (; j + 1 < n; j += 2) {
+        step(j, pfA, pfB);
+        step(j + 1, pfB, pfA);
+      }
+      if (j < n) {
+        step(j, pfA, pfB);
+        last_pv(pfB);
+      } else {
+        last_pv(pfA);
       }
       ent += KV_ENTS * n;
     }

@@ -325,6 +325,10 @@ __device__ __forceinline__ uint32_t pack_e4m3x4(float a0, float a1, float a2, fl
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// arrive on named barrier `id` without waiting: the other side of a bar.sync of `nthreads`
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 template <uint32_t N>
 __device__ __forceinline__ void setmaxnreg_inc() {
