@@ -308,9 +308,9 @@ int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rot
  *              included) and do not change the result.
  * The host never reads cu_seqlens_q, cache_seqlens or block_table: the call (append included) can be captured in a
  * CUDA graph and replayed with new contents of the same total_q.  The kernels clamp every length and offset, so
- * malformed contents cannot make a store leave out, lse or a sequence's appended cache slots.  No split-KV (a
- * decode-only batch keeps tfa_attn_kvcache_fwd(), which has it).  Every argument is checked before any device work.
- * Launches: 1, + 1 with k_new. */
+ * malformed contents cannot make a store leave out, lse or a sequence's appended cache slots.  One pass over each
+ * sequence's keys; tfa_attn_varlen_kvcache_split_fwd() below adds split-KV.  Every argument is checked before any
+ * device work.  Launches: 1, + 1 with k_new. */
 typedef struct tfa_attn_varlen_kvcache_args {
   const void* q;
   void* k_cache;
@@ -360,7 +360,8 @@ int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args);
  * s' must stay a normal fp32 number with fp32(s' * log2 e) finite: when it overflows that, or when softmax_scale > 0
  * and it underflows below FLT_MIN (which would make the attention uniform), the call returns TFA_EINVAL_SCALE.
  * Every check runs before any device work, those of the 16-bit call first (TFA_EINVAL_KVQUANT after them).  Launches
- * and CUDA-graph capture as the 16-bit calls; split-KV as tfa_attn_kvcache_fwd() (the varlen call has none). */
+ * and CUDA-graph capture as the 16-bit calls; split-KV as tfa_attn_kvcache_fwd() (the varlen call through
+ * tfa_attn_varlen_kvcache_split_fwd()). */
 typedef struct tfa_kv_quant_args {
   int32_t cache_dtype;      /* TFA_FP8_E4M3 */
   float k_scale, v_scale;   /* finite, > 0 */
@@ -452,8 +453,8 @@ int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quan
  * tfa_attn_kvcache_qkv8_fwd and tfa_attn_varlen_kvcache_qkv8_fwd.  The problems of tfa_attn_kvcache_fwd() and
  * tfa_attn_varlen_kvcache_fwd(), unchanged -- lengths and the capacity clamp, the block table, dropped tokens, key-less
  * rows out = 0 / lse = +inf, slots past K_b holding any byte (NaN codes 0x7f / 0xff included) without changing the
- * result, nothing read back to the host (CUDA-graph capture), split-KV for the dense-query call only (num_splits /
- * workspace sized as for tfa_attn_kvcache_fwd()) -- with q and the caches holding one byte per element, and the
+ * result, nothing read back to the host (CUDA-graph capture), split-KV (num_splits / workspace sized as for
+ * tfa_attn_kvcache_fwd(); the varlen call through tfa_attn_varlen_kvcache_qkv8_split_fwd()) -- with q and the caches holding one byte per element, and the
  * arithmetic of tfa_attn_fp8_fwd().  tfa_attn_kvcache_fp8_fwd() widens every cache tile to q's 16-bit type; these calls
  * read q and K in place and only transpose V, so nothing is widened.
  *
@@ -506,8 +507,9 @@ int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, c
  *              q8, the same scales and args->dtype; out keeps q's element strides (dense-query call) or is (total_q,
  *              Hq, D) contiguous (varlen call).  The pools are bit-identical to tfa_attn_kvcache_fp8_fwd()'s /
  *              tfa_attn_varlen_kvcache_rotary_fwd()'s with the same rotary (tfa_attn_varlen_kvcache_fp8_fwd()'s
- *              without it).  Lengths, the capacity clamp, dropped tokens, key-less rows, split-KV (dense-query call
- *              only) and CUDA-graph capture are those of the e4m3-query calls.
+ *              without it).  Lengths, the capacity clamp, dropped tokens, key-less rows, split-KV (the varlen call
+ *              through tfa_attn_varlen_kvcache_qkv8_split_fwd()) and CUDA-graph capture are those of the e4m3-query
+ *              calls.
  * Every check runs before any device work, in this order: a NULL args or quant, or a NULL or misaligned q8
  * (TFA_EINVAL_PTR); the cache arguments (TFA_EINVAL_KVCACHE); the shapes, strides, dtype and scale of the 16-bit call;
  * (varlen) cu_seqlens_q / max_seqlen_q (TFA_EINVAL_SEQLENS); the rotary arguments but q_rot (TFA_EINVAL_ROTARY); the
@@ -518,6 +520,60 @@ int tfa_attn_kvcache_qkv8_q16_fwd(const tfa_attn_kvcache_args* args, const tfa_r
 int tfa_attn_varlen_kvcache_qkv8_q16_fwd(const tfa_attn_varlen_kvcache_args* args,
                                          const tfa_rotary_args* rotary /* NULL: none */,
                                          const tfa_qkv_quant_args* quant, void* q8);
+
+/* ---- split-KV for the variable-length KV-cache calls: the long decodes of a mixed prefill / decode batch spread over
+ * the GPU ----
+ * Added without an ABI version change (TFA_ABI_VERSION stays 2): callers detect them by the exported symbols
+ * tfa_attn_varlen_kvcache_split_fwd, tfa_attn_varlen_kvcache_qkv8_split_fwd, tfa_attn_varlen_kvcache_num_splits and
+ * tfa_attn_varlen_kvcache_workspace_bytes.  Each key range is cut into splits run by independent CTAs; their fp32
+ * partials go to `workspace` and one more kernel merges them through their LSEs (as tfa_attn_kvcache_fwd() does).
+ *
+ *   tfa_attn_varlen_kvcache_split_fwd  : tfa_attn_varlen_kvcache_fwd() (rotary NULL, quant NULL),
+ *              tfa_attn_varlen_kvcache_fp8_fwd() (rotary NULL, quant given) or tfa_attn_varlen_kvcache_rotary_fwd()
+ *              (rotary given, quant NULL-able), with split-KV.
+ *   tfa_attn_varlen_kvcache_qkv8_split_fwd : tfa_attn_varlen_kvcache_qkv8_fwd() (q8 NULL: q is e4m3; rotary must be NULL,
+ *              TFA_EINVAL_ROTARY otherwise) or tfa_attn_varlen_kvcache_qkv8_q16_fwd() (q8 given, 16-byte aligned), with
+ *              split-KV.
+ *   split rule : the split count is tfa_attn_num_splits() of the dense problem (B, Hq, Sq = max_seqlen_q, Sk = capacity,
+ *              is_causal) with num_splits; tfa_attn_varlen_kvcache_num_splits() gives it without a device (0 = auto then
+ *              gives 1 when the SM count is unknown).  Every sequence's keys are cut at the same places: split s covers
+ *              KV tiles [s t, (s + 1) t) with t = ceil(ceil(capacity / 128) / nsplit), so a sequence with few keys fills
+ *              only its first splits.  The host never reads a length.
+ *   workspace : nsplit * Hq * total_q * (D + 1) * 4 bytes (tfa_attn_varlen_kvcache_workspace_bytes(); 0 for nsplit 1):
+ *              packed fp32 partials (nsplit, Hq, total_q, D), then their LSEs (nsplit, Hq, total_q).  Its contents
+ *              before the call do not matter.  Under num_splits = 0 a NULL, small or misaligned workspace means one
+ *              pass; an explicit num_splits > 1 without a usable one returns TFA_EINVAL_WORKSPACE before the append, so
+ *              the cache is left untouched.
+ *   result   : when the count resolves to 1, out, lse and the pools are bit-identical to the call without split, with
+ *              the same launches.  Otherwise each sequence's out and lse are bit-identical to the dense-query cache call
+ *              (tfa_attn_kvcache_fwd() / _fp8_fwd() / _rotary_fwd() / _qkv8_fwd() / _qkv8_q16_fwd()) on that sequence
+ *              alone with Sq = Snew = n_b, the same capacity, table row, scales, rotary and num_splits.  Rows beyond a
+ *              sequence's first max_seqlen_q and rows in no sequence keep what out and lse held.  Whatever
+ *              cu_seqlens_q, cache_seqlens and the table hold, no store leaves out, lse, the workspace or the appended
+ *              slots.
+ * Every check runs before any device work: a NULL args or split (and for the qkv8 call a NULL quant or misaligned
+ * q8) is TFA_EINVAL_PTR; then the checks of the call without split, in its order, with num_splits < 0 reported as
+ * TFA_EINVAL_SHAPE among the shape checks; the workspace (TFA_EINVAL_WORKSPACE) comes after TFA_EARCH.  Launches:
+ * those of the call without split, + 1 when it splits.  Nothing is read back to the host: with a caller-owned
+ * workspace the call can be captured in a CUDA graph and replayed with new contents of the same total_q. */
+typedef struct tfa_split_args {
+  int32_t num_splits;       /* 1 = one pass, n > 1 = as asked (clamped so no split is empty), 0 = library decides */
+  void* workspace;          /* device, 16-byte aligned; may be NULL when num_splits resolves to 1 */
+  size_t workspace_bytes;
+} tfa_split_args;
+
+int tfa_attn_varlen_kvcache_split_fwd(const tfa_attn_varlen_kvcache_args* args,
+                                      const tfa_rotary_args* rotary /* NULL: none */,
+                                      const tfa_kv_quant_args* quant /* NULL: 16-bit cache */,
+                                      const tfa_split_args* split);
+int tfa_attn_varlen_kvcache_qkv8_split_fwd(const tfa_attn_varlen_kvcache_args* args,
+                                           const tfa_rotary_args* rotary /* NULL: none */,
+                                           const tfa_qkv_quant_args* quant, void* q8 /* NULL: q is e4m3 */,
+                                           const tfa_split_args* split);
+/* The split count the calls above use for `num_splits` (resolves 0 = auto, clamps n), >= 1. */
+int tfa_attn_varlen_kvcache_num_splits(const tfa_attn_varlen_kvcache_args* args, int num_splits);
+/* Workspace needed for `num_splits` (as returned above): num_splits * Hq * total_q * (D + 1) * 4 bytes; 0 for 1. */
+size_t tfa_attn_varlen_kvcache_workspace_bytes(const tfa_attn_varlen_kvcache_args* args, int num_splits);
 
 /* Host-buffer forward: q/k/v/out/lse are HOST pointers ((B,H,S,D) contiguous; pinned
  * memory gives full PCIe speed).  Copies in, runs tfa_fwd per (batch*head) chunk on

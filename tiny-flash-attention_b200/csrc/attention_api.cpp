@@ -590,8 +590,25 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_fp8(
 // block_table and seqused_k): q (total_q, Hq, D) with cu_seqlens_q int32 (B + 1) offsets as flash_attention_v2_varlen;
 // k_cache / v_cache / block_table / cache_seqlens as flash_attention_v2_kvcache; k_new / v_new None or packed
 // (total_q, Hkv, D) sharing cu_seqlens_q, written into the cache in place at keys [cache_seqlens[b], + the sequence's
-// query rows) before the attention.  Returns out (total_q, Hq, D) and lse (Hq, total_q).  No split-KV.
+// query rows) before the attention.  Returns out (total_q, Hq, D) and lse (Hq, total_q).  num_splits as
+// flash_attention_v2_kvcache, for the dense problem of max_seqlen_q rows per sequence
+// (tfa_attn_varlen_kvcache_split_fwd).
 namespace {
+
+// Split-KV of a variable-length cache call: asks the library for the split count and, when it splits, allocates the
+// workspace on q's device and sets `s`.  Returns the workspace (undefined for one pass), as split_workspace.
+torch::Tensor varlen_split_workspace(const tfa_attn_varlen_kvcache_args& a, int64_t num_splits, tfa_split_args& s,
+                                     const torch::Tensor& q) {
+  torch::Tensor ws;
+  s = tfa_split_args{1, nullptr, 0};
+  const int nsplit = tfa_attn_varlen_kvcache_num_splits(&a, static_cast<int>(num_splits));
+  if (nsplit > 1) {
+    const size_t need = tfa_attn_varlen_kvcache_workspace_bytes(&a, nsplit);
+    ws = torch::empty({static_cast<int64_t>((need + 3) / 4)}, q.options().dtype(at::kFloat));
+    s = tfa_split_args{nsplit, ws.data_ptr(), need};
+  }
+  return ws;
+}
 
 // flash_attention_v2_varlen_kvcache, or with `quant` its FP8-cache form; with rotary_cos / rotary_sin, q and k_new
 // are rotated first (tfa_attn_varlen_kvcache_rotary_fwd) through a q_rot allocated here.  `qkv8`: the e4m3-query form,
@@ -604,7 +621,8 @@ std::vector<torch::Tensor> varlen_kvcache(
     const std::optional<torch::Tensor>& v_new, bool is_causal, float softmax_scale, const tfa_kv_quant_args* quant,
     const std::optional<torch::Tensor>& rotary_cos = std::nullopt,
     const std::optional<torch::Tensor>& rotary_sin = std::nullopt, bool rotary_interleaved = false,
-    const tfa_qkv_quant_args* qkv8 = nullptr, at::ScalarType out_dtype = at::kBFloat16, bool q16 = false) {
+    const tfa_qkv_quant_args* qkv8 = nullptr, at::ScalarType out_dtype = at::kBFloat16, bool q16 = false,
+    int64_t num_splits = 1) {
   TFA_CHECK_CUDA(q);
   TORCH_CHECK(q.dim() == 3, "q must have 3 dimensions (total_q, heads, head_dim)");
   TORCH_CHECK(cu_seqlens_q.scalar_type() == at::kInt, "cu_seqlens_q must be int32");
@@ -635,11 +653,12 @@ std::vector<torch::Tensor> varlen_kvcache(
                   mbps < (1LL << 31),
               "tensors too large");
   TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value(), "rotary_cos and rotary_sin must be given together");
+  TORCH_CHECK(num_splits >= 0 && num_splits <= 1024, "num_splits must be in [0, 1024]");
   tfa_rotary_args r;
   if (rotary_cos.has_value())
     r = check_rotary(q, D, mbps * page, k_new.has_value(), *rotary_cos, *rotary_sin, rotary_interleaved);
 
-  torch::Tensor out, lse, q_rot, q8;
+  torch::Tensor out, lse, q_rot, q8, ws;
   int rc = 0;
   {
     c10::cuda::CUDAGuard guard(q.device());
@@ -669,17 +688,19 @@ std::vector<torch::Tensor> varlen_kvcache(
     a.softmax_scale = softmax_scale;
     a.out_fp32 = 0;
     a.stream = at::cuda::getCurrentCUDAStream(q.device().index()).stream();
+    tfa_split_args sp;
+    ws = varlen_split_workspace(a, num_splits, sp, q);
     if (q16) {
       q8 = torch::empty({total_q, Hq, D}, q.options().dtype(at::kFloat8_e4m3fn));
-      rc = tfa_attn_varlen_kvcache_qkv8_q16_fwd(&a, rotary_cos.has_value() ? &r : nullptr, qkv8, q8.data_ptr());
+      rc = tfa_attn_varlen_kvcache_qkv8_split_fwd(&a, rotary_cos.has_value() ? &r : nullptr, qkv8, q8.data_ptr(), &sp);
     } else if (qkv8) {
-      rc = tfa_attn_varlen_kvcache_qkv8_fwd(&a, qkv8);
-    } else if (rotary_cos.has_value()) {
-      q_rot = torch::empty({total_q, Hq, D}, q.options().memory_format(at::MemoryFormat::Contiguous));
-      r.q_rot = q_rot.data_ptr();
-      rc = tfa_attn_varlen_kvcache_rotary_fwd(&a, &r, quant);
+      rc = tfa_attn_varlen_kvcache_qkv8_split_fwd(&a, nullptr, qkv8, nullptr, &sp);
     } else {
-      rc = quant ? tfa_attn_varlen_kvcache_fp8_fwd(&a, quant) : tfa_attn_varlen_kvcache_fwd(&a);
+      if (rotary_cos.has_value()) {
+        q_rot = torch::empty({total_q, Hq, D}, q.options().memory_format(at::MemoryFormat::Contiguous));
+        r.q_rot = q_rot.data_ptr();
+      }
+      rc = tfa_attn_varlen_kvcache_split_fwd(&a, rotary_cos.has_value() ? &r : nullptr, quant, &sp);
     }
   }
   raise_on_error(rc);
@@ -691,9 +712,10 @@ std::vector<torch::Tensor> varlen_kvcache(
 std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
-    std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale) {
+    std::optional<torch::Tensor> v_new, bool is_causal, float softmax_scale, int64_t num_splits) {
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
-                        is_causal, softmax_scale, nullptr);
+                        is_causal, softmax_scale, nullptr, std::nullopt, std::nullopt, false, nullptr, at::kBFloat16,
+                        false, num_splits);
 }
 
 // The same with rotary position embedding: q and k_new are rotated at each sequence's cache positions
@@ -703,9 +725,10 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_rotary(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
     std::optional<torch::Tensor> v_new, torch::Tensor rotary_cos, torch::Tensor rotary_sin, bool rotary_interleaved,
-    bool is_causal, float softmax_scale) {
+    bool is_causal, float softmax_scale, int64_t num_splits) {
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
-                        is_causal, softmax_scale, nullptr, rotary_cos, rotary_sin, rotary_interleaved);
+                        is_causal, softmax_scale, nullptr, rotary_cos, rotary_sin, rotary_interleaved, nullptr,
+                        at::kBFloat16, false, num_splits);
 }
 
 // The same against an FP8 cache (float8_e4m3fn k_cache / v_cache with per-tensor k_scale / v_scale), as
@@ -714,10 +737,12 @@ std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_fp8(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
     std::optional<torch::Tensor> v_new, double k_scale, double v_scale, bool is_causal, float softmax_scale,
-    std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin, bool rotary_interleaved) {
+    std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin, bool rotary_interleaved,
+    int64_t num_splits) {
   const tfa_kv_quant_args qa = check_quant(k_scale, v_scale);
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
-                        is_causal, softmax_scale, &qa, rotary_cos, rotary_sin, rotary_interleaved);
+                        is_causal, softmax_scale, &qa, rotary_cos, rotary_sin, rotary_interleaved, nullptr,
+                        at::kBFloat16, false, num_splits);
 }
 
 namespace {
@@ -750,15 +775,16 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_qkv8(
 
 // The packed variable-length form: q (total_q, Hq, D) float8_e4m3fn with cu_seqlens_q as
 // flash_attention_v2_varlen_kvcache; the rest as flash_attention_v2_kvcache_qkv8.  Returns out (total_q, Hq, D) in
-// out_dtype and lse (Hq, total_q).  No split-KV.
+// out_dtype and lse (Hq, total_q).  num_splits as flash_attention_v2_varlen_kvcache.
 std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_qkv8(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
     std::optional<torch::Tensor> v_new, double q_scale, double k_scale, double v_scale, bool is_causal,
-    float softmax_scale, at::ScalarType out_dtype) {
+    float softmax_scale, at::ScalarType out_dtype, int64_t num_splits) {
   const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
-                        is_causal, softmax_scale, nullptr, std::nullopt, std::nullopt, false, &qa, out_dtype);
+                        is_causal, softmax_scale, nullptr, std::nullopt, std::nullopt, false, &qa, out_dtype, false,
+                        num_splits);
 }
 
 // The e4m3-query cache call fed from a 16-bit q (tfa_attn_kvcache_qkv8_q16_fwd in include/tfa_b200.h): q (B, Sq, Hq, D)
@@ -782,17 +808,17 @@ std::vector<torch::Tensor> flash_attention_v2_kvcache_qkv8_q16(
 
 // The packed variable-length form: q (total_q, Hq, D) bfloat16 / float16 with cu_seqlens_q as
 // flash_attention_v2_varlen_kvcache; the rest as flash_attention_v2_kvcache_qkv8_q16.  Returns out (total_q, Hq, D) in
-// q's dtype and lse (Hq, total_q).  No split-KV.
+// q's dtype and lse (Hq, total_q).  num_splits as flash_attention_v2_varlen_kvcache.
 std::vector<torch::Tensor> flash_attention_v2_varlen_kvcache_qkv8_q16(
     torch::Tensor q, torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor cu_seqlens_q, int64_t max_seqlen_q,
     torch::Tensor cache_seqlens, std::optional<torch::Tensor> block_table, std::optional<torch::Tensor> k_new,
     std::optional<torch::Tensor> v_new, double q_scale, double k_scale, double v_scale, bool is_causal,
     float softmax_scale, std::optional<torch::Tensor> rotary_cos, std::optional<torch::Tensor> rotary_sin,
-    bool rotary_interleaved) {
+    bool rotary_interleaved, int64_t num_splits) {
   const tfa_qkv_quant_args qa = check_qkv8_quant(q_scale, k_scale, v_scale);
   return varlen_kvcache(q, k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new,
                         is_causal, softmax_scale, nullptr, rotary_cos, rotary_sin, rotary_interleaved, &qa,
-                        q.scalar_type(), true);
+                        q.scalar_type(), true, num_splits);
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -825,7 +851,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "num_splits)");
   m.def("flash_attention_v2_varlen_kvcache", &flash_attention_v2_varlen_kvcache,
         "a packed variable-length batch of queries against a (paged) KV cache with an optional in-place append: (q, "
-        "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, is_causal, scale)");
+        "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, is_causal, scale), "
+        "optional split-KV (num_splits)",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
+        py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("is_causal"),
+        py::arg("softmax_scale"), py::arg("num_splits") = 1);
   m.def("flash_attention_v2_kvcache_fp8", &flash_attention_v2_kvcache_fp8,
         "the KV-cache forward against an FP8 (float8_e4m3fn) cache with per-tensor scales, k_new / v_new quantized on "
         "append, optional rotary",
@@ -840,11 +870,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
         py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("k_scale"),
         py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("rotary_cos") = py::none(),
-        py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
+        py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false, py::arg("num_splits") = 1);
   m.def("flash_attention_v2_varlen_kvcache_rotary", &flash_attention_v2_varlen_kvcache_rotary,
         "the variable-length KV-cache call with q and k_new rotated (RoPE) at each sequence's cache positions: (q, "
         "k_cache, v_cache, cu_seqlens_q, max_seqlen_q, cache_seqlens, block_table, k_new, v_new, rotary_cos, "
-        "rotary_sin, rotary_interleaved, is_causal, scale)");
+        "rotary_sin, rotary_interleaved, is_causal, scale), optional split-KV (num_splits)",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
+        py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("rotary_cos"),
+        py::arg("rotary_sin"), py::arg("rotary_interleaved"), py::arg("is_causal"), py::arg("softmax_scale"),
+        py::arg("num_splits") = 1);
   m.def("flash_attention_v2_kvcache_qkv8", &flash_attention_v2_kvcache_qkv8,
         "float8_e4m3fn q against an FP8 (float8_e4m3fn) cache with per-tensor scales, both products on e4m3 tensor "
         "cores, k_new / v_new (out_dtype) quantized on append -> [out (out_dtype), lse]",
@@ -856,7 +890,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         "on e4m3 tensor cores -> [out (out_dtype), lse]",
         py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
         py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"),
-        py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"));
+        py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"), py::arg("out_dtype"),
+        py::arg("num_splits") = 1);
   m.def("flash_attention_v2_kvcache_qkv8_q16", &flash_attention_v2_kvcache_qkv8_q16,
         "bfloat16 / float16 q, optionally rotated (RoPE), quantized to e4m3 in the append's launch and run against an "
         "FP8 (float8_e4m3fn) cache on e4m3 tensor cores -> [out (q's dtype), lse]",
@@ -871,7 +906,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cu_seqlens_q"), py::arg("max_seqlen_q"),
         py::arg("cache_seqlens"), py::arg("block_table"), py::arg("k_new"), py::arg("v_new"), py::arg("q_scale"),
         py::arg("k_scale"), py::arg("v_scale"), py::arg("is_causal"), py::arg("softmax_scale"),
-        py::arg("rotary_cos") = py::none(), py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false);
+        py::arg("rotary_cos") = py::none(), py::arg("rotary_sin") = py::none(), py::arg("rotary_interleaved") = false,
+        py::arg("num_splits") = 1);
   m.def("launch_count",[]() { return tfa_launch_count(); }, "kernels launched by the library so far");
   m.def("abi_version", []() { return tfa_abi_version(); });
 }

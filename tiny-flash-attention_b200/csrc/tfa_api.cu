@@ -215,6 +215,7 @@ struct Problem {
   void* ws;
   size_t ws_bytes;
   cudaStream_t stream;
+  bool packed;                              // q / out / lse are packed rows: one batch entry of Sq = total_q rows
 };
 
 // The kernels take exponents in log2 units, c = fp32(scale * log2 e): a scale >= 0 is accepted while c is finite,
@@ -243,12 +244,12 @@ int validate(const Problem& a) {
 // one.  The split count and the schedule are chosen for these rows: the items of the others load nothing.
 int keyed_rows(bool causal, int Sq, int Sk) { return (causal && Sk < Sq) ? Sk : Sq; }
 
-// Split-KV decision.  `want` 0 = auto: split only when the plain grid would leave more than half of the SMs idle,
-// into as many splits as still fit one wave of CTAs (one CTA more than the SMs would double the time), each with
-// >= 4 KV tiles;
+// Split-KV decision for the dense problem of S query rows per (batch, head) (a.Sq, or a packed call's max_seqlen_q).
+// `want` 0 = auto: split only when the plain grid would leave more than half of the SMs idle, into as many splits as
+// still fit one wave of CTAs (one CTA more than the SMs would double the time), each with >= 4 KV tiles;
 // n > 1 = as asked, clamped so that no split is empty.
-int resolve_splits(const Problem& a, int want, int sms) {
-  const long long items = ((static_cast<long long>(keyed_rows(a.causal != 0, a.Sq, a.Sk)) + 127) / 128) * a.B * a.Hq;
+int resolve_splits(const Problem& a, int S, int want, int sms) {
+  const long long items = ((static_cast<long long>(keyed_rows(a.causal != 0, S, a.Sk)) + 127) / 128) * a.B * a.Hq;
   const int nkv = (a.Sk + 127) / 128;
   int n = want;
   if (n == 0) {
@@ -264,10 +265,12 @@ int resolve_splits(const Problem& a, int want, int sms) {
 }
 
 // Split-KV workspace: `nsplit` normalised fp32 partials of the (B, Hq, S, D) output, then their nsplit (B, Hq, S)
-// LSEs (set_output partitions it).  Every split writes the LSEs of all Sq rows.
+// LSEs (set_output partitions it); packed, (Hq, total_q, D) partials and (Hq, total_q) LSEs.  Every split writes the
+// LSEs of all rows it computes.
 size_t splitkv_ws_bytes(const Problem& a, int nsplit) {
   if (nsplit <= 1) return 0;
-  return static_cast<size_t>(nsplit) * a.B * a.Hq * a.Sq * (static_cast<size_t>(a.D) + 1) * sizeof(float);
+  return static_cast<size_t>(nsplit) * (a.packed ? 1 : a.B) * a.Hq * a.Sq * (static_cast<size_t>(a.D) + 1) *
+         sizeof(float);
 }
 
 struct SplitPlan {
@@ -275,10 +278,10 @@ struct SplitPlan {
   int split_tiles;   // KV tiles per split
 };
 
-// The split count of a dense or cache call.  Under auto (num_splits == 0) a missing, small or misaligned workspace
-// means one pass; an asked-for count without its workspace is an error.
-int plan_splits(const Problem& a, SplitPlan& plan) {
-  int nsplit = resolve_splits(a, a.num_splits, num_sms());
+// The split count of a cache or dense call over S query rows per (batch, head).  Under auto (num_splits == 0) a
+// missing, small or misaligned workspace means one pass; an asked-for count without its workspace is an error.
+int plan_splits(const Problem& a, int S, SplitPlan& plan) {
+  int nsplit = resolve_splits(a, S, a.num_splits, num_sms());
   if (nsplit > 1) {
     const size_t need = splitkv_ws_bytes(a, nsplit);
     const bool ws_ok = a.ws != nullptr && !(reinterpret_cast<uintptr_t>(a.ws) & 15u) && a.ws_bytes >= need;
@@ -294,16 +297,18 @@ int plan_splits(const Problem& a, SplitPlan& plan) {
 }
 
 // Where the forward over S query rows per (batch, head) writes: the caller's out / lse in one pass; with split-KV,
-// contiguous (B, Hq, S, D) fp32 partials per split with their LSEs, which the combine merges into out / lse.
+// contiguous (B, Hq, S, D) fp32 partials per split with their LSEs, which the combine merges into out / lse.  Packed:
+// (Hq, total_q, D) partials, each sequence's rows at their packed offsets (the forward's ol.o(b, h, q0 + row)).
 void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
   if (nsplit > 1) {
-    const long long rows = static_cast<long long>(a.B) * a.Hq * S;
+    const long long per_b = a.packed ? 0 : static_cast<long long>(a.Hq) * S;   // partial rows between batch entries
+    const long long per_h = a.packed ? a.Sq : S;                                // between heads
+    const long long rows = a.packed ? static_cast<long long>(a.Hq) * a.Sq : a.B * per_b;
     float* ws_o = static_cast<float*>(a.ws);
     p.out = nullptr;
     p.out_f32 = ws_o;
     p.lse = ws_o + static_cast<size_t>(nsplit) * rows * a.D;
-    p.ol = {static_cast<long long>(a.Hq) * S * a.D, static_cast<long long>(S) * a.D, a.D,
-            static_cast<long long>(a.Hq) * S, S};
+    p.ol = {per_b * a.D, per_h * a.D, a.D, per_b, per_h};
     p.part_stride = rows * a.D;
     p.lse_part_stride = rows;
   } else {
@@ -318,10 +323,11 @@ void set_output(FwdParams& p, const Problem& a, int S, int nsplit) {
 }
 
 // the combine kernel takes D / 4 threads per row
-template <int D>
+template <int D, bool PACKED>
 int launch_combine(const tfa::CombineParams& cp, bool bf16, bool f32, cudaStream_t stream) {
-  auto kern = f32 ? tfa::splitkv_combine_kernel<D, true, true>
-                  : bf16 ? tfa::splitkv_combine_kernel<D, true, false> : tfa::splitkv_combine_kernel<D, false, false>;
+  auto kern = f32 ? tfa::splitkv_combine_kernel<D, true, true, PACKED>
+                  : bf16 ? tfa::splitkv_combine_kernel<D, true, false, PACKED>
+                         : tfa::splitkv_combine_kernel<D, false, false, PACKED>;
   return launch_small(kern, cp.rows, 256 / (D / 4), cp, stream);
 }
 
@@ -365,10 +371,20 @@ int run_forward(const Problem& a, FwdParams p, int S, const CUtensorMap& tq, con
   cp.out = a.out;
   cp.lse = a.lse;
   cp.ol = a.ol;
-  cp.rows = static_cast<long long>(a.B) * a.Hq * S;
-  cp.H = a.Hq; cp.S = S;
   cp.nsplit = plan.nsplit;
-  return (a.D == 64) ? launch_combine<64>(cp, bf16, f32, a.stream) : launch_combine<128>(cp, bf16, f32, a.stream);
+  cp.H = a.Hq;
+  if (a.packed) {         // one row per packed row of every head; a row outside its sequence's first S is not stored
+    cp.rows = static_cast<long long>(a.Hq) * a.Sq;
+    cp.S = a.Sq;
+    cp.cu_q = p.cu_q; cp.B = a.B; cp.max_seqlen_q = S;
+    return (a.D == 64) ? launch_combine<64, true>(cp, bf16, f32, a.stream)
+                       : launch_combine<128, true>(cp, bf16, f32, a.stream);
+  }
+  cp.rows = static_cast<long long>(a.B) * a.Hq * S;
+  cp.S = S;
+  cp.cu_q = nullptr; cp.B = a.B; cp.max_seqlen_q = S;
+  return (a.D == 64) ? launch_combine<64, false>(cp, bf16, f32, a.stream)
+                     : launch_combine<128, false>(cp, bf16, f32, a.stream);
 }
 
 // The effective softmax scale s' of an FP8 call, as the caller rounds it from softmax_scale and the quantization scales,
@@ -416,7 +432,7 @@ int fwd_impl(Problem a, const tfa_qkv_quant_args* quant, void* const* extra_dst 
   }
 
   SplitPlan plan;
-  if ((rc = plan_splits(a, plan))) return rc;
+  if ((rc = plan_splits(a, a.Sq, plan))) return rc;
 
   FwdParams p{};
   p.Sk = a.Sk;
@@ -445,6 +461,7 @@ Problem from_fwd_args(const tfa_fwd_args& a) {
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = false;
   return q;
 }
 
@@ -458,6 +475,7 @@ Problem from_attn_args(const tfa_attn_args& a) {
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = false;
   return q;
 }
 
@@ -472,6 +490,7 @@ Problem from_varlen_args(const tfa_attn_varlen_args& a) {
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = true;
   return q;
 }
 
@@ -528,6 +547,7 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = a.num_splits; q.ws = a.workspace; q.ws_bytes = a.workspace_bytes;
   q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = false;
   return q;
 }
 
@@ -664,7 +684,7 @@ int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, con
   const int snew = ka.k_new ? ka.Snew : 0;
 
   SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
-  if ((rc = plan_splits(a, plan))) return rc;
+  if ((rc = plan_splits(a, a.Sq, plan))) return rc;
 
   // qkv8: the 8-bit swizzled Q and K maps the wgmma reads in place, as fwd_impl builds them
   const bool fp8_cache = quant || qkv8;
@@ -708,14 +728,20 @@ Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
   q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
   q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
   q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = true;
   return q;
 }
 
 // `ra`, `quant`, `qkv8` and `q8` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and
-// the forward reads its queries from ra->q_rot (from q8 with `q8`).
+// the forward reads its queries from ra->q_rot (from q8 with `q8`).  `split` nullptr: one pass.  Otherwise split-KV as
+// kvcache_impl plans it for the dense problem of max_seqlen_q rows per sequence, into packed partials.
 int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* ra,
-                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr) {
+                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr,
+                        const tfa_split_args* split = nullptr) {
   Problem a = from_varlen_kvcache_args(va);
+  if (split) {
+    a.num_splits = split->num_splits; a.ws = split->workspace; a.ws_bytes = split->workspace_bytes;
+  }
   int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
   if (rc) return rc;
   if ((rc = validate(a))) return rc;
@@ -733,6 +759,9 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
   }
   if (!arch_ok()) return TFA_EARCH;
   init_dbg();
+
+  SplitPlan plan;                       // before the append, as kvcache_impl
+  if ((rc = plan_splits(a, va.max_seqlen_q, plan))) return rc;
 
   const bool fp8_cache = quant || qkv8;
   CUtensorMap tq, tk, tv;
@@ -754,16 +783,17 @@ int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary
   p.cu_q = va.cu_seqlens_q;
   p.total_q = a.Sq;
   p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
-  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head), one split holds every KV tile
+  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head); every split covers the same KV tiles of
+  // every sequence, so a sequence with few keys fills only its first splits
   if (qkv8) {
     p.v_scale = qs.v_scale;
-    return run_forward<tfa::kVarlenCacheQkv8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+    return run_forward<tfa::kVarlenCacheQkv8>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
   }
   if (quant) {
     p.v_scale = qs.v_scale;
-    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
   }
-  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, SplitPlan{1, 0x7fffffff});
+  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
 }
 
 // ---- host-buffer path workspace ----
@@ -875,12 +905,38 @@ int tfa_attn_num_splits(const tfa_attn_args* args) {
   if (!args) return 1;
   const Problem a = from_attn_args(*args);
   if (a.B < 1 || a.Hq < 1 || a.Sq < 1 || a.Sk < 1 || a.num_splits < 0) return 1;
-  return resolve_splits(a, a.num_splits, num_sms());
+  return resolve_splits(a, a.Sq, a.num_splits, num_sms());
 }
 
 size_t tfa_attn_workspace_bytes(const tfa_attn_args* args, int num_splits) {
   if (!args || args->B < 1 || args->Hq < 1 || args->Sq < 1) return 0;
   return splitkv_ws_bytes(from_attn_args(*args), num_splits);
+}
+
+int tfa_attn_varlen_kvcache_split_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
+                                      const tfa_kv_quant_args* quant, const tfa_split_args* split) {
+  if (!args || !split) return TFA_EINVAL_PTR;
+  return varlen_kvcache_impl(*args, rotary, quant, nullptr, nullptr, split);
+}
+
+int tfa_attn_varlen_kvcache_qkv8_split_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
+                                           const tfa_qkv_quant_args* quant, void* q8, const tfa_split_args* split) {
+  if (!args || !quant || !split || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
+  if (!q8 && rotary) return TFA_EINVAL_ROTARY;          // an e4m3 q arrives quantized: nothing to rotate
+  return varlen_kvcache_impl(*args, rotary, nullptr, quant, q8, split);
+}
+
+// The dense problem (B, Hq, Sq = max_seqlen_q, Sk = capacity) of a variable-length cache call, for its split count.
+int tfa_attn_varlen_kvcache_num_splits(const tfa_attn_varlen_kvcache_args* args, int num_splits) {
+  if (!args) return 1;
+  const Problem a = from_varlen_kvcache_args(*args);
+  if (a.B < 1 || a.Hq < 1 || args->max_seqlen_q < 1 || a.Sk < 1 || num_splits < 0) return 1;
+  return resolve_splits(a, args->max_seqlen_q, num_splits, num_sms());
+}
+
+size_t tfa_attn_varlen_kvcache_workspace_bytes(const tfa_attn_varlen_kvcache_args* args, int num_splits) {
+  if (!args || args->Hq < 1 || args->total_q < 1 || args->D < 1) return 0;
+  return splitkv_ws_bytes(from_varlen_kvcache_args(*args), num_splits);
 }
 
 int tfa_fwd_multi(const tfa_fwd_args* args, void* const* extra_out, int n_extra) {
@@ -1028,6 +1084,12 @@ long long tfa_internal_varlen_append_offset(int raw, const int* block_table, lon
                                             int page, int capacity, int n, int num_blocks, long long cs_b,
                                             long long cs_s, long long cs_h) {
   return tfa::append_offset(raw, block_table, bt_stride, b, i, h, page, capacity, n, num_blocks, cs_b, cs_s, cs_h);
+}
+// development aid (not in the public header): the split-KV combine's packed row -> sequence rule on the host.
+// out2 = {b, i}: packed row r is row i of sequence b; returns whether the combine merges it.
+int tfa_internal_packed_row_seq(const int* cu, int B, int total, int S, int r, int* out2) {
+  out2[0] = out2[1] = -1;
+  return tfa::packed_row_seq(cu, B, total, S, r, out2[0], out2[1]) ? 1 : 0;
 }
 // development aid (not in the public header): the rotary position rule of fa_kvcache_append.cuh on the host
 int tfa_internal_rotary_pos(int cache_len, int i, int causal, int is_query, int seqlen_ro) {

@@ -112,6 +112,11 @@ class QkvQuantArgs(ctypes.Structure):
                 ("v_scale", ctypes.c_float)]
 
 
+class SplitArgs(ctypes.Structure):
+    """struct tfa_split_args (include/tfa_b200.h)."""
+    _fields_ = [("num_splits", ctypes.c_int32), ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t)]
+
+
 class RotaryArgs(ctypes.Structure):
     """struct tfa_rotary_args (include/tfa_b200.h)."""
     _fields_ = [
@@ -171,6 +176,17 @@ def lib():
         L.tfa_attn_varlen_kvcache_qkv8_q16_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs),
                                                            ctypes.POINTER(RotaryArgs), ctypes.POINTER(QkvQuantArgs), vp]
         L.tfa_attn_varlen_kvcache_qkv8_q16_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_split_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ctypes.POINTER(RotaryArgs),
+                                                        ctypes.POINTER(KvQuantArgs), ctypes.POINTER(SplitArgs)]
+        L.tfa_attn_varlen_kvcache_split_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_qkv8_split_fwd.argtypes = [ctypes.POINTER(VarlenKvcacheArgs),
+                                                             ctypes.POINTER(RotaryArgs), ctypes.POINTER(QkvQuantArgs),
+                                                             vp, ctypes.POINTER(SplitArgs)]
+        L.tfa_attn_varlen_kvcache_qkv8_split_fwd.restype = ci
+        L.tfa_attn_varlen_kvcache_num_splits.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ci]
+        L.tfa_attn_varlen_kvcache_num_splits.restype = ci
+        L.tfa_attn_varlen_kvcache_workspace_bytes.argtypes = [ctypes.POINTER(VarlenKvcacheArgs), ci]
+        L.tfa_attn_varlen_kvcache_workspace_bytes.restype = ctypes.c_size_t
         L.tfa_selftest_wgmma_fp8.argtypes = [vp, vp, vp, ci, ci, ci, ci, vp]
         L.tfa_selftest_wgmma_fp8.restype = ci
         L.tfa_fwd_host.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, cf, ci]
@@ -492,7 +508,8 @@ def attn_kvcache_fwd(q, k_cache, v_cache, cache_seqlens, block_table=None, k_new
 def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqlens, block_table=None, k_new=None,
                             v_new=None, is_causal=False, scale=None, out_fp32=False, out=None, lse=None, stream=None,
                             k_scale=1.0, v_scale=1.0, rotary_cos=None, rotary_sin=None, rotary_interleaved=False,
-                            q_rot=None, q_scale=1.0, out_dtype=None, q8_scale=None, q8=None):
+                            q_rot=None, q_scale=1.0, out_dtype=None, q8_scale=None, q8=None, num_splits=1,
+                            return_splits=False, workspace=None):
     """A packed variable-length batch of queries against a KV cache through tfa_attn_varlen_kvcache_fwd(): q
     (total_q, Hq, D) with unit head_dim stride and cu_q int32 (B + 1) offsets, as attn_varlen_fwd; k_cache / v_cache
     and block_table as attn_kvcache_fwd; cache_seqlens (B,) int32; optional k_new / v_new packed (total_q, Hkv, D),
@@ -502,7 +519,11 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
     to `q_rot`, a contiguous (total_q, Hq, D) tensor of q's dtype, or to a buffer allocated here.  A
     torch.float8_e4m3fn q with an FP8 cache goes through tfa_attn_varlen_kvcache_qkv8_fwd() as attn_kvcache_fwd's, and
     a 16-bit q with q8_scale through tfa_attn_varlen_kvcache_qkv8_q16_fwd() (`q8`: (total_q, Hq, D)) as its.
-    Returns out (total_q, Hq, D) and lse (Hq, total_q); `out` / `lse` may be given to write into caller-owned buffers."""
+    num_splits != 1 takes the split-KV forms (tfa_attn_varlen_kvcache_split_fwd() /
+    tfa_attn_varlen_kvcache_qkv8_split_fwd()): n > 1 as asked, 0 library heuristic, with a workspace allocated here
+    when it splits, or the caller's `workspace` (a device tensor, passed as is with num_splits; given, it takes the
+    split-KV form at num_splits = 1 too).  Returns out (total_q, Hq, D) and lse (Hq, total_q), and with return_splits the split count;
+    `out` / `lse` may be given to write into caller-owned buffers."""
     import torch
     assert q.is_cuda and q.dim() == 3 and k_cache.dim() == 4 and k_cache.shape == v_cache.shape
     assert k_cache.stride() == v_cache.stride() and q.stride(2) == 1 and k_cache.stride(3) == 1
@@ -525,6 +546,9 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
                           _cache_dtype_code(q, qkv8, odt),
                           int(bool(is_causal)), float(scale), int(bool(out_fp32)), st)
     r = _rotary_args(q, rotary_cos, rotary_sin, rotary_interleaved, q_rot, st, q8_scale is None)
+    if num_splits != 1 or workspace is not None:
+        n = _varlen_split(a, num_splits, q.device, st, q, q8, q8_scale, qkv8, quant, r, workspace)
+        return (out, lse, n) if return_splits else (out, lse)
     if q8_scale is not None:
         q8 = _q8_scratch(q, q8, st)
         check(lib().tfa_attn_varlen_kvcache_qkv8_q16_fwd(ctypes.byref(a), ctypes.byref(r) if r is not None else None,
@@ -538,7 +562,35 @@ def attn_varlen_kvcache_fwd(q, k_cache, v_cache, cu_q, max_seqlen_q, cache_seqle
         check(lib().tfa_attn_varlen_kvcache_fp8_fwd(ctypes.byref(a), ctypes.byref(quant)))
     else:
         check(lib().tfa_attn_varlen_kvcache_fwd(ctypes.byref(a)))
-    return out, lse
+    return (out, lse, 1) if return_splits else (out, lse)
+
+
+def _varlen_split(a, num_splits, device, stream, q, q8, q8_scale, qkv8, quant, r, workspace):
+    """The split-KV form of attn_varlen_kvcache_fwd's call on the filled argument struct `a`; returns the split count."""
+    import torch
+    L = lib()
+    n = int(L.tfa_attn_varlen_kvcache_num_splits(ctypes.byref(a), int(num_splits)))
+    sp = SplitArgs(int(num_splits), None, 0)
+    if workspace is not None:
+        sp = SplitArgs(int(num_splits), workspace.data_ptr() if workspace.numel() else None,
+                       workspace.numel() * workspace.element_size())
+    elif n > 1:
+        need = int(L.tfa_attn_varlen_kvcache_workspace_bytes(ctypes.byref(a), n))
+        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=device)
+        sp = SplitArgs(n, ws.data_ptr(), need)
+        _WORKSPACES[(device.index, int(stream))] = ws       # kept alive as _split_workspace keeps its own
+    rp = ctypes.byref(r) if r is not None else None
+    if q8_scale is not None:
+        q8 = _q8_scratch(q, q8, stream)
+        check(L.tfa_attn_varlen_kvcache_qkv8_split_fwd(ctypes.byref(a), rp, ctypes.byref(qkv8), q8.data_ptr(),
+                                                       ctypes.byref(sp)))
+    elif qkv8 is not None:
+        check(L.tfa_attn_varlen_kvcache_qkv8_split_fwd(ctypes.byref(a), None, ctypes.byref(qkv8), None,
+                                                       ctypes.byref(sp)))
+    else:
+        check(L.tfa_attn_varlen_kvcache_split_fwd(ctypes.byref(a), rp, ctypes.byref(quant) if quant is not None else None,
+                                                  ctypes.byref(sp)))
+    return n
 
 
 def fwd_multi(q, k, v, is_causal, softmax_scale, out, extra_ptrs, lse=None, stream=None):
