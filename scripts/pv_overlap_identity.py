@@ -11,7 +11,11 @@ compare against), then run from the repository root on the GPU:
 Each library runs in a subprocess of its own (TFA_LIB selects it) and saves its results; this process compares them.
 Calls: the benchmark's workload (B64 H32 S4096 D128 bf16 causal; its first and last 8 (batch, head) compared
 element-wise, the whole out / lse by SHA-256), cfg2-cfg4, an fp16 D=64 causal call with an odd tile count, a split-KV
-fp32-output call, a varlen batch, a paged bf16 cache, a paged FP8 cache and an e4m3 (Q, K, V) call."""
+fp32-output call, a varlen batch, a paged bf16 cache, a paged FP8 cache, e4m3 (Q, K, V) dense and varlen calls, and
+cache calls that append k_new (their caches compared too): dense-query with rotary, with an e4m3 q, and with a 16-bit q
+quantized after rotary; variable-length with split-KV, with an FP8 cache, with an e4m3 q, and with a 16-bit q
+quantized after rotary.  Together they reach every forward mode and both cache calls' appends: 16-bit, rotary, FP8,
+and FP8 with the quantized q."""
 import argparse
 import hashlib
 import json
@@ -92,6 +96,47 @@ def run_cases(path):
     out, lse = tfa.attn_fwd(q, k, v, True, 128 ** -0.5, q_scale=0.25, k_scale=0.25, v_scale=0.25,
                             out_dtype=torch.bfloat16)
     res["e4m3 Q/K/V B2 H16 S2048 D128 causal, bf16 out"] = {"out": out.cpu(), "lse": lse.cpu()}
+
+    g = gen(26)
+    lens = [1000, 77, 2048, 513]
+    cu = torch.tensor([0] + list(torch.tensor(lens).cumsum(0)), dtype=torch.int32, device=dev)
+    q, k, v = (rnd(g, sum(lens), 16, 128).float().div(0.25).to(torch.float8_e4m3fn) for _ in range(3))
+    out, lse = tfa.attn_varlen_fwd(q, k, v, cu, cu, max(lens), True, 128 ** -0.5, q_scale=0.25, k_scale=0.25,
+                                   v_scale=0.25, out_dtype=torch.bfloat16)
+    res["e4m3 varlen 4 seqs H16 D128 causal, bf16 out"] = {"out": out.cpu(), "lse": lse.cpu()}
+
+    # calls that append k_new to the paged caches above (a fresh copy each), the cache after the call compared too:
+    # the dense-query calls append 64 rows per sequence, the variable-length ones each sequence's query rows
+    g = gen(27)
+    e4m3 = lambda x: x.float().div(0.25).clamp(-448, 448).to(torch.float8_e4m3fn)    # noqa: E731
+    cos, sin = (rnd(g, nper * page, 32) for _ in range(2))                            # rotary_dim 64
+    kn, vn = rnd(g, Bc, Sq, Hkv, Dc), rnd(g, Bc, Sq, Hkv, Dc)
+    qlens = [64, 1, 37, 100]
+    cuq = torch.tensor([0] + list(torch.tensor(qlens).cumsum(0)), dtype=torch.int32, device=dev)
+    qv, knv, vnv = rnd(g, sum(qlens), Hq, Dc), rnd(g, sum(qlens), Hkv, Dc), rnd(g, sum(qlens), Hkv, Dc)
+    fp8 = dict(k_scale=0.25, v_scale=0.25)
+    appends = {
+        "paged bf16 cache + rotary append B4 Sq64 causal": (qc, kc, vc, dict(rotary_cos=cos, rotary_sin=sin)),
+        "paged e4m3 q + FP8 cache append B4 Sq64 causal": (e4m3(qc), k8, v8, dict(q_scale=0.25,
+                                                                                 out_dtype=torch.bfloat16, **fp8)),
+        "paged 16-bit q quantized + rotary, FP8 cache append B4 Sq64 causal": (
+            qc, k8, v8, dict(q8_scale=0.25, rotary_cos=cos, rotary_sin=sin, **fp8)),
+        "varlen paged bf16 cache append, split-KV x4": (qv, kc, vc, dict(num_splits=4)),
+        "varlen paged FP8 cache append": (qv, k8, v8, fp8),
+        "varlen paged e4m3 q + FP8 cache append": (e4m3(qv), k8, v8, dict(q_scale=0.25, out_dtype=torch.bfloat16,
+                                                                          **fp8)),
+        "varlen paged 16-bit q quantized + rotary, FP8 cache append": (
+            qv, k8, v8, dict(q8_scale=0.25, rotary_cos=cos, rotary_sin=sin, **fp8)),
+    }
+    for name, (qa, kca, vca, kw) in appends.items():
+        kca, vca = kca.clone(), vca.clone()
+        if qa.dim() == 4:
+            out, lse = tfa.attn_kvcache_fwd(qa, kca, vca, sl, table, k_new=kn, v_new=vn, is_causal=True, **kw)
+        else:
+            out, lse = tfa.attn_varlen_kvcache_fwd(qa, kca, vca, cuq, max(qlens), sl, table, k_new=knv, v_new=vnv,
+                                                   is_causal=True, **kw)
+        res[name] = {"out": out.cpu(), "lse": lse.cpu(), "k_cache": kca.view(torch.uint8).cpu(),
+                     "v_cache": vca.view(torch.uint8).cpu()}
     torch.cuda.synchronize()
     torch.save(res, path)
 

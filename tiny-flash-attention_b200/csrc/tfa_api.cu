@@ -16,7 +16,6 @@
 #include <cudaTypedefs.h>
 #include <atomic>
 #include <mutex>
-#include <type_traits>
 #include <vector>
 #include <cfloat>
 #include <cmath>
@@ -412,46 +411,6 @@ int validate_qkv_quant(const tfa_qkv_quant_args& q, Problem& a) {
   return 0;
 }
 
-// The dense forward.  `quant` nullptr: 16-bit q / k / v, optionally with the fused exchange (n_extra > 0).  Otherwise
-// e4m3 ones, checked after the 16-bit checks, for the kDenseFp8 forward.
-int fwd_impl(Problem a, const tfa_qkv_quant_args* quant, void* const* extra_dst = nullptr, int n_extra = 0) {
-  int rc = validate(a);
-  if (rc) return rc;
-  if (quant && (rc = validate_qkv_quant(*quant, a))) return rc;
-  if (!arch_ok()) return TFA_EARCH;
-  init_dbg();
-  const bool causal = a.causal != 0, f32 = a.out_fp32 != 0;
-  const bool plain = (a.Sq == a.Sk) && (a.Hq == a.Hkv);
-  if (n_extra > 0) {
-    // fused exchange: 16-bit output of the reference-shaped problem only, in one pass (tfa_fwd_args has no split
-    // count: from_fwd_args asks for one)
-    if (n_extra > 7 || extra_dst == nullptr || f32 || !plain || a.num_splits > 1)
-      return TFA_EINVAL_SHAPE;
-    for (int i = 0; i < n_extra; ++i)
-      if (extra_dst[i] == nullptr || (reinterpret_cast<uintptr_t>(extra_dst[i]) & 15u)) return TFA_EINVAL_PTR;
-  }
-
-  SplitPlan plan;
-  if ((rc = plan_splits(a, a.Sq, plan))) return rc;
-
-  FwdParams p{};
-  p.Sk = a.Sk;
-  p.causal_off = causal ? a.Sk - a.Sq : 0;             // < 0: the first Sq - Sk rows see no key
-  p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
-  for (int i = 0; i < n_extra; ++i) p.extra_dst[i] = extra_dst[i];
-  p.n_extra_dst = n_extra;
-
-  // FP8: 8-bit swizzled Q / K maps the wgmma reads in place, the raw V map the converter transposes, and V's scale
-  const int dt = quant ? TFA_FP8_E4M3 : a.dtype;
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, dt, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss, quant != nullptr))) return rc;
-  if ((rc = make_tmap(&tk, a.k, dt, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss, quant != nullptr))) return rc;
-  if ((rc = make_tmap(&tv, a.v, dt, a.D, a.Sk, a.B, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
-  if (!quant) return run_forward<tfa::kDense>(a, p, a.Sq, tq, tk, tv, plan);
-  p.v_scale = quant->v_scale;
-  return run_forward<tfa::kDenseFp8>(a, p, a.Sq, tq, tk, tv, plan);
-}
-
 Problem from_fwd_args(const tfa_fwd_args& a) {
   Problem q;
   q.q = a.q; q.k = a.k; q.v = a.v; q.out = a.out; q.lse = a.lse;
@@ -494,46 +453,6 @@ Problem from_varlen_args(const tfa_attn_varlen_args& a) {
   return q;
 }
 
-// cu_seqlens_q of a packed query batch, a non-null 4-byte aligned pointer, and max_seqlen_q in [1, total_q].
-template <typename Args>
-int validate_seqlens_q(const Args& va) {
-  if (!va.cu_seqlens_q || (reinterpret_cast<uintptr_t>(va.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
-  if (va.max_seqlen_q < 1 || va.max_seqlen_q > va.total_q) return TFA_EINVAL_SEQLENS;
-  return 0;
-}
-
-// The variable-length forward over the packed tensors as one batch entry.  `quant` as fwd_impl, for the kVarlenFp8
-// forward.
-int varlen_impl(const tfa_attn_varlen_args& va, const tfa_qkv_quant_args* quant) {
-  Problem a = from_varlen_args(va);
-  int rc = validate(a);
-  if (rc) return rc;
-  if ((rc = validate_seqlens_q(va))) return rc;
-  if (!va.cu_seqlens_k || (reinterpret_cast<uintptr_t>(va.cu_seqlens_k) & 3u)) return TFA_EINVAL_SEQLENS;
-  if (quant && (rc = validate_qkv_quant(*quant, a))) return rc;
-  if (!arch_ok()) return TFA_EARCH;
-  init_dbg();
-
-  FwdParams p{};
-  p.cu_q = va.cu_seqlens_q;
-  p.cu_k = va.cu_seqlens_k;
-  p.total_q = a.Sq;
-  p.total_k = a.Sk;
-
-  // FP8: as fwd_impl
-  const int dt = quant ? TFA_FP8_E4M3 : a.dtype;
-  CUtensorMap tq, tk, tv;
-  if ((rc = make_tmap(&tq, a.q, dt, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, quant != nullptr))) return rc;
-  if ((rc = make_tmap(&tk, a.k, dt, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss, quant != nullptr))) return rc;
-  if ((rc = make_tmap(&tv, a.v, dt, a.D, a.Sk, 1, a.Hkv, 0, a.ksh, a.kss))) return rc;
-  // the grid covers max_seqlen_q rows of every (sequence, head); items past a sequence's end return at once.  One
-  // split holds every KV tile of any sequence.
-  const SplitPlan one{1, 0x7fffffff};
-  if (!quant) return run_forward<tfa::kVarlen>(a, p, va.max_seqlen_q, tq, tk, tv, one);
-  p.v_scale = quant->v_scale;
-  return run_forward<tfa::kVarlenFp8>(a, p, va.max_seqlen_q, tq, tk, tv, one);
-}
-
 // The cache problem as the dense one of Sk = capacity keys (what validate() and the split-KV helpers see of it).
 Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   Problem q;
@@ -551,73 +470,153 @@ Problem from_kvcache_args(const tfa_attn_kvcache_args& a) {
   return q;
 }
 
+// The variable-length cache problem as the varlen one of total_q query rows (what validate() checks of q and out)
+// against the cache of Sk = capacity keys.
+Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
+  Problem q;
+  q.q = a.q; q.k = a.k_cache; q.v = a.v_cache; q.out = a.out; q.lse = a.lse;
+  q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.D = a.D;
+  const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
+  q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
+  q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
+  q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
+  q.ol = {0, a.D, static_cast<long long>(a.Hq) * a.D, 0, a.total_q};   // out (total_q, Hq, D), lse (Hq, total_q)
+  q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
+  q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
+  q.stream = static_cast<cudaStream_t>(a.stream);
+  q.packed = true;
+  return q;
+}
+
 // The cache arguments of both cache calls: the lengths, the block table or the contiguous cache, k_new with v_new and
 // their strides.  Only the dense-query call has Snew and a batch stride of k_new.
+struct CacheArgs {
+  void *k_cache, *v_cache;
+  const void *k_new, *v_new;
+  const int32_t *cache_seqlens, *block_table;
+  int num_blocks, page_block_size, max_blocks_per_seq;
+  long long block_table_stride, new_stride_s, new_stride_h;
+  int Snew;                      // the dense-query call's
+  long long new_stride_b;        // the dense-query call's
+};
+
 template <typename Args>
-int validate_cache(const Args& ka) {
-  constexpr bool dense_q = std::is_same_v<Args, tfa_attn_kvcache_args>;
+CacheArgs from_cache_args(const Args& ka) {
+  CacheArgs c{};
+  c.k_cache = ka.k_cache; c.v_cache = ka.v_cache; c.k_new = ka.k_new; c.v_new = ka.v_new;
+  c.cache_seqlens = ka.cache_seqlens; c.block_table = ka.block_table;
+  c.num_blocks = ka.num_blocks; c.page_block_size = ka.page_block_size; c.max_blocks_per_seq = ka.max_blocks_per_seq;
+  c.block_table_stride = ka.block_table_stride; c.new_stride_s = ka.new_stride_s; c.new_stride_h = ka.new_stride_h;
+  return c;
+}
+
+// Where a call's keys come from: the Problem's k / v tensors, packed ones through cu_seqlens_k, or the cache.
+enum class Keys { kTensors, kPacked, kCache };
+
+// A forward call: its Problem and what it asks for beyond it.  A null pointer: the call has no such part.
+struct Call {
+  Problem a;
+  Keys keys;
+  const int32_t* cu_seqlens_q = nullptr;     // a.packed: the sequences' query rows, at most max_seqlen_q each
+  int max_seqlen_q = 0;
+  const int32_t* cu_seqlens_k = nullptr;     // Keys::kPacked
+  CacheArgs cache{};                          // Keys::kCache
+  // the append also rotates q and k_new, and the forward reads its queries from rotary->q_rot (from q8 with q8)
+  const tfa_rotary_args* rotary = nullptr;
+  // an FP8 cache, into which the append quantizes and which the forward widens in shared memory
+  const tfa_kv_quant_args* kv_quant = nullptr;
+  // e4m3 q and K / V (or an FP8 cache) on 8-bit wgmma; a.dtype is the output's and k_new's
+  const tfa_qkv_quant_args* qkv_quant = nullptr;
+  // with qkv_quant, a 16-bit q: the append writes e4m3(q / q_scale) (rot(q) with rotary, rotary->q_rot unused) into
+  // this contiguous scratch, the forward's q, whose layout the quantization checks see
+  void* q8 = nullptr;
+  void* const* extra_dst = nullptr;          // the fused exchange: n_extra more destinations of the output
+  int n_extra = 0;
+};
+
+Call dense_call(const Problem& a, const tfa_qkv_quant_args* qkv_quant, void* const* extra_dst = nullptr,
+                int n_extra = 0) {
+  Call c{a, Keys::kTensors};
+  c.qkv_quant = qkv_quant;
+  c.extra_dst = extra_dst;
+  c.n_extra = n_extra;
+  return c;
+}
+
+Call varlen_call(const tfa_attn_varlen_args& va, const tfa_qkv_quant_args* qkv_quant) {
+  Call c{from_varlen_args(va), Keys::kPacked};
+  c.cu_seqlens_q = va.cu_seqlens_q; c.max_seqlen_q = va.max_seqlen_q; c.cu_seqlens_k = va.cu_seqlens_k;
+  c.qkv_quant = qkv_quant;
+  return c;
+}
+
+Call kvcache_call(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* rotary, const tfa_kv_quant_args* kv_quant,
+                  const tfa_qkv_quant_args* qkv_quant = nullptr, void* q8 = nullptr) {
+  Call c{from_kvcache_args(ka), Keys::kCache};
+  c.cache = from_cache_args(ka);
+  c.cache.Snew = ka.Snew; c.cache.new_stride_b = ka.new_stride_b;
+  c.rotary = rotary; c.kv_quant = kv_quant; c.qkv_quant = qkv_quant; c.q8 = q8;
+  return c;
+}
+
+// `split` nullptr: one pass.  Otherwise split-KV as the dense-query call plans it, for the dense problem of
+// max_seqlen_q rows per sequence, into packed partials.
+Call varlen_kvcache_call(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* rotary,
+                         const tfa_kv_quant_args* kv_quant, const tfa_qkv_quant_args* qkv_quant = nullptr,
+                         void* q8 = nullptr, const tfa_split_args* split = nullptr) {
+  Call c{from_varlen_kvcache_args(va), Keys::kCache};
+  if (split) {
+    c.a.num_splits = split->num_splits; c.a.ws = split->workspace; c.a.ws_bytes = split->workspace_bytes;
+  }
+  c.cu_seqlens_q = va.cu_seqlens_q; c.max_seqlen_q = va.max_seqlen_q;
+  c.cache = from_cache_args(va);
+  c.rotary = rotary; c.kv_quant = kv_quant; c.qkv_quant = qkv_quant; c.q8 = q8;
+  return c;
+}
+
+// cu_seqlens_q of a packed query batch, a non-null 4-byte aligned pointer, and max_seqlen_q in [1, total_q].
+int validate_seqlens_q(const Call& c) {
+  if (!c.cu_seqlens_q || (reinterpret_cast<uintptr_t>(c.cu_seqlens_q) & 3u)) return TFA_EINVAL_SEQLENS;
+  if (c.max_seqlen_q < 1 || c.max_seqlen_q > c.a.Sq) return TFA_EINVAL_SEQLENS;
+  return 0;
+}
+
+// The cache arguments; Snew and the batch stride of k_new only for the dense-query call.
+int validate_cache(const Call& c) {
+  const CacheArgs& ka = c.cache;
   if (!ka.cache_seqlens || (reinterpret_cast<uintptr_t>(ka.cache_seqlens) & 3u) ||
       (reinterpret_cast<uintptr_t>(ka.block_table) & 3u))
     return TFA_EINVAL_KVCACHE;
   if (ka.num_blocks < 1 || ka.max_blocks_per_seq < 1 || ka.page_block_size < 1) return TFA_EINVAL_KVCACHE;
   if (ka.block_table) {
     if (ka.page_block_size % 128 || ka.block_table_stride < ka.max_blocks_per_seq) return TFA_EINVAL_KVCACHE;
-  } else if (ka.max_blocks_per_seq != 1 || ka.num_blocks < ka.B) {
+  } else if (ka.max_blocks_per_seq != 1 || ka.num_blocks < c.a.B) {
     return TFA_EINVAL_KVCACHE;           // contiguous: one page (block b) per sequence
   }
   if ((ka.k_new == nullptr) != (ka.v_new == nullptr)) return TFA_EINVAL_KVCACHE;
   if (ka.k_new) {
-    if constexpr (dense_q) {
+    if (!c.a.packed) {
       const long long cap = static_cast<long long>(ka.max_blocks_per_seq) * ka.page_block_size;
       if (ka.Snew < 1 || ka.Snew > cap) return TFA_EINVAL_KVCACHE;
     }
     if ((reinterpret_cast<uintptr_t>(ka.k_new) | reinterpret_cast<uintptr_t>(ka.v_new)) & 15u) return TFA_EINVAL_PTR;
     if ((ka.new_stride_s % 8) || (ka.new_stride_h % 8) || ka.new_stride_s < 0 || ka.new_stride_h < 0)
       return TFA_EINVAL_STRIDE;
-    if constexpr (dense_q) {
-      if ((ka.new_stride_b % 8) || ka.new_stride_b < 0) return TFA_EINVAL_STRIDE;
-    }
+    if (!c.a.packed && ((ka.new_stride_b % 8) || ka.new_stride_b < 0)) return TFA_EINVAL_STRIDE;
   }
   return 0;
 }
 
-// The cache side of a cache call whose arguments passed (a = its Problem, capacity = a.Sk): the K/V tensor maps over
-// the pages, the append of `n` rows per sequence (ap.chunks = 0 without k_new; the caller sets its k_new layout fields
-// n_sb / cu_q / total_q) and the cache fields of the forward but snew.
-// `cache_dtype`: a.dtype, or TFA_FP8_E4M3 for an FP8 cache.  `k_operand8`: the FP8 cache's K map is the 8-bit wgmma
-// operand the e4m3-query modes read in place (make_tmap's operand8); V's stays the raw map the converter reads.
-template <typename Args>
-int setup_cache(const Args& ka, const Problem& a, int n, CUtensorMap& tk, CUtensorMap& tv, tfa::AppendParams& ap,
-                FwdParams& p, int cache_dtype, bool k_operand8 = false) {
-  const int page = ka.block_table ? ka.page_block_size : a.Sk;
-  if (int rc = make_tmap(&tk, a.k, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss, k_operand8))
-    return rc;
-  if (int rc = make_tmap(&tv, a.v, cache_dtype, a.D, page, ka.num_blocks, a.Hkv, a.ksb, a.ksh, a.kss)) return rc;
-  ap = tfa::AppendParams{};
-  ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
-  ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
-  ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
-  ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
-  ap.page = page; ap.capacity = a.Sk; ap.snew = n; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
-  ap.chunks = ka.k_new ? static_cast<long long>(a.B) * n * a.Hkv * (a.D / 8) : 0;
-  p.cache_seqlens = ka.cache_seqlens;
-  p.block_table = ka.block_table;
-  p.bt_stride = ka.block_table_stride;
-  p.page = page;
-  p.capacity = a.Sk;
-  return 0;
-}
-
-// The rotary arguments of either cache call whose cache arguments passed (capacity = a.Sk).  `q_rot` false: the call
-// writes its rotated queries elsewhere (the q8 scratch) and ra.q_rot is not read.
-template <typename Args>
-int validate_rotary(const Args& ka, const Problem& a, const tfa_rotary_args& ra, bool q_rot = true) {
+// The rotary arguments of a cache call whose cache arguments passed (capacity = a.Sk).  With q8 the call writes its
+// rotated queries there and rotary->q_rot is not read.
+int validate_rotary(const Call& c) {
+  const tfa_rotary_args& ra = *c.rotary;
   if (!ra.cos || !ra.sin || ((reinterpret_cast<uintptr_t>(ra.cos) | reinterpret_cast<uintptr_t>(ra.sin)) & 15u))
     return TFA_EINVAL_ROTARY;
-  if (q_rot && (!ra.q_rot || (reinterpret_cast<uintptr_t>(ra.q_rot) & 15u))) return TFA_EINVAL_ROTARY;
-  if (ra.rotary_dim < 16 || ra.rotary_dim > a.D || ra.rotary_dim % 16) return TFA_EINVAL_ROTARY;
-  if (ra.seqlen_ro < a.Sk) return TFA_EINVAL_ROTARY;      // every key position is below the capacity
-  if (!ka.k_new) return TFA_EINVAL_ROTARY;                // as flash-attn: rotary rotates the appended keys
+  if (!c.q8 && (!ra.q_rot || (reinterpret_cast<uintptr_t>(ra.q_rot) & 15u))) return TFA_EINVAL_ROTARY;
+  if (ra.rotary_dim < 16 || ra.rotary_dim > c.a.D || ra.rotary_dim % 16) return TFA_EINVAL_ROTARY;
+  if (ra.seqlen_ro < c.a.Sk) return TFA_EINVAL_ROTARY;    // every key position is below the capacity
+  if (!c.cache.k_new) return TFA_EINVAL_ROTARY;            // as flash-attn: rotary rotates the appended keys
   return 0;
 }
 
@@ -639,11 +638,10 @@ int validate_quant(const tfa_kv_quant_args& q, Problem& a, tfa::KvQuant& qs) {
 
 // The query side of an append that writes the queries the forward reads: rot(q) (`ra`), or with `q8` the e4m3 codes of
 // q or rot(q) into q8.  Sets a.q to that scratch with its contiguous strides: (B, S, Hq, D), or packed (total_q, Hq, D)
-// when `packed` (S = max_seqlen_q rows of every sequence then).  out and lse keep their layout (a.ol).
-void set_query_append(tfa::AppendKernelParams& rp, Problem& a, const tfa_rotary_args* ra, void* q8, int S,
-                      bool packed) {
+// (S = max_seqlen_q rows of every sequence then).  out and lse keep their layout (a.ol).
+void set_query_append(tfa::AppendKernelParams& rp, Problem& a, const tfa_rotary_args* ra, void* q8, int S) {
   rp.q = a.q; rp.q_rot = q8 ? q8 : ra->q_rot;
-  rp.q_sb = packed ? 0 : a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
+  rp.q_sb = a.packed ? 0 : a.qsb; rp.q_ss = a.qss; rp.q_sh = a.qsh;
   if (ra) {
     rp.cos = ra->cos; rp.sin = ra->sin;
     rp.rotary_dim = ra->rotary_dim; rp.seqlen_ro = ra->seqlen_ro;
@@ -654,146 +652,146 @@ void set_query_append(tfa::AppendKernelParams& rp, Problem& a, const tfa_rotary_
   a.q = rp.q_rot;
   a.qss = static_cast<long long>(a.Hq) * a.D;
   a.qsh = a.D;
-  a.qsb = packed ? 0 : a.qss * a.Sq;
+  a.qsb = a.packed ? 0 : a.qss * a.Sq;
 }
 
-// `ra` nullptr: the plain cache forward.  Otherwise the append also rotates q and k_new, and the forward reads its
-// queries from ra->q_rot.  `quant` nullptr: a 16-bit cache; otherwise an FP8 one, into which the append quantizes and
-// which the kCacheFp8 forward reads.  `qkv8` (with `quant` nullptr): e4m3 q against an FP8 cache, a.dtype the output's
-// and k_new's; the append quantizes as for `quant` and the kCacheQkv8 forward reads q and the cache on 8-bit wgmma.
-// Without `q8`, q arrives in e4m3 and `ra` is nullptr.  With `q8`, q is 16-bit: the append writes e4m3(q / q_scale)
-// (rot(q) with `ra`, ra->q_rot unused) into the contiguous scratch q8, the forward's q, whose layout the quantization
-// checks see.
-int kvcache_impl(const tfa_attn_kvcache_args& ka, const tfa_rotary_args* ra, const tfa_kv_quant_args* quant,
-                 const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr) {
-  Problem a = from_kvcache_args(ka);
-  int rc = validate_cache(ka);          // first: a table of 0 pages is a cache error, not a 0-key shape error
-  if (rc) return rc;
+// The cache side of a cache call whose arguments passed (a = its Problem, capacity = a.Sk; `page` rows per K/V map
+// entry): the key side of the append (ap.chunks = 0 without k_new) and the cache fields of the forward.  The
+// dense-query call appends Snew rows of every sequence from (B, Snew, Hkv, D) k_new, and p.snew counts them; the
+// variable-length call appends each sequence's n_b <= S rows, packed as q, and p.snew is a flag: sequence b appends as
+// many keys as it has query rows.
+void setup_cache(const Call& c, const Problem& a, int S, int page, tfa::AppendParams& ap, FwdParams& p) {
+  const CacheArgs& ka = c.cache;
+  const int n = a.packed ? S : ka.k_new ? ka.Snew : 0;
+  ap.k_new = ka.k_new; ap.v_new = ka.v_new; ap.k_cache = ka.k_cache; ap.v_cache = ka.v_cache;
+  ap.n_ss = ka.new_stride_s; ap.n_sh = ka.new_stride_h;
+  if (a.packed) {
+    ap.cu_q = c.cu_seqlens_q;
+    ap.total_q = a.Sq;
+  } else {
+    ap.n_sb = ka.new_stride_b;
+  }
+  ap.c_sb = a.ksb; ap.c_ss = a.kss; ap.c_sh = a.ksh;
+  ap.cache_seqlens = ka.cache_seqlens; ap.block_table = ka.block_table; ap.bt_stride = ka.block_table_stride;
+  ap.page = page; ap.capacity = a.Sk; ap.snew = n; ap.num_blocks = ka.num_blocks; ap.Hkv = a.Hkv;
+  ap.chunks = ka.k_new ? static_cast<long long>(a.B) * n * a.Hkv * (a.D / 8) : 0;
+  p.cache_seqlens = ka.cache_seqlens;
+  p.block_table = ka.block_table;
+  p.bt_stride = ka.block_table_stride;
+  p.page = page;
+  p.capacity = a.Sk;
+  p.snew = a.packed ? (ka.k_new ? 1 : 0) : n;
+}
+
+// How a call computes: on 16-bit operands, against an FP8 cache widened to 16 bits in shared memory, or with e4m3 q
+// on 8-bit wgmma.
+enum class Datapath { k16Bit, kFp8Cache, kE4m3 };
+
+// The forward mode that solves `problem` (tfa::kDense / kVarlen / kCache / kVarlenCache) on `path`; -1: none does.
+int forward_mode(int problem, Datapath path) {
+  static constexpr int fp8_cache[4] = {-1, -1, tfa::kCacheFp8, tfa::kVarlenCacheFp8};
+  static constexpr int e4m3[4] = {tfa::kDenseFp8, tfa::kVarlenFp8, tfa::kCacheQkv8, tfa::kVarlenCacheQkv8};
+  return path == Datapath::k16Bit ? problem : path == Datapath::kFp8Cache ? fp8_cache[problem] : e4m3[problem];
+}
+
+// Every forward call.  Its checks run in this order, each only when the call has that part; they and the split plan
+// come before anything is written, so a rejected call leaves the cache untouched.  Then the tensor maps, the append,
+// the forward and, with split-KV, the combine.
+int run_call(Call c) {
+  Problem& a = c.a;
+  const bool cache = c.keys == Keys::kCache;
+  int rc;
+  // the cache first: a table of 0 pages is a cache error, not a 0-key shape error
+  if (cache && (rc = validate_cache(c))) return rc;
   if ((rc = validate(a))) return rc;
-  if (ra && (rc = validate_rotary(ka, a, *ra, q8 == nullptr))) return rc;
+  if (a.packed && (rc = validate_seqlens_q(c))) return rc;
+  if (c.keys == Keys::kPacked && (!c.cu_seqlens_k || (reinterpret_cast<uintptr_t>(c.cu_seqlens_k) & 3u)))
+    return TFA_EINVAL_SEQLENS;
+  if (c.rotary && (rc = validate_rotary(c))) return rc;
+  // the query rows per (batch, head) the grid covers: packed, max_seqlen_q of every sequence (items past a sequence's
+  // end return at once), and so do the append's query and key chunks (they return past n_b)
+  const int S = a.packed ? c.max_seqlen_q : a.Sq;
   tfa::AppendKernelParams rp{};
-  if (ra || q8) set_query_append(rp, a, ra, q8, a.Sq, false);
+  if (c.rotary || c.q8) set_query_append(rp, a, c.rotary, c.q8, S);
   tfa::KvQuant qs{1.0f, 1.0f};
-  if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
-  if (qkv8) {
-    if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
-    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale, qkv8->q_scale};
+  if (c.kv_quant && (rc = validate_quant(*c.kv_quant, a, qs))) return rc;
+  if (c.qkv_quant) {
+    if ((rc = validate_qkv_quant(*c.qkv_quant, a))) return rc;
+    qs = tfa::KvQuant{c.qkv_quant->k_scale, c.qkv_quant->v_scale, c.qkv_quant->q_scale};
   }
   if (!arch_ok()) return TFA_EARCH;
-  init_dbg();
-  const int snew = ka.k_new ? ka.Snew : 0;
-
-  SplitPlan plan;                       // before the append: a workspace error leaves the cache untouched
-  if ((rc = plan_splits(a, a.Sq, plan))) return rc;
-
-  // qkv8: the 8-bit swizzled Q and K maps the wgmma reads in place, as fwd_impl builds them
-  const bool fp8_cache = quant || qkv8;
-  CUtensorMap tq, tk, tv;
-  FwdParams p{};
-  if ((rc = make_tmap(&tq, a.q, qkv8 ? TFA_FP8_E4M3 : a.dtype, a.D, a.Sq, a.B, a.Hq, a.qsb, a.qsh, a.qss,
-                      qkv8 != nullptr)))
-    return rc;
-  if ((rc = setup_cache(ka, a, snew, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype, qkv8 != nullptr))) return rc;
-  rp.ap.n_sb = ka.new_stride_b;
-  // rotary needs k_new (validate_rotary): every rotary call appends; a quantized q is written even without k_new
-  if (snew > 0 || q8) {
-    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, q8 != nullptr, a.D, a.dtype == TFA_BF16,
-                                    ra != nullptr, ra && ra->interleaved != 0, a.stream);
-    if (rc) return rc;
+  if (c.n_extra > 0) {
+    // fused exchange: 16-bit output of the reference-shaped problem only, in one pass (tfa_fwd_args has no split
+    // count: from_fwd_args asks for one)
+    if (c.n_extra > 7 || c.extra_dst == nullptr || a.out_fp32 || a.Sq != a.Sk || a.Hq != a.Hkv || a.num_splits > 1)
+      return TFA_EINVAL_SHAPE;
+    for (int i = 0; i < c.n_extra; ++i)
+      if (c.extra_dst[i] == nullptr || (reinterpret_cast<uintptr_t>(c.extra_dst[i]) & 15u)) return TFA_EINVAL_PTR;
   }
-
-  p.snew = snew;
-  if (qkv8) {
-    p.v_scale = qs.v_scale;
-    return run_forward<tfa::kCacheQkv8>(a, p, a.Sq, tq, tk, tv, plan);
-  }
-  if (quant) {
-    p.v_scale = qs.v_scale;
-    return run_forward<tfa::kCacheFp8>(a, p, a.Sq, tq, tk, tv, plan);
-  }
-  return run_forward<tfa::kCache>(a, p, a.Sq, tq, tk, tv, plan);
-}
-
-// The variable-length cache problem as the varlen one of total_q query rows (what validate() checks of q and out)
-// against the cache of Sk = capacity keys.
-Problem from_varlen_kvcache_args(const tfa_attn_varlen_kvcache_args& a) {
-  Problem q;
-  q.q = a.q; q.k = a.k_cache; q.v = a.v_cache; q.out = a.out; q.lse = a.lse;
-  q.B = a.B; q.Hq = a.Hq; q.Hkv = a.Hkv; q.Sq = a.total_q; q.D = a.D;
-  const long long cap = static_cast<long long>(a.max_blocks_per_seq) * a.page_block_size;
-  q.Sk = cap > 0x7fffffffLL ? 0 : static_cast<int>(cap);          // 0 fails validate() as TFA_EINVAL_SHAPE
-  q.qsb = 0; q.qsh = a.q_stride_h; q.qss = a.q_stride_s;
-  q.ksb = a.cache_stride_block; q.ksh = a.cache_stride_h; q.kss = a.cache_stride_s;
-  q.ol = {0, a.D, static_cast<long long>(a.Hq) * a.D, 0, a.total_q};   // out (total_q, Hq, D), lse (Hq, total_q)
-  q.dtype = a.dtype; q.causal = a.is_causal; q.scale = a.softmax_scale; q.out_fp32 = a.out_fp32;
-  q.num_splits = 1; q.ws = nullptr; q.ws_bytes = 0;
-  q.stream = static_cast<cudaStream_t>(a.stream);
-  q.packed = true;
-  return q;
-}
-
-// `ra`, `quant`, `qkv8` and `q8` as kvcache_impl: with `ra`, the append also rotates the packed q rows and k_new, and
-// the forward reads its queries from ra->q_rot (from q8 with `q8`).  `split` nullptr: one pass.  Otherwise split-KV as
-// kvcache_impl plans it for the dense problem of max_seqlen_q rows per sequence, into packed partials.
-int varlen_kvcache_impl(const tfa_attn_varlen_kvcache_args& va, const tfa_rotary_args* ra,
-                        const tfa_kv_quant_args* quant, const tfa_qkv_quant_args* qkv8 = nullptr, void* q8 = nullptr,
-                        const tfa_split_args* split = nullptr) {
-  Problem a = from_varlen_kvcache_args(va);
-  if (split) {
-    a.num_splits = split->num_splits; a.ws = split->workspace; a.ws_bytes = split->workspace_bytes;
-  }
-  int rc = validate_cache(va);          // first, as for tfa_attn_kvcache_fwd
-  if (rc) return rc;
-  if ((rc = validate(a))) return rc;
-  if ((rc = validate_seqlens_q(va))) return rc;
-  if (ra && (rc = validate_rotary(va, a, *ra, q8 == nullptr))) return rc;
-  // without rotary or q8 only rp.ap is used; with them the query chunks cover max_seqlen_q rows of every sequence, as
-  // the key chunks do (the append returns past n_b)
-  tfa::AppendKernelParams rp{};
-  if (ra || q8) set_query_append(rp, a, ra, q8, va.max_seqlen_q, true);
-  tfa::KvQuant qs{1.0f, 1.0f};
-  if (quant && (rc = validate_quant(*quant, a, qs))) return rc;
-  if (qkv8) {
-    if ((rc = validate_qkv_quant(*qkv8, a))) return rc;
-    qs = tfa::KvQuant{qkv8->k_scale, qkv8->v_scale, qkv8->q_scale};
-  }
-  if (!arch_ok()) return TFA_EARCH;
   init_dbg();
 
-  SplitPlan plan;                       // before the append, as kvcache_impl
-  if ((rc = plan_splits(a, va.max_seqlen_q, plan))) return rc;
+  // packed keys: one split holds every KV tile of any sequence.  Otherwise every split covers the same KV tiles of
+  // every sequence, so a packed sequence with few keys fills only its first splits.
+  SplitPlan plan{1, 0x7fffffff};
+  if (c.keys != Keys::kPacked && (rc = plan_splits(a, S, plan))) return rc;
 
-  const bool fp8_cache = quant || qkv8;
+  // e4m3: the 8-bit swizzled Q and K maps the wgmma reads in place, the raw V map the converter transposes.  An FP8
+  // cache: raw maps the converter widens.  A contiguous cache is one page of capacity rows per sequence.
+  const Datapath path = c.qkv_quant ? Datapath::kE4m3 : c.kv_quant ? Datapath::kFp8Cache : Datapath::k16Bit;
+  const bool e4m3 = path == Datapath::kE4m3;
+  const int kv_dtype = path == Datapath::k16Bit ? a.dtype : TFA_FP8_E4M3;
+  const int kv_rows = cache && c.cache.block_table ? c.cache.page_block_size : a.Sk;
+  const int kv_b = cache ? c.cache.num_blocks : a.packed ? 1 : a.B;
   CUtensorMap tq, tk, tv;
+  if ((rc = make_tmap(&tq, a.q, e4m3 ? TFA_FP8_E4M3 : a.dtype, a.D, a.Sq, a.packed ? 1 : a.B, a.Hq, a.qsb, a.qsh, a.qss,
+                      e4m3)))
+    return rc;
+  if ((rc = make_tmap(&tk, a.k, kv_dtype, a.D, kv_rows, kv_b, a.Hkv, a.ksb, a.ksh, a.kss, e4m3))) return rc;
+  if ((rc = make_tmap(&tv, a.v, kv_dtype, a.D, kv_rows, kv_b, a.Hkv, a.ksb, a.ksh, a.kss))) return rc;
+
   FwdParams p{};
-  if ((rc = make_tmap(&tq, a.q, qkv8 ? TFA_FP8_E4M3 : a.dtype, a.D, a.Sq, 1, a.Hq, 0, a.qsh, a.qss, qkv8 != nullptr)))
-    return rc;
-  if ((rc = setup_cache(va, a, va.max_seqlen_q, tk, tv, rp.ap, p, fp8_cache ? TFA_FP8_E4M3 : a.dtype,
-                        qkv8 != nullptr)))
-    return rc;
-  // rotary needs k_new (validate_rotary): every rotary call appends; a quantized q is written even without k_new
-  if (va.k_new || q8) {
-    rp.ap.cu_q = va.cu_seqlens_q;
-    rp.ap.total_q = a.Sq;
-    rc = tfa_internal_launch_append(rp, fp8_cache ? &qs : nullptr, q8 != nullptr, a.D, a.dtype == TFA_BF16,
-                                    ra != nullptr, ra && ra->interleaved != 0, a.stream);
-    if (rc) return rc;
+  if (cache) {
+    setup_cache(c, a, S, kv_rows, rp.ap, p);
+    // rotary needs k_new (validate_rotary): every rotary call appends; a quantized q is written even without k_new
+    if (c.cache.k_new || c.q8) {
+      rc = tfa_internal_launch_append(rp, e4m3 || c.kv_quant ? &qs : nullptr, c.q8 != nullptr, a.D,
+                                      a.dtype == TFA_BF16, c.rotary != nullptr, c.rotary && c.rotary->interleaved != 0,
+                                      a.stream);
+      if (rc) return rc;
+    }
   }
 
-  p.cu_q = va.cu_seqlens_q;
-  p.total_q = a.Sq;
-  p.snew = va.k_new ? 1 : 0;            // a flag: sequence b appends as many keys as it has query rows
-  // as varlen: the grid covers max_seqlen_q rows of every (sequence, head); every split covers the same KV tiles of
-  // every sequence, so a sequence with few keys fills only its first splits
-  if (qkv8) {
-    p.v_scale = qs.v_scale;
-    return run_forward<tfa::kVarlenCacheQkv8>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
+  if (c.keys == Keys::kTensors) {
+    p.Sk = a.Sk;
+    p.causal_off = a.causal ? a.Sk - a.Sq : 0;            // < 0: the first Sq - Sk rows see no key
+    p.keyless_pairs = p.causal_off < 0 ? -p.causal_off / 128 : 0;
+    for (int i = 0; i < c.n_extra; ++i) p.extra_dst[i] = c.extra_dst[i];
+    p.n_extra_dst = c.n_extra;
   }
-  if (quant) {
-    p.v_scale = qs.v_scale;
-    return run_forward<tfa::kVarlenCacheFp8>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
+  if (a.packed) {
+    p.cu_q = c.cu_seqlens_q;
+    p.total_q = a.Sq;
   }
-  return run_forward<tfa::kVarlenCache>(a, p, va.max_seqlen_q, tq, tk, tv, plan);
+  if (c.keys == Keys::kPacked) {
+    p.cu_k = c.cu_seqlens_k;
+    p.total_k = a.Sk;
+  }
+  if (path != Datapath::k16Bit) p.v_scale = qs.v_scale;
+
+  const int problem = cache ? (a.packed ? tfa::kVarlenCache : tfa::kCache) : (a.packed ? tfa::kVarlen : tfa::kDense);
+  switch (forward_mode(problem, path)) {
+    case tfa::kDense: return run_forward<tfa::kDense>(a, p, S, tq, tk, tv, plan);
+    case tfa::kVarlen: return run_forward<tfa::kVarlen>(a, p, S, tq, tk, tv, plan);
+    case tfa::kCache: return run_forward<tfa::kCache>(a, p, S, tq, tk, tv, plan);
+    case tfa::kVarlenCache: return run_forward<tfa::kVarlenCache>(a, p, S, tq, tk, tv, plan);
+    case tfa::kCacheFp8: return run_forward<tfa::kCacheFp8>(a, p, S, tq, tk, tv, plan);
+    case tfa::kVarlenCacheFp8: return run_forward<tfa::kVarlenCacheFp8>(a, p, S, tq, tk, tv, plan);
+    case tfa::kDenseFp8: return run_forward<tfa::kDenseFp8>(a, p, S, tq, tk, tv, plan);
+    case tfa::kVarlenFp8: return run_forward<tfa::kVarlenFp8>(a, p, S, tq, tk, tv, plan);
+    case tfa::kCacheQkv8: return run_forward<tfa::kCacheQkv8>(a, p, S, tq, tk, tv, plan);
+    case tfa::kVarlenCacheQkv8: return run_forward<tfa::kVarlenCacheQkv8>(a, p, S, tq, tk, tv, plan);
+  }
+  return TFA_EINVAL_KVQUANT;                            // an FP8 cache asked of keys that are not a cache
 }
 
 // ---- host-buffer path workspace ----
@@ -824,81 +822,81 @@ int tfa_abi_version(void) { return TFA_ABI_VERSION; }
 
 int tfa_fwd_ex(const tfa_fwd_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return fwd_impl(from_fwd_args(*args), nullptr);
+  return run_call(dense_call(from_fwd_args(*args), nullptr));
 }
 
 int tfa_attn_fwd(const tfa_attn_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return fwd_impl(from_attn_args(*args), nullptr);
+  return run_call(dense_call(from_attn_args(*args), nullptr));
 }
 
 int tfa_attn_varlen_fwd(const tfa_attn_varlen_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return varlen_impl(*args, nullptr);
+  return run_call(varlen_call(*args, nullptr));
 }
 
 int tfa_attn_kvcache_fwd(const tfa_attn_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, nullptr, nullptr);
+  return run_call(kvcache_call(*args, nullptr, nullptr));
 }
 
 int tfa_attn_kvcache_rotary_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary) {
   if (!args || !rotary) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, rotary, nullptr);
+  return run_call(kvcache_call(*args, rotary, nullptr));
 }
 
 int tfa_attn_varlen_kvcache_fwd(const tfa_attn_varlen_kvcache_args* args) {
   if (!args) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, nullptr, nullptr);
+  return run_call(varlen_kvcache_call(*args, nullptr, nullptr));
 }
 
 int tfa_attn_varlen_kvcache_rotary_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
                                        const tfa_kv_quant_args* quant) {
   if (!args || !rotary) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, rotary, quant);
+  return run_call(varlen_kvcache_call(*args, rotary, quant));
 }
 
 int tfa_attn_kvcache_fp8_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary,
                              const tfa_kv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, rotary, quant);
+  return run_call(kvcache_call(*args, rotary, quant));
 }
 
 int tfa_attn_varlen_kvcache_fp8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_kv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, nullptr, quant);
+  return run_call(varlen_kvcache_call(*args, nullptr, quant));
 }
 
 int tfa_attn_fp8_fwd(const tfa_attn_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return fwd_impl(from_attn_args(*args), quant);
+  return run_call(dense_call(from_attn_args(*args), quant));
 }
 
 int tfa_attn_varlen_fp8_fwd(const tfa_attn_varlen_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return varlen_impl(*args, quant);
+  return run_call(varlen_call(*args, quant));
 }
 
 int tfa_attn_kvcache_qkv8_fwd(const tfa_attn_kvcache_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, nullptr, nullptr, quant);
+  return run_call(kvcache_call(*args, nullptr, nullptr, quant));
 }
 
 int tfa_attn_varlen_kvcache_qkv8_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_qkv_quant_args* quant) {
   if (!args || !quant) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, nullptr, nullptr, quant);
+  return run_call(varlen_kvcache_call(*args, nullptr, nullptr, quant));
 }
 
 int tfa_attn_kvcache_qkv8_q16_fwd(const tfa_attn_kvcache_args* args, const tfa_rotary_args* rotary,
                                   const tfa_qkv_quant_args* quant, void* q8) {
   if (!args || !quant || !q8 || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
-  return kvcache_impl(*args, rotary, nullptr, quant, q8);
+  return run_call(kvcache_call(*args, rotary, nullptr, quant, q8));
 }
 
 int tfa_attn_varlen_kvcache_qkv8_q16_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
                                          const tfa_qkv_quant_args* quant, void* q8) {
   if (!args || !quant || !q8 || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, rotary, nullptr, quant, q8);
+  return run_call(varlen_kvcache_call(*args, rotary, nullptr, quant, q8));
 }
 
 int tfa_attn_num_splits(const tfa_attn_args* args) {
@@ -916,14 +914,14 @@ size_t tfa_attn_workspace_bytes(const tfa_attn_args* args, int num_splits) {
 int tfa_attn_varlen_kvcache_split_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
                                       const tfa_kv_quant_args* quant, const tfa_split_args* split) {
   if (!args || !split) return TFA_EINVAL_PTR;
-  return varlen_kvcache_impl(*args, rotary, quant, nullptr, nullptr, split);
+  return run_call(varlen_kvcache_call(*args, rotary, quant, nullptr, nullptr, split));
 }
 
 int tfa_attn_varlen_kvcache_qkv8_split_fwd(const tfa_attn_varlen_kvcache_args* args, const tfa_rotary_args* rotary,
                                            const tfa_qkv_quant_args* quant, void* q8, const tfa_split_args* split) {
   if (!args || !quant || !split || (reinterpret_cast<uintptr_t>(q8) & 15u)) return TFA_EINVAL_PTR;
   if (!q8 && rotary) return TFA_EINVAL_ROTARY;          // an e4m3 q arrives quantized: nothing to rotate
-  return varlen_kvcache_impl(*args, rotary, nullptr, quant, q8, split);
+  return run_call(varlen_kvcache_call(*args, rotary, nullptr, quant, q8, split));
 }
 
 // The dense problem (B, Hq, Sq = max_seqlen_q, Sk = capacity) of a variable-length cache call, for its split count.
@@ -942,7 +940,7 @@ size_t tfa_attn_varlen_kvcache_workspace_bytes(const tfa_attn_varlen_kvcache_arg
 int tfa_fwd_multi(const tfa_fwd_args* args, void* const* extra_out, int n_extra) {
   if (!args) return TFA_EINVAL_PTR;
   if (n_extra < 0) return TFA_EINVAL_SHAPE;
-  return fwd_impl(from_fwd_args(*args), nullptr, extra_out, n_extra);
+  return run_call(dense_call(from_fwd_args(*args), nullptr, extra_out, n_extra));
 }
 
 int tfa_fwd(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int S, int D, int dtype,
@@ -959,7 +957,7 @@ int tfa_fwd(const void* q, const void* k, const void* v, void* out, float* lse, 
   a.softmax_scale = softmax_scale;
   a.out_fp32 = 0;
   a.stream = cuda_stream;
-  return fwd_impl(from_fwd_args(a), nullptr);
+  return run_call(dense_call(from_fwd_args(a), nullptr));
 }
 
 int tfa_fwd_host(const void* q, const void* k, const void* v, void* out, float* lse, int B, int H, int S, int D,
